@@ -1,9 +1,11 @@
 #!/usr/bin/env python
-"""Benchmark of the B200-native centroid-triplet re-ID hot path (driver contract: ONE JSON line).
+"""Benchmark of the H100-native centroid-triplet re-ID hot path (prints ONE JSON line).
 
     python bench.py --gpus N --steps K --warmup W                      (our CUDA path)
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
     python bench.py --impl reference [--workload embed|retrieval|train] (the reference on the host cores)
+    python bench.py ... --dump-outputs DIR   (embed workload: what the last timed step returned, DIR/<name>.npy;
+                                             all-gathered embeddings under torchrun)
 
 Primary metric (BASELINE.json): embeddings/sec @256x128 -- one "step" = one pass of the eval embedding path (trunk ->
 global average pool -> BatchNorm1d, modelling/bases.py:169-177) over one batch of 256 synthetic 256x128 crops per GPU,
@@ -56,11 +58,12 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sust=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     src="measured (MEASURED_PEAKS.json)")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sust=1400.0, src="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense BF16 989 TFLOP/s -- not reached figures
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sust=989.0, src="H100 SXM data sheet (dense BF16, 700 W)")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed regions (B200_PROFILING.md).  The sampler
+    """nvidia-smi clocks / throttle reasons DURING the timed regions.  The sampler
     process is started once (nvidia-smi needs ~0.5 s to come up) and polls every 20 ms; `window()`
     marks the wall-clock intervals of the timed loops and only samples inside them are summarised."""
 
@@ -193,7 +196,7 @@ def run_embed(args, world, rank, local):
     dev = torch.device("cuda", local)
     eng = build_engine(dev)
     gen = torch.Generator(device="cpu").manual_seed(1234 + rank)
-    n_rot = 4  # 4 x 100.7 MB of inputs > 126 MB L2; activations (hundreds of MB per layer) never fit anyway
+    n_rot = 4  # 4 x 100.7 MB of inputs > 50 MB L2; activations (hundreds of MB per layer) never fit anyway
     dev_in = [torch.randn(BATCH, 3, H, W, generator=gen).to(dev) for _ in range(n_rot)]
     graphs = [GraphedForward(eng, d, want_emb=True) for d in dev_in]  # one CUDA graph per rotating input
     steps = args.steps
@@ -218,6 +221,17 @@ def run_embed(args, world, rank, local):
     finish()
     with clk.window():
         ms = timed_steps(step, steps, 0, world, finish)
+    # what the last timed step returned (its graph's static outputs are overwritten by later replays); with several
+    # ranks the caller receives the all-gathered embeddings, [world * BATCH, 2048] in rank order
+    if world > 1:
+        last_out = {"emb": gathered[:, steps - 1].reshape(world * BATCH, 2048).float().cpu().numpy()}
+    else:
+        last_out = {k: v.detach().float().cpu().numpy() for k, v in graphs[(steps - 1) % n_rot].out.items()
+                    if torch.is_tensor(v)}
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for k, v in last_out.items():
+            np.save(os.path.join(args.dump_outputs, f"{k}.npy"), v)
     launches = (graphs[0].launches + 1) * steps
     value = world * BATCH * steps / (ms / 1e3)
 
@@ -331,35 +345,18 @@ def run_embed(args, world, rank, local):
         conv_flops = (GFLOP_PER_IMG - stem_gflop) * 1e9 * BATCH
         pk = peaks()
         ach = conv_flops / (conv_ms * 1e-3) / 1e12
-        traffic = conv_traffic()
-        roof = {"kernel": "conv_gemm_pair / conv_gemm / conv3x3_c64 (48 launches per step: conv + folded BN + shortcut + ReLU)",
+        roof = {"kernel": "conv_gemm / conv3x3_c64 (48 launches per step: conv + folded BN + shortcut + ReLU)",
                 "bound": "tensor", "achieved": ach, "peak": pk["tf_sust"], "unit": "TFLOP/s", "frac": ach / pk["tf_sust"],
                 "frac_of_burst_peak": ach / pk["tf_burst"], "peak_burst": pk["tf_burst"],
-                "peak_source": pk["src"] + ": bf16 sustained (cuBLAS back to back for 4 s, 1000 W cap); the burst figure "
-                                           "(best of 10 short GEMMs) is the like-for-like denominator for a 50 ms timed region",
-                "traffic": traffic, "conv_ms": round(conv_ms, 4), "ms_per_step": round(step_ms, 4),
+                "peak_source": pk["src"],
+                "conv_ms": round(conv_ms, 4), "ms_per_step": round(step_ms, 4),
                 "share_of_step": conv_ms / step_ms,
                 "segments_graph_ms": {k: round(v, 4) for k, v in seg_ms.items()},
                 "method": "CUDA-graph replay of the step and of its three segments (stem | 48 conv launches | GAP+BN); "
                           "conv_ms = step - stem - tail",
-                "whole_step_tflops": GFLOP_PER_IMG * BATCH / step_ms, "hbm_achieved_gbs": (traffic / (conv_ms * 1e-3) / 1e9) if traffic else None,
+                "whole_step_tflops": GFLOP_PER_IMG * BATCH / step_ms,
                 "hbm_peak_gbs": pk["hbm"]}
     return ms, value, launches, e2e, roof, clk.summary()
-
-
-def _json_metric(name, key):
-    path = os.path.join(ROOT, "profiles", name)
-    try:
-        with open(path) as f:
-            return json.load(f)[key]
-    except (OSError, KeyError, ValueError):
-        return None
-
-
-def conv_traffic():
-    """DRAM bytes (read + write) of the conv launches of one bs-256 forward, from the committed ncu metrics
-    pass (profiles/conv_traffic.json, written by tools/launchlist.py on the GPU box); None if absent."""
-    return _json_metric("conv_traffic.json", "dram_bytes_per_step")
 
 
 # ----------------------------------------------------------------------------------------------
@@ -568,10 +565,9 @@ def run_retrieval(args, world, rank, local, steps=None, warmup=None):
                              "eager path, both operands' planes built every step from the freshly uploaded host features"},
         "e2e": {"value": RET_Q * RET_G / dte, "unit": "pairs/s", "h2d_bytes_per_step": (RET_Q + RET_G) * RET_D * 4,
                 "d2h_bytes_per_step": RET_Q * RET_K * 12},
-        "roofline": {"kernel": "dist_gemm_kernel (split-fp16 x3 tcgen05, one pass)", "bound": "tensor",
+        "roofline": {"kernel": "dist_gemm_kernel (split-fp16 x3 wgmma, one pass)", "bound": "tensor",
                      "achieved": ach, "peak": pk["tf_burst"], "unit": "TFLOP/s", "frac": ach / pk["tf_burst"],
                      "peak_source": pk["src"] + ", bf16 burst (a 0.5 ms kernel timed alone)", "pass_ms": pass_ms, "pass2_ms": pass2_ms,
-                     "traffic": _json_metric("dist_traffic.json", "dram_bytes_per_pass"),
                      "tensor_pipe_tflops": 3 * ach,
                      "note": "achieved = algorithmic 2*Q*G*D flop per pass; the fp32-equivalent split issues 3 fp16 "
                              "MMA products per element (tensor_pipe_tflops = 3 x achieved, %.2f of the burst peak)"
@@ -707,7 +703,7 @@ def _best_threads(fn):
 
 
 def _reference():
-    """The reference's own modules (oracle/_ref on the GPU box, /root/reference in the build container) or None."""
+    """The reference's own modules (the vendored copy oracle/_ref, see oracle/vendor_ref.py) or None."""
     from oracle import ref_import  # bench.py's cpu legs are one of the two sanctioned users of oracle/
 
     if not ref_import.reference_available():
@@ -870,7 +866,13 @@ def main():
     ap.add_argument("--train-size", default="256x128", help="HxW of the training crops (config 4: 320x320)")
     ap.add_argument("--train-pk", default="16x16", help="ids x instances per GPU (config 4: 32x4)")
     ap.add_argument("--no-secondary", action="store_true", help="skip the nested metrics and the CPU baselines")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="embed workload only: after the timed steps, write what the last timed step returned as "
+                         "DIR/<name>.npy (float32): emb and global_feat on one GPU; under torchrun (world > 1) rank 0 "
+                         "writes the all-gathered embeddings of all ranks, emb [world*256, 2048]")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "ours" or args.workload != "embed"):
+        raise SystemExit("--dump-outputs is implemented for the embed workload of --impl ours")
     args.warmup = max(args.warmup, 3)
     world, rank, local = dist_env()
 
@@ -907,7 +909,7 @@ def main():
                     "data": "synthetic",
                     "config": {"workload": workload_name, "batch_per_gpu": BATCH, "global_batch": BATCH * world,
                                "model": "resnet50 last_stride=1", "gflop_per_embedding": GFLOP_PER_IMG,
-                               "l2": "4 rotating input batches (403 MB) > 126 MB L2; per-layer activations 67-268 MB",
+                               "l2": "4 rotating input batches (403 MB) > 50 MB L2; per-layer activations 67-268 MB",
                                "parallelism": f"dp{world}: per-rank batches, ONE NCCL all_gather_into_tensor of the "
                                               "extracted embeddings inside the timed region"},
                     "tflops": value * GFLOP_PER_IMG / 1e3, "roofline": roof, "e2e": e2e, "gpu_launches": launches,

@@ -1,4 +1,4 @@
-"""centroids-reid_b200 -- B200-native engine for the centroid-triplet re-ID hot path
+"""centroids-reid_b200 -- H100-native engine for the centroid-triplet re-ID hot path
 (embedding forward -> CTL / center / CE losses -> query x gallery retrieval and CMC / mAP) of
 mikwieczorek/centroids-reid, behind the reference's own module surface:
 
@@ -12,7 +12,7 @@ mikwieczorek/centroids-reid, behind the reference's own module surface:
 
 The directory name carries a hyphen (it is mandated by the build contract), so import it as
 ``importlib.import_module("centroids-reid_b200")`` or through the ``ctl_b200`` alias module
-at the repository root.  All arithmetic runs in hand-written sm_100a CUDA reached through
+at the repository root.  All arithmetic runs in hand-written sm_90a CUDA reached through
 the C ABI of ``libctl_b200.so`` (include/ctl_b200.h); there is no CPU fallback.
 """
 __version__ = "0.1.0"

@@ -2,7 +2,7 @@
 
 The library is built in-tree by ``csrc/build.sh`` (``__graft_entry__.build()``); it is NOT
 optional: there is no CPU or PyTorch fallback behind any compute entry point, and a missing
-library or a non-sm_100 device raises here.
+library or a non-sm_90 device raises here.
 """
 from __future__ import annotations
 
@@ -176,7 +176,7 @@ def require_cuda(*tensors: torch.Tensor):
     for t in tensors:
         if not isinstance(t, torch.Tensor) or not t.is_cuda:
             raise RuntimeError(
-                "centroids-reid_b200 computes on a B200 only: expected CUDA tensors "
+                "centroids-reid_b200 computes on a H100 only: expected CUDA tensors "
                 f"(got {type(t).__name__}{'' if not isinstance(t, torch.Tensor) else ' on ' + str(t.device)})"
             )
     check(lib().ctl_device_check())

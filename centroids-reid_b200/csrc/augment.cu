@@ -8,7 +8,7 @@
 #include <algorithm>
 
 #include "common.h"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace ctl {
 

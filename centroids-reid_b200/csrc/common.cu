@@ -23,7 +23,7 @@ int sm_count() {
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0)
       cached = n;
     else
-      return 148;
+      return 132;  // H100 SXM
   }
   return cached;
 }
@@ -99,8 +99,8 @@ int ctl_device_check(void) {
     cudaGetLastError();
     return CTL_ERR_NO_DEVICE;  // not cached: a device may appear later in the process
   }
-  if (major != 10) {
-    ctl::set_error("device compute capability %d.x is not sm_100 (B200); kernels are built for sm_100a only", major);
+  if (major != 9) {
+    ctl::set_error("device compute capability %d.x is not sm_90 (H100); kernels are built for sm_90a only", major);
     return CTL_ERR_NO_DEVICE;
   }
   cached = 0;

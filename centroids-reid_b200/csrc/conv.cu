@@ -1,5 +1,5 @@
 // Trunk (ResNet50 / ResNet50-IBN-A) inference forward: fused conv + folded-BN (+ residual)
-// (+ ReLU) as implicit GEMM on tcgen05 tensor cores, fed by TMA.
+// (+ ReLU) as implicit GEMM on Hopper tensor cores (wgmma), fed by TMA.
 //
 // Replaces modelling/backbones/resnet.py:51-133, resnet_ibn_a.py:18-141,
 // modelling/baseline.py:91-96 and the eval embedding path modelling/bases.py:169-177 /
@@ -13,8 +13,8 @@
 // 128-row x 128-byte K-major operand tile (SWIZZLE_128B); out-of-bounds coordinates are
 // zero-filled by the TMA unit, which IS the convolution's zero padding.  Stride-2 convolutions
 // read four parity views {h%2, w%2} of the input (strided tensor maps), so every box is still a
-// dense stride-1 box.  Accumulators live in TMEM (double-buffered), the epilogue applies
-// bias / residual / ReLU and writes fp16 NHWC.
+// dense stride-1 box.  Accumulators live in the registers of the two consumer warpgroups
+// (64 pixels each), whose epilogue applies bias / residual / ReLU and writes fp16 NHWC.
 //
 // Roofline: tensor pipe for the 3x3 and wide 1x1 convolutions, HBM for the narrow 1x1s
 // (arithmetic intensity 2*Cin*Cout/(2*(Cin+Cout)) flop/B < 221); algorithmic bytes per conv =
@@ -24,14 +24,19 @@
 #include <algorithm>
 
 #include "common.h"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace ctl {
 
 static constexpr int CBM = 128;  // output pixels per tile
 static constexpr int CBK = 64;   // channels per k-block (128 bytes)
-static constexpr int CONV_THREADS = 320;  // TMA warp, MMA warp, 8 epilogue warps
+// producer warpgroup (one TMA thread) + two consumer warpgroups, each the wgmma issuer and the
+// epilogue of 64 of the tile's 128 pixels
+static constexpr int CONV_THREADS = 384;
 static constexpr int A_TILE_BYTES = CBM * CBK * 2;
+static constexpr int A_HALF_BYTES = A_TILE_BYTES / 2;  // the 64 rows of one consumer warpgroup
+// register split between the warpgroups (setmaxnreg): 128 x 40 + 256 x 232 <= 64 K registers
+static constexpr uint32_t PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 
 struct ConvTap {
   int map;      // which A tensor map (parity view, or the second source of a K-concatenated 1x1)
@@ -62,12 +67,10 @@ struct ConvCfg {
   static constexpr int B_TILE_BYTES = BN * CBK * 2;
   static constexpr int STAGE_BYTES = A_TILE_BYTES + B_TILE_BYTES;
   static constexpr int STAGES = BN == 64 ? 5 : (BN == 128 ? 4 : 3);
-  static constexpr int TMEM_COLS = BN == 64 ? 128 : (BN == 128 ? 256 : 512);  // 2 accumulator stages
   static constexpr int OUT_SLABS = 4;                  // [128 px][64 ch] fp16 staging slabs for the TMA stores
-  static constexpr int IDENT_BYTES = 64 * CBK * 2;     // 64x64 identity operand (residual add on the tensor core)
   static constexpr int BIAS_BYTES = 2048 * 4;          // the layer's whole bias vector (Cout <= 2048), loaded once
-  static constexpr size_t SMEM =
-      (size_t)STAGES * STAGE_BYTES + OUT_SLABS * A_TILE_BYTES + IDENT_BYTES + BIAS_BYTES + 1024 + 256;
+  static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + OUT_SLABS * A_TILE_BYTES + BIAS_BYTES + 1024 + 256;
+  static_assert(SMEM <= 227 * 1024, "conv_gemm_kernel shared memory");
 };
 
 // Tile order: n fastest, then pixel tiles row-major inside an image, then images.  Each CTA owns a
@@ -98,6 +101,38 @@ struct TileIter {
   }
 };
 
+// One 64-channel sub-tile of a consumer warpgroup's accumulator (d = its 32 registers, channels ch0 .. ch0 + 63 of
+// the n-tile) -> (+residual) +bias, ReLU from channel relu_from on -> fp16 -> rows of the swizzled [128 px][64 ch]
+// staging slab.  `res` (may be null) is a [128 px][64 ch] fp16 residual tile in the same swizzled layout, as the TMA
+// unit lands it; it is added before the bias.
+__device__ __forceinline__ void store_subtile_f16(const float* d, uint8_t* slab, int row0, const float* bias, int ch_abs0,
+                                                  int relu, int relu_from, const uint8_t* res = nullptr) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int c = 8 * i + 2 * (lane & 3);
+    const float2 bb = *reinterpret_cast<const float2*>(bias + c);
+    const bool do_relu = relu && ch_abs0 + c >= relu_from;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int px = row0 + (lane >> 2) + 8 * h;
+      const int off = px * 128 + ((i ^ (px & 7)) << 4) + (lane & 3) * 4;
+      float a0 = d[4 * i + 2 * h], a1 = d[4 * i + 2 * h + 1];
+      if (res) {
+        const float2 r = __half22float2(*reinterpret_cast<const __half2*>(res + off));
+        a0 += r.x;
+        a1 += r.y;
+      }
+      float v0 = a0 + bb.x, v1 = a1 + bb.y;
+      if (do_relu) {
+        v0 = fmaxf(v0, 0.f);
+        v1 = fmaxf(v1, 0.f);
+      }
+      *reinterpret_cast<__half2*>(slab + off) = __floats2half2_rn(v0, v1);
+    }
+  }
+}
+
 template <int BN>
 __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid_constant__ ConvKernelParams p) {
   using Cfg = ConvCfg<BN>;
@@ -105,17 +140,13 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t out_stage = smem_base + Cfg::STAGES * Cfg::STAGE_BYTES;
-  const uint32_t ident = out_stage + Cfg::OUT_SLABS * A_TILE_BYTES;
-  const uint32_t bias_sm = ident + Cfg::IDENT_BYTES;
+  const uint32_t bias_sm = out_stage + Cfg::OUT_SLABS * A_TILE_BYTES;
   const uint32_t bar_base = bias_sm + Cfg::BIAS_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (Cfg::STAGES + s); };
-  auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * Cfg::STAGES + s); };
-  auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * Cfg::STAGES + 2 + s); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * Cfg::STAGES + 4);
   uint8_t* gsm = smem_raw + (smem_base - smem_u32(smem_raw));  // generic view of the aligned arena
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5;
   const int num_tiles = p.m_tiles * p.n_tiles;
   const int conv_kblocks = p.k_blocks;
   // contiguous, balanced tile range of this CTA
@@ -126,44 +157,24 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid
   if (threadIdx.x == 0) {
     for (int s = 0; s < Cfg::STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(tfull_bar(s), 1);
-      mbar_init(tempty_bar(s), 8);
+      mbar_init(empty_bar(s), 2);  // one arrive per consumer warpgroup
     }
     fence_barrier_init();
-  }
-  if (warp == 0 && lane == 0) {
     for (int i = 0; i < 4; ++i) tma_prefetch_desc(&p.a_map[i]);
     tma_prefetch_desc(&p.b_map);
     tma_prefetch_desc(&p.out_map);
     tma_prefetch_desc(&p.res_map);
   }
-  if (warp == 1) tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
   for (int i = threadIdx.x; i < p.Cout; i += blockDim.x)
     reinterpret_cast<float*>(gsm + (bias_sm - smem_base))[i] = p.bias[i];
-  {  // 64x64 fp16 identity, K-major, SWIZZLE_128B: row r holds a single 1.0 at k = r
-    uint8_t* id = gsm + (ident - smem_base);
-    for (int i = threadIdx.x; i < Cfg::IDENT_BYTES / 16; i += blockDim.x) reinterpret_cast<uint4*>(id)[i] = make_uint4(0, 0, 0, 0);
-    __syncthreads();
-    if (threadIdx.x < 64) {
-      const int r = threadIdx.x;
-      *reinterpret_cast<__half*>(id + r * 128 + (((r >> 3) ^ (r & 7)) << 4) + (r & 7) * 2) = __float2half(1.f);
-    }
-    fence_proxy_async();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   pdl_launch_dependents();  // the next kernel may begin its prologue
   pdl_wait();               // activations of the previous kernel are complete and visible
-  uint32_t tmem_base;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===================== TMA producer =====================
-    if (lane == 0 && t_begin < t_end) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (threadIdx.x == 0 && t_begin < t_end) {
       int stage = 0;
       uint32_t phase = 0;
       TileIter it;
@@ -185,8 +196,8 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid
           }
         }
         if (p.has_residual) {
-          // the residual rides the same ring: one [128 px][64 ch] slab per 64 output channels,
-          // added to the accumulator by an identity MMA (exact: fp16 x 1.0 into fp32)
+          // the residual rides the same ring: one [128 px][64 ch] slab per 64 output channels, read by
+          // the epilogue of that sub-tile straight from its ring slot
           for (int j = 0; j < NSUB; ++j) {
             mbar_wait(empty_bar(stage), phase ^ 1u);
             mbar_arrive_expect_tx(full_bar(stage), A_TILE_BYTES);
@@ -200,466 +211,76 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_f16(CBM, BN);
-      constexpr uint32_t idesc64 = make_idesc_f16(CBM, 64);
-      const uint64_t d_ident = make_sw128_kmajor_desc(ident);
-      int stage = 0;
-      uint32_t phase = 0;
-      int as = 0;
-      uint32_t aphase = 0;
-      for (int tile = t_begin; tile < t_end; ++tile) {
-        mbar_wait(tempty_bar(as), aphase ^ 1u);
-        tc_fence_after();
-        const uint32_t acc = tmem_base + as * BN;
-        for (int kb = 0; kb < conv_kblocks; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          const uint32_t base = smem_base + stage * Cfg::STAGE_BYTES;
-          const uint64_t da = make_sw128_kmajor_desc(base);
-          const uint64_t db = make_sw128_kmajor_desc(base + A_TILE_BYTES);
-#pragma unroll
-          for (int k = 0; k < CBK / 16; ++k)
-            umma_f16(acc, desc_advance_k(da, k), desc_advance_k(db, k), idesc, (kb > 0 || k > 0) ? 1u : 0u);
-          umma_commit(empty_bar(stage));
-          if (++stage == Cfg::STAGES) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-        if (p.has_residual) {
-          for (int j = 0; j < NSUB; ++j) {
-            mbar_wait(full_bar(stage), phase);
-            tc_fence_after();
-            const uint64_t da = make_sw128_kmajor_desc(smem_base + stage * Cfg::STAGE_BYTES);
-#pragma unroll
-            for (int k = 0; k < CBK / 16; ++k)
-              umma_f16(acc + j * 64, desc_advance_k(da, k), desc_advance_k(d_ident, k), idesc64, 1u);
-            umma_commit(empty_bar(stage));
-            if (++stage == Cfg::STAGES) {
-              stage = 0;
-              phase ^= 1u;
-            }
-          }
-        }
-        umma_commit(tfull_bar(as));
-        if (++as == 2) {
-          as = 0;
-          aphase ^= 1u;
-        }
-      }
-    }
   } else {
-    // ===== epilogue: 8 warps (two per 32-lane TMEM quarter, splitting the columns).  The
-    // accumulator (conv + residual) is drained in 64-channel sub-tiles: TMEM -> registers ->
-    // (+bias, ReLU) -> fp16 -> swizzled staging slab -> one TMA store per sub-tile; four slabs
-    // keep up to three stores in flight.  No global memory access is issued by these warps
-    // except the per-tile bias slice.
-    const int ew = warp - 2;              // 0..7
-    const int et = threadIdx.x - 64;      // 0..255
-    const int quarter = warp & 3;         // TMEM lane quarter this warp may read
-    const int chalf = ew >> 2;            // which 32-channel half of every 64-channel sub-tile
-    const int pix = quarter * 32 + lane;  // pixel inside the tile == TMEM lane == staging row
-    const bool leader = (ew == 0 && lane == 0);
-    const uint32_t row_off = pix * 128;
-    const uint32_t sw = pix & 7;
+    // ===== consumers: warpgroup wg issues the wgmmas of tile rows [64 wg, 64 wg + 64) (M = 64, N = BN) into its
+    // registers, then drains them in 64-channel sub-tiles: (+residual from the ring, +bias, ReLU) -> fp16 -> swizzled
+    // staging slab shared by both warpgroups -> one TMA store per sub-tile; four slabs keep up to three stores in
+    // flight.
+    setmaxnreg_inc<CONSUMER_REGS>();
+    const int wg = (threadIdx.x >> 7) - 1;
+    const bool wg_leader = (threadIdx.x & 127) == 0;
+    const bool leader = threadIdx.x == 128;
+    const int row0 = 64 * wg + 16 * (warp & 3);  // first accumulator row of this warp
     uint8_t* oslabs = gsm + (out_stage - smem_base);
-    float* bias_s = reinterpret_cast<float*>(gsm + (bias_sm - smem_base));
-    int as = 0;
-    uint32_t aphase = 0;
+    const float* bias_s = reinterpret_cast<const float*>(gsm + (bias_sm - smem_base));
+    float acc[BN / 2];
+    int stage = 0;
+    uint32_t phase = 0;
     uint32_t g = 0;  // running sub-tile counter -> staging slab
     TileIter it;
     if (t_begin < t_end) it.init(t_begin, p);
     for (int tile = t_begin; tile < t_end; ++tile, it.next(p)) {
       const int h0 = it.th * p.TH, w0 = it.tw * p.TW;
-      const float* bias_t = bias_s + it.nt * BN;  // whole bias vector staged in the prologue
-      mbar_wait(tfull_bar(as), aphase);
-      tc_fence_after();
-      const uint32_t t0 = tmem_base + as * BN + (static_cast<uint32_t>(quarter * 32) << 16) + chalf * 32;
-#pragma unroll 1
+      int held = -1;  // ring slot still read by the wgmma group in flight
+      for (int kb = 0; kb < conv_kblocks; ++kb) {
+        mbar_wait(full_bar(stage), phase);
+        const uint32_t base = smem_base + stage * Cfg::STAGE_BYTES;
+        const uint64_t da = make_sw128_kmajor_desc(base + wg * A_HALF_BYTES);
+        const uint64_t db = make_sw128_kmajor_desc(base + A_TILE_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < CBK / 16; ++k)
+          wgmma_f16<BN>(acc, desc_advance_k(da, k), desc_advance_k(db, k), (kb > 0 || k > 0) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();  // the previous k-block's group is done reading its slot
+        if (held >= 0 && wg_leader) mbar_arrive(empty_bar(held));
+        held = stage;
+        if (++stage == Cfg::STAGES) {
+          stage = 0;
+          phase ^= 1u;
+        }
+      }
+      wgmma_wait<0>();
+      if (held >= 0 && wg_leader) mbar_arrive(empty_bar(held));
+#pragma unroll
       for (int j = 0; j < NSUB; ++j, ++g) {
         const uint32_t b = g & (Cfg::OUT_SLABS - 1);
-        const int ch0 = j * 64 + chalf * 32;  // first of this thread's 32 channels inside the n-tile
-        uint32_t r[32];
-        tmem_ld16(t0 + j * 64, *reinterpret_cast<uint32_t(*)[16]>(&r[0]));
-        tmem_ld16(t0 + j * 64 + 16, *reinterpret_cast<uint32_t(*)[16]>(&r[16]));
+        const uint8_t* res = nullptr;
+        if (p.has_residual) {  // this sub-tile's residual slab, next in the ring
+          mbar_wait(full_bar(stage), phase);
+          res = gsm + stage * Cfg::STAGE_BYTES;
+        }
         // slab b was handed to a TMA store OUT_SLABS sub-tiles ago: wait until that store has read it
         if (leader) tma_store_wait_read<Cfg::OUT_SLABS - 1>();
-        named_bar_sync(1, 256);  // also publishes this tile's bias slice
-        tmem_ld_wait();
-        if (j == NSUB - 1) {  // last TMEM read of this accumulator stage: hand it back to the MMA warp
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(tempty_bar(as));
-        }
-        uint8_t* oslab = oslabs + b * A_TILE_BYTES + row_off;
-        const bool do_relu = p.relu && (it.nt * BN + ch0) >= p.relu_from;  // relu_from is a multiple of 32
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {  // four 16-byte chunks = 32 channels
-          const float4 b0 = *reinterpret_cast<const float4*>(bias_t + ch0 + c * 8);
-          const float4 b1 = *reinterpret_cast<const float4*>(bias_t + ch0 + c * 8 + 4);
-          float v[8];
-          v[0] = __uint_as_float(r[c * 8 + 0]) + b0.x;
-          v[1] = __uint_as_float(r[c * 8 + 1]) + b0.y;
-          v[2] = __uint_as_float(r[c * 8 + 2]) + b0.z;
-          v[3] = __uint_as_float(r[c * 8 + 3]) + b0.w;
-          v[4] = __uint_as_float(r[c * 8 + 4]) + b1.x;
-          v[5] = __uint_as_float(r[c * 8 + 5]) + b1.y;
-          v[6] = __uint_as_float(r[c * 8 + 6]) + b1.z;
-          v[7] = __uint_as_float(r[c * 8 + 7]) + b1.w;
-          if (do_relu) {
-#pragma unroll
-            for (int q = 0; q < 8; ++q) v[q] = fmaxf(v[q], 0.f);
-          }
-          uint4 o;
-          __half2* po = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-          for (int q = 0; q < 4; ++q) po[q] = __floats2half2_rn(v[2 * q], v[2 * q + 1]);
-          *reinterpret_cast<uint4*>(oslab + (((uint32_t)(chalf * 4 + c) ^ sw) << 4)) = o;
-        }
+        named_bar_sync(1, 256);
+        store_subtile_f16(acc + 32 * j, oslabs + b * A_TILE_BYTES, row0, bias_s + it.nt * BN + j * 64,
+                          it.nt * BN + j * 64, p.relu, p.relu_from, res);
         fence_proxy_async();     // staging writes (generic proxy) -> visible to the TMA store (async proxy)
-        named_bar_sync(1, 256);  // slab complete
-        if (leader) {
-          tma_store_4d(&p.out_map, out_stage + b * A_TILE_BYTES, it.nt * BN + j * 64, w0, h0, it.img);
-          tma_store_commit();
-        }
-      }
-      if (++as == 2) {
-        as = 0;
-        aphase ^= 1u;
-      }
-    }
-    if (leader) tma_store_wait<0>();  // shared memory must outlive the last stores
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
-  }
-}
-
-// ---------------------------------------------------------------------------------------
-// CTA-pair variant (cta_group::2) for the compute-bound wide convolutions.
-//
-// Two CTAs of a cluster own two neighbouring 128-pixel tiles and the SAME 256 output channels.
-// CTA 0 issues one tcgen05.mma.cta_group::2 (M = 256, N = 256) per 16-wide k-step: rows 0-127 of A
-// come from CTA 0's shared memory, rows 128-255 from CTA 1's; each CTA stages only HALF of the weight
-// tile (128 of the 256 output channels).  Per CTA and k-block that is 16 KiB of activations + 16 KiB of
-// weights instead of 16 + 32 KiB: the shared-memory fill rate (~50-60 B/clk/SM measured), not the
-// tensor pipe, is what bounds the single-CTA kernel on these layers.
-// Protocol: both producers credit their TMA bytes to CTA 0's `full` barrier; the leader's commits are
-// multicast to both CTAs' `empty` / `tmem_full` barriers; both epilogues release the accumulator
-// stage on CTA 0's `tmem_empty` barrier.  Each CTA drains its own 128 TMEM lanes.
-// ---------------------------------------------------------------------------------------
-// VAR selects the shared-memory split (the total is the 227 KiB of one SM):
-//   1: non-residual layers -- 5 operand stages (6 for 128-wide tiles) + 2 output staging slabs
-//      (measured 2.5-3 % faster than 4 + 4 on the bs-256 trunk);
-//   2: residual layers     -- 4 (5) operand stages + 5 staging slabs that double as residual landing
-//      buffers: the residual tile is TMA-loaded INTO the staging slab three sub-tiles ahead, the
-//      epilogue adds it in place (ld.shared / add / st.shared on the thread's own 64 bytes) and the
-//      same slab is TMA-stored.  Round 1 added the residual with an identity MMA through the operand
-//      ring, which cost 16 N=64 MMAs per 256x256 tile (25 % of the tensor time of a K=512 layer).
-template <int BN_, int VAR_ = 1>
-struct PairCfg {
-  static constexpr int BN = BN_;                                  // 256 or 128 output channels per pair tile
-  static constexpr bool RES = VAR_ == 2;
-  static constexpr int B_HALF_BYTES = (BN / 2) * CBK * 2;         // this CTA's half of the weight tile: 16 / 8 KiB
-  static constexpr int STAGE_BYTES = A_TILE_BYTES + B_HALF_BYTES;  // 32 / 24 KiB
-  static constexpr int STAGES = (BN == 256 ? 4 : 5) + (RES ? 0 : 1);
-  static constexpr int TMEM_COLS = 2 * BN;                        // two accumulator stages
-  static constexpr int OUT_SLABS = RES ? 5 : 2;
-  static constexpr int RES_AHEAD = 3;                             // residual prefetch distance, sub-tiles
-  static constexpr int BIAS_BYTES = 2048 * 4;  // the layer's whole bias vector, loaded once
-  static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + OUT_SLABS * A_TILE_BYTES + BIAS_BYTES + 1024 + 256;
-};
-
-// pair tile -> (n tile, this CTA's 128-pixel tile); n fastest.  Coordinates advance by carries: one set of
-// integer divisions per role, not per tile.
-struct PairIter {
-  int nt, w_t, h_t, img;
-  __device__ __forceinline__ void init(int tile, const ConvKernelParams& q, int rank_, int per_img) {
-    const int pm = tile / q.n_tiles;
-    nt = tile - pm * q.n_tiles;
-    const int mt = 2 * pm + rank_;
-    img = mt / per_img;
-    const int tr = mt - img * per_img;
-    h_t = tr / q.tiles_w;
-    w_t = tr - h_t * q.tiles_w;
-  }
-  __device__ __forceinline__ void next(const ConvKernelParams& q) {
-    if (++nt < q.n_tiles) return;
-    nt = 0;
-    w_t += 2;  // the pair advances by two 128-pixel tiles
-    while (w_t >= q.tiles_w) {
-      w_t -= q.tiles_w;
-      if (++h_t == q.tiles_h) {
-        h_t = 0;
-        ++img;
-      }
-    }
-  }
-};
-
-template <int BN_T, int VAR_T>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(CONV_THREADS, 1)
-    conv_gemm_pair_kernel(const __grid_constant__ ConvKernelParams p) {
-  using Cfg = PairCfg<BN_T, VAR_T>;
-  constexpr int BN = Cfg::BN;
-  constexpr int NSUB = BN / 64;
-  constexpr int SLABS = Cfg::OUT_SLABS;
-  constexpr int RES_WAIT = Cfg::RES ? SLABS - Cfg::RES_AHEAD - 1 : 0;  // stores that may still be reading their slab
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t out_stage = smem_base + Cfg::STAGES * Cfg::STAGE_BYTES;
-  const uint32_t bias_sm = out_stage + SLABS * A_TILE_BYTES;
-  const uint32_t bar_base = bias_sm + Cfg::BIAS_BYTES;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };                         // used in CTA 0 only
-  auto empty_bar = [&](int s) { return bar_base + 8u * (Cfg::STAGES + s); };         // per CTA
-  auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * Cfg::STAGES + s); };     // per CTA
-  auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * Cfg::STAGES + 2 + s); };  // used in CTA 0 only
-  auto res_bar = [&](int s) { return bar_base + 8u * (2 * Cfg::STAGES + 4 + s); };   // per CTA: residual landed in slab s
-  const uint32_t tmem_slot = bar_base + 8u * (2 * Cfg::STAGES + 4 + SLABS);
-  uint8_t* gsm = smem_raw + (smem_base - smem_u32(smem_raw));
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool is_leader = rank == 0;
-  const int n_clusters = (int)gridDim.x >> 1, cid = (int)blockIdx.x >> 1;
-  const int m_pairs = p.m_tiles >> 1;
-  const int num_tiles = m_pairs * p.n_tiles;  // pair tiles
-  const int conv_kblocks = p.k_blocks;
-  const int per = num_tiles / n_clusters, rem = num_tiles - per * n_clusters;
-  const int t_begin = cid * per + min(cid, rem);
-  const int t_end = t_begin + per + (cid < rem ? 1 : 0);
-  const int tiles_per_img = p.tiles_w * p.tiles_h;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < Cfg::STAGES; ++s) {
-      mbar_init(full_bar(s), 2);   // one arrive per producer of the pair (+ both CTAs' TMA bytes)
-      mbar_init(empty_bar(s), 1);  // leader's multicast commit
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(tfull_bar(s), 1);    // leader's multicast commit
-      mbar_init(tempty_bar(s), 16);  // 8 epilogue warps of each CTA
-    }
-    for (int s = 0; s < SLABS; ++s) mbar_init(res_bar(s), 1);
-    fence_barrier_init();
-  }
-  if (warp == 0 && lane == 0) {
-    for (int i = 0; i < 4; ++i) tma_prefetch_desc(&p.a_map[i]);
-    tma_prefetch_desc(&p.b_map);
-    tma_prefetch_desc(&p.out_map);
-    tma_prefetch_desc(&p.res_map);
-  }
-  if (warp == 1) tmem_alloc2<Cfg::TMEM_COLS>(tmem_slot);
-  for (int i = threadIdx.x; i < p.Cout; i += blockDim.x)
-    reinterpret_cast<float*>(gsm + (bias_sm - smem_base))[i] = p.bias[i];
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();  // barriers of both CTAs initialised before any remote arrive / TMA credit
-  tc_fence_after();
-  pdl_launch_dependents();  // the next kernel may begin its prologue
-  pdl_wait();               // activations of the previous kernel are complete and visible
-  uint32_t tmem_base;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
-
-  if (warp == 0) {
-    // ===================== TMA producer (both CTAs) =====================
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      PairIter it;
-      if (t_begin < t_end) it.init(t_begin, p, (int)rank, tiles_per_img);
-      for (int tile = t_begin; tile < t_end; ++tile, it.next(p)) {
-        const int nt = it.nt, w0 = it.w_t * p.TW, h0 = it.h_t * p.TH, img = it.img;
-        for (int t = 0; t < p.n_taps; ++t) {
-          const ConvTap tap = p.taps[t];
-          for (int cb = 0; cb < tap.cblocks; ++cb) {
-            mbar_wait(empty_bar(stage), phase ^ 1u);
-            const uint32_t dst = smem_base + stage * Cfg::STAGE_BYTES;
-            if (is_leader) mbar_arrive_expect_tx(full_bar(stage), 2 * Cfg::STAGE_BYTES);
-            else mbar_arrive_cta0(full_bar(stage));
-            tma2_load_4d(dst, &p.a_map[tap.map], full_bar(stage), cb * CBK, w0 + tap.dw, h0 + tap.dh, img);
-            tma2_load_2d(dst + A_TILE_BYTES, &p.b_map, full_bar(stage), tap.koff + cb * CBK,
-                         nt * BN + (int)rank * (BN / 2));
-            if (++stage == Cfg::STAGES) {
-              stage = 0;
-              phase ^= 1u;
-            }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA only) =====================
-    if (is_leader && lane == 0) {
-      constexpr uint32_t idesc = make_idesc_f16(256, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int as = 0;
-      uint32_t aphase = 0;
-      for (int tile = t_begin; tile < t_end; ++tile) {
-        mbar_wait(tempty_bar(as), aphase ^ 1u);
-        tc_fence_after();
-        const uint32_t acc = tmem_base + as * BN;
-        for (int kb = 0; kb < conv_kblocks; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          const uint32_t base = smem_base + stage * Cfg::STAGE_BYTES;
-          const uint64_t da = make_sw128_kmajor_desc(base);
-          const uint64_t db = make_sw128_kmajor_desc(base + A_TILE_BYTES);
-#pragma unroll
-          for (int k = 0; k < CBK / 16; ++k)
-            umma2_f16(acc, desc_advance_k(da, k), desc_advance_k(db, k), idesc, (kb > 0 || k > 0) ? 1u : 0u);
-          umma2_commit_mc(empty_bar(stage), 3);
+        named_bar_sync(1, 256);  // slab complete; both warpgroups are done with the residual slot
+        if (p.has_residual) {
+          if (wg_leader) mbar_arrive(empty_bar(stage));
           if (++stage == Cfg::STAGES) {
             stage = 0;
             phase ^= 1u;
           }
         }
-        umma2_commit_mc(tfull_bar(as), 3);
-        if (++as == 2) {
-          as = 0;
-          aphase ^= 1u;
-        }
-      }
-    }
-  } else {
-    // ===================== epilogue (both CTAs, own 128 TMEM lanes) =====================
-    // Per 64-channel sub-tile: TMEM -> registers -> (+bias, +residual from the staging slab, ReLU) -> fp16 ->
-    // swizzled staging slab -> one TMA store.  No global memory access is issued by these warps.
-    const int ew = warp - 2;
-    const int quarter = warp & 3;
-    const int chalf = ew >> 2;
-    const int pix = quarter * 32 + lane;
-    const bool leader_thread = (ew == 0 && lane == 0);
-    const uint32_t row_off = pix * 128;
-    const uint32_t sw = pix & 7;
-    uint8_t* oslabs = gsm + (out_stage - smem_base);
-    float* bias_s = reinterpret_cast<float*>(gsm + (bias_sm - smem_base));
-    const bool with_res = Cfg::RES && p.has_residual;
-    int as = 0;
-    uint32_t aphase = 0;
-    int b = 0;            // staging slab of the current sub-tile
-    uint32_t bphase = 0;  // parity of res_bar(b)
-    // residual prefetch state (leader thread): the sub-tile RES_AHEAD ahead of the one being drained
-    PairIter pit;
-    int ptile = t_begin, pj = 0, pb = 0;
-    auto prefetch_res = [&]() {
-      if (ptile < t_end) {
-        mbar_arrive_expect_tx(res_bar(pb), A_TILE_BYTES);
-        tma_load_4d(out_stage + pb * A_TILE_BYTES, &p.res_map, res_bar(pb), pit.nt * BN + pj * 64, pit.w_t * p.TW,
-                    pit.h_t * p.TH, pit.img);
-        if (++pb == SLABS) pb = 0;
-        if (++pj == NSUB) {
-          pj = 0;
-          ++ptile;
-          pit.next(p);
-        }
-      }
-    };
-    if (with_res && leader_thread && t_begin < t_end) {
-      pit.init(t_begin, p, (int)rank, tiles_per_img);
-      for (int i = 0; i < Cfg::RES_AHEAD; ++i) prefetch_res();
-    }
-    PairIter it;
-    if (t_begin < t_end) it.init(t_begin, p, (int)rank, tiles_per_img);
-    for (int tile = t_begin; tile < t_end; ++tile, it.next(p)) {
-      const int nt = it.nt, w0 = it.w_t * p.TW, h0 = it.h_t * p.TH, img = it.img;
-      const float* bias_t = bias_s + nt * BN;  // whole bias vector staged in the prologue
-      mbar_wait(tfull_bar(as), aphase);
-      tc_fence_after();
-      const uint32_t t0 = tmem_base + as * BN + (static_cast<uint32_t>(quarter * 32) << 16) + chalf * 32;
-#pragma unroll 1
-      for (int j = 0; j < NSUB; ++j) {
-        const int ch0 = j * 64 + chalf * 32;
-        uint32_t r[32];
-        tmem_ld16(t0 + j * 64, *reinterpret_cast<uint32_t(*)[16]>(&r[0]));
-        tmem_ld16(t0 + j * 64 + 16, *reinterpret_cast<uint32_t(*)[16]>(&r[16]));
-        if (with_res) {
-          // the slab RES_AHEAD sub-tiles ahead was stored SLABS - RES_AHEAD sub-tiles ago: once that store has
-          // read it, the next residual tile may land there
-          if (leader_thread) {
-            tma_store_wait_read<RES_WAIT>();
-            prefetch_res();
-          }
-          mbar_wait(res_bar(b), bphase);  // this sub-tile's residual is in slab b (which is therefore free)
-        } else {
-          // slab b was handed to a TMA store SLABS sub-tiles ago: wait until that store has read it
-          if (leader_thread) tma_store_wait_read<SLABS - 1>();
-          named_bar_sync(1, 256);
-        }
-        tmem_ld_wait();
-        if (j == NSUB - 1) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive_cta0(tempty_bar(as));
-        }
-        uint8_t* oslab = oslabs + b * A_TILE_BYTES + row_off;
-        const bool do_relu = p.relu && (nt * BN + ch0) >= p.relu_from;
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          uint4* slot = reinterpret_cast<uint4*>(oslab + (((uint32_t)(chalf * 4 + c) ^ sw) << 4));
-          const float4 b0 = *reinterpret_cast<const float4*>(bias_t + ch0 + c * 8);
-          const float4 b1 = *reinterpret_cast<const float4*>(bias_t + ch0 + c * 8 + 4);
-          float v[8];
-          v[0] = __uint_as_float(r[c * 8 + 0]) + b0.x;
-          v[1] = __uint_as_float(r[c * 8 + 1]) + b0.y;
-          v[2] = __uint_as_float(r[c * 8 + 2]) + b0.z;
-          v[3] = __uint_as_float(r[c * 8 + 3]) + b0.w;
-          v[4] = __uint_as_float(r[c * 8 + 4]) + b1.x;
-          v[5] = __uint_as_float(r[c * 8 + 5]) + b1.y;
-          v[6] = __uint_as_float(r[c * 8 + 6]) + b1.z;
-          v[7] = __uint_as_float(r[c * 8 + 7]) + b1.w;
-          if (with_res) {
-            const uint4 rv = *slot;
-            const __half2* rh = reinterpret_cast<const __half2*>(&rv);
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const float2 f = __half22float2(rh[q]);
-              v[2 * q] += f.x;
-              v[2 * q + 1] += f.y;
-            }
-          }
-          if (do_relu) {
-#pragma unroll
-            for (int q = 0; q < 8; ++q) v[q] = fmaxf(v[q], 0.f);
-          }
-          uint4 o;
-          __half2* po = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-          for (int q = 0; q < 4; ++q) po[q] = __floats2half2_rn(v[2 * q], v[2 * q + 1]);
-          *slot = o;
-        }
-        fence_proxy_async();
-        named_bar_sync(1, 256);
-        if (leader_thread) {
-          tma_store_4d(&p.out_map, out_stage + b * A_TILE_BYTES, nt * BN + j * 64, w0, h0, img);
+        if (leader) {
+          tma_store_4d(&p.out_map, out_stage + b * A_TILE_BYTES, it.nt * BN + j * 64, w0, h0, it.img);
           tma_store_commit();
         }
-        if (++b == SLABS) {
-          b = 0;
-          bphase ^= 1u;
-        }
-      }
-      if (++as == 2) {
-        as = 0;
-        aphase ^= 1u;
       }
     }
-    if (leader_thread) tma_store_wait<0>();
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();  // the peer's shared memory / barriers stay valid until both CTAs are done
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc2<Cfg::TMEM_COLS>(tmem_base);
+    if (leader) tma_store_wait<0>();  // shared memory must outlive the last stores
   }
 }
 
@@ -670,11 +291,11 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(CONV_THREADS, 1)
 // each 16 x 8 output tile loads ONE halo slab -- 18 rows x 16 pixel lines x 128 B, i.e. the 18 x 10
 // halo padded to a 2 KiB row pitch -- by a single TMA box; the nine taps are nine SHIFTED VIEWS of
 // that slab: descriptor start = slab + (r*16 + s)*128 B, 8-row groups 2 KiB apart (one output row
-// each).  MEASURED on B200: the tensor core derives the 128-byte-swizzle XOR from the absolute
-// shared-memory address bits [7,10) -- exactly what the TMA unit used when it wrote the slab -- so
-// a start address shifted by whole 128-byte lines needs NO descriptor base_offset (base_offset = s
-// gives wrong results; tests/test_trunk_gpu.py::test_conv_shapes[case3] pins this).  36 KiB of fill
-// per tile instead of 216 KiB.
+// each).  The 128-byte-swizzle XOR is a function of the absolute shared-memory address bits [7,10)
+// -- exactly what the TMA unit used when it wrote the slab -- so a start address shifted by whole
+// 128-byte lines needs NO descriptor base_offset (tests/test_trunk_gpu.py::test_conv_shapes[case3]
+// pins this).  36 KiB of fill per tile instead of 216 KiB.  Consumer warpgroup wg computes output
+// rows [8 wg, 8 wg + 8) of the tile (M = 64, N = 64).
 // ---------------------------------------------------------------------------------------
 static constexpr int C64_HALO_BYTES = 18 * 16 * 128;  // 36 KiB
 static constexpr int C64_W_BYTES = 9 * 64 * 128;      // 72 KiB
@@ -701,11 +322,8 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv3x3_c64_kernel(const __gr
   const uint32_t w_bar = bar_base;
   auto full_bar = [&](int s) { return bar_base + 8u * (1 + s); };
   auto empty_bar = [&](int s) { return bar_base + 8u * (1 + C64_HALOS + s); };
-  auto tfull_bar = [&](int s) { return bar_base + 8u * (1 + 2 * C64_HALOS + s); };
-  auto tempty_bar = [&](int s) { return bar_base + 8u * (3 + 2 * C64_HALOS + s); };
-  const uint32_t tmem_slot = bar_base + 8u * (5 + 2 * C64_HALOS);
   uint8_t* gsm = smem_raw + (smem_base - smem_u32(smem_raw));
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5;
   const int tiles_per_img = p.tiles_h * p.tiles_w;
   const int num_tiles = p.n_img * tiles_per_img;
   const int per = num_tiles / (int)gridDim.x, rem = num_tiles - per * (int)gridDim.x;
@@ -721,29 +339,21 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv3x3_c64_kernel(const __gr
     mbar_init(w_bar, 1);
     for (int s = 0; s < C64_HALOS; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(tfull_bar(s), 1);
-      mbar_init(tempty_bar(s), 8);
+      mbar_init(empty_bar(s), 2);
     }
     fence_barrier_init();
     tma_prefetch_desc(&p.x_map);
     tma_prefetch_desc(&p.w_map);
     tma_prefetch_desc(&p.out_map);
   }
-  if (warp == 1) tmem_alloc<128>(tmem_slot);
-  if (threadIdx.x >= 64 && threadIdx.x < 128) reinterpret_cast<float*>(gsm + (bias_sm - smem_base))[threadIdx.x - 64] = p.bias[threadIdx.x - 64];
-  tc_fence_before();
+  if (threadIdx.x >= 128 && threadIdx.x < 192) reinterpret_cast<float*>(gsm + (bias_sm - smem_base))[threadIdx.x - 128] = p.bias[threadIdx.x - 128];
   __syncthreads();
-  tc_fence_after();
   pdl_launch_dependents();  // the next kernel may begin its prologue
   pdl_wait();               // activations of the previous kernel are complete and visible
-  uint32_t tmem_base;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (threadIdx.x == 0) {
       mbar_arrive_expect_tx(w_bar, C64_W_BYTES);
       for (int t = 0; t < 9; ++t) tma_load_2d(w_sm + t * 64 * 128, &p.w_map, w_bar, t * 64, 0);
       int stage = 0;
@@ -760,106 +370,52 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv3x3_c64_kernel(const __gr
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_f16(128, 64);
-      mbar_wait(w_bar, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int as = 0;
-      uint32_t aphase = 0;
-      for (int tile = t_begin; tile < t_end; ++tile) {
-        mbar_wait(tempty_bar(as), aphase ^ 1u);
-        mbar_wait(full_bar(stage), phase);
-        tc_fence_after();
-        const uint32_t slab = halo_sm + stage * C64_HALO_BYTES;
-#pragma unroll
-        for (int t = 0; t < 9; ++t) {
-          const int r = t / 3, s = t - 3 * r;
-          const uint32_t a0 = slab + (r * 16 + s) * 128;
-          const uint64_t da = make_sw128_kmajor_desc_ex(a0, 2048, p.use_base_offset ? ((a0 >> 7) & 7u) : 0u);
-          const uint64_t db = make_sw128_kmajor_desc(w_sm + t * 64 * 128);
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_f16(tmem_base + as * 64, desc_advance_k(da, k), desc_advance_k(db, k), idesc, (t | k) ? 1u : 0u);
-        }
-        umma_commit(empty_bar(stage));
-        umma_commit(tfull_bar(as));
-        if (++stage == C64_HALOS) {
-          stage = 0;
-          phase ^= 1u;
-        }
-        if (++as == 2) {
-          as = 0;
-          aphase ^= 1u;
-        }
-      }
-    }
   } else {
-    const int ew = warp - 2;
-    const int quarter = warp & 3;
-    const int chalf = ew >> 2;
-    const int pix = quarter * 32 + lane;  // output pixel (row = pix / 8, col = pix % 8) == TMEM lane
-    const bool leader = (ew == 0 && lane == 0);
-    const uint32_t row_off = pix * 128, sw = pix & 7;
+    setmaxnreg_inc<CONSUMER_REGS>();
+    const int wg = (threadIdx.x >> 7) - 1;
+    const bool leader = threadIdx.x == 128;
+    const int row0 = 64 * wg + 16 * (warp & 3);
     uint8_t* oslabs = gsm + (out_stage - smem_base);
     const float* bias_s = reinterpret_cast<const float*>(gsm + (bias_sm - smem_base));
-    int as = 0;
-    uint32_t aphase = 0, g = 0;
+    mbar_wait(w_bar, 0);
+    float acc[32];
+    int stage = 0;
+    uint32_t phase = 0, g = 0;
     for (int tile = t_begin; tile < t_end; ++tile, ++g) {
       int w0, h0, img;
       coords(tile, w0, h0, img);
-      mbar_wait(tfull_bar(as), aphase);
-      tc_fence_after();
+      mbar_wait(full_bar(stage), phase);
+      const uint32_t slab = halo_sm + stage * C64_HALO_BYTES + wg * 8 * 2048;
+      wgmma_fence();
+#pragma unroll
+      for (int t = 0; t < 9; ++t) {
+        const int r = t / 3, s = t - 3 * r;
+        const uint32_t a0 = slab + (r * 16 + s) * 128;
+        uint64_t da = make_sw128_kmajor_desc(a0, 2048);
+        if (p.use_base_offset) da |= static_cast<uint64_t>((a0 >> 7) & 7u) << 49;
+        const uint64_t db = make_sw128_kmajor_desc(w_sm + t * 64 * 128);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_f16<64>(acc, desc_advance_k(da, k), desc_advance_k(db, k), (t | k) ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      if ((threadIdx.x & 127) == 0) mbar_arrive(empty_bar(stage));
+      if (++stage == C64_HALOS) {
+        stage = 0;
+        phase ^= 1u;
+      }
       const uint32_t b = g & (C64_OUT_SLABS - 1);
-      uint32_t r[32];
-      const uint32_t t0 = tmem_base + as * 64 + (static_cast<uint32_t>(quarter * 32) << 16) + chalf * 32;
-      tmem_ld16(t0, *reinterpret_cast<uint32_t(*)[16]>(&r[0]));
-      tmem_ld16(t0 + 16, *reinterpret_cast<uint32_t(*)[16]>(&r[16]));
       if (leader) tma_store_wait_read<C64_OUT_SLABS - 1>();
       named_bar_sync(1, 256);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(as));
-      uint8_t* oslab = oslabs + b * A_TILE_BYTES + row_off;
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        const float4 b0 = *reinterpret_cast<const float4*>(bias_s + chalf * 32 + c * 8);
-        const float4 b1 = *reinterpret_cast<const float4*>(bias_s + chalf * 32 + c * 8 + 4);
-        float v[8] = {__uint_as_float(r[c * 8 + 0]) + b0.x, __uint_as_float(r[c * 8 + 1]) + b0.y,
-                      __uint_as_float(r[c * 8 + 2]) + b0.z, __uint_as_float(r[c * 8 + 3]) + b0.w,
-                      __uint_as_float(r[c * 8 + 4]) + b1.x, __uint_as_float(r[c * 8 + 5]) + b1.y,
-                      __uint_as_float(r[c * 8 + 6]) + b1.z, __uint_as_float(r[c * 8 + 7]) + b1.w};
-        if (p.relu) {
-#pragma unroll
-          for (int q = 0; q < 8; ++q) v[q] = fmaxf(v[q], 0.f);
-        }
-        uint4 o;
-        __half2* po = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) po[q] = __floats2half2_rn(v[2 * q], v[2 * q + 1]);
-        *reinterpret_cast<uint4*>(oslab + (((uint32_t)(chalf * 4 + c) ^ sw) << 4)) = o;
-      }
+      store_subtile_f16(acc, oslabs + b * A_TILE_BYTES, row0, bias_s, 0, p.relu, 0);
       fence_proxy_async();
       named_bar_sync(1, 256);
       if (leader) {
         tma_store_4d(&p.out_map, out_stage + b * A_TILE_BYTES, 0, w0, h0, img);
         tma_store_commit();
       }
-      if (++as == 2) {
-        as = 0;
-        aphase ^= 1u;
-      }
     }
     if (leader) tma_store_wait<0>();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc<128>(tmem_base);
   }
 }
 
@@ -942,16 +498,16 @@ __global__ void __launch_bounds__(256) stem_conv_kernel(const float* __restrict_
 // Per tile of 4 x 32 output pixels: the fp32 NCHW input patch (13 x 72 x 3) is converted to
 // fp16 in shared memory, every thread then assembles 16-byte K-chunks -- the 8 taps of one
 // (c, r) group are 8 CONSECUTIVE patch columns -- straight into the SWIZZLE_128B operand
-// layout (generic-proxy stores + fence.proxy.async), one thread issues 12 tcgen05.mma
-// (M=128, N=64), and the epilogue adds the folded-BN bias (+ReLU for IBN) and writes one full
-// 128-byte NHWC line per pixel.  Weights [64][192] fp16 stay resident in shared memory.
+// layout (generic-proxy stores + fence.proxy.async), one warpgroup issues 2 x 12 wgmma
+// (M=64, N=64), adds the folded-BN bias (+ReLU for IBN) and writes one full 128-byte NHWC line
+// per pixel.  Weights [64][192] fp16 stay resident in shared memory.
 // ---------------------------------------------------------------------------------------
 static constexpr int SK = 192;                    // padded K
 static constexpr int S_TH = 4, S_TW = 32;         // output tile
 static constexpr int S_PH = 2 * S_TH + 5;         // 13 input rows
 static constexpr int S_PW = 72;                   // 2*32 + 5 = 69 input columns, padded to 72
-static constexpr int STEM_BUILDERS = 256;                   // warps 0-7 assemble operand tiles
-static constexpr int STEM_TC_THREADS = STEM_BUILDERS + 32 + 128;  // + MMA warp (8) + 4 epilogue warps (9-12)
+static constexpr int STEM_BUILDERS = 256;                   // warpgroups 0-1 assemble operand tiles
+static constexpr int STEM_TC_THREADS = STEM_BUILDERS + 128;  // + the MMA / epilogue warpgroup
 static constexpr int S_A_BYTES = 3 * A_TILE_BYTES;          // 48 KiB: three [128][64] fp16 slabs
 static constexpr int S_B_BYTES = 3 * 64 * 128;              // 24 KiB: three [64][64] fp16 slabs
 static constexpr int S_PATCH_BYTES = 3 * S_PH * S_PW * 2;   // 5.6 KiB
@@ -967,11 +523,10 @@ struct StemParams {
   int n_img, H, W, Ho, Wo, tiles_h, tiles_w, relu;
 };
 
-// Persistent, one CTA per SM, three roles connected by mbarriers:
+// Persistent, one CTA per SM, two roles connected by mbarriers:
 //   builders (8 warps): prefetched fp32 patch -> fp16 patch in smem -> swizzled operand tile A[buf]
-//   MMA warp          : 12 tcgen05.mma (M=128, N=64) per tile into TMEM stage `as`
-//   epilogue (4 warps): TMEM -> +bias (+ReLU) -> fp16 -> one 128-byte NHWC line per pixel
-// A, the patch and the accumulator are double-buffered, so all three roles overlap.
+//   MMA warpgroup     : 2 x 12 wgmma (M=64, N=64) per tile -> +bias (+ReLU) -> fp16 -> one TMA store per tile
+// A and the patch are double-buffered, so the builders assemble tile i+1 while tile i is multiplied.
 __global__ void __launch_bounds__(STEM_TC_THREADS, 1) stem_tc_kernel(const __grid_constant__ StemParams p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -983,9 +538,6 @@ __global__ void __launch_bounds__(STEM_TC_THREADS, 1) stem_tc_kernel(const __gri
   const uint32_t bar_w = bars;  // weights landed
   auto a_full = [&](int b) { return bars + 8u * (1 + b); };
   auto a_empty = [&](int b) { return bars + 8u * (3 + b); };
-  auto t_full = [&](int b) { return bars + 8u * (5 + b); };
-  auto t_empty = [&](int b) { return bars + 8u * (7 + b); };
-  const uint32_t tmem_slot = bars + 8u * 9;
   float* bias_s = reinterpret_cast<float*>(gbase + S_FIXED + 2 * S_PATCH_BYTES + 128);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   if (tid < 64) bias_s[tid] = p.bias[tid];
@@ -994,14 +546,11 @@ __global__ void __launch_bounds__(STEM_TC_THREADS, 1) stem_tc_kernel(const __gri
     for (int b = 0; b < 2; ++b) {
       mbar_init(a_full(b), STEM_BUILDERS / 32);  // one arrive per builder warp
       mbar_init(a_empty(b), 1);
-      mbar_init(t_full(b), 1);
-      mbar_init(t_empty(b), 4);
     }
     fence_barrier_init();
     tma_prefetch_desc(&p.w_map);
     tma_prefetch_desc(&p.out_map);
   }
-  if (warp == 8) tmem_alloc<128>(tmem_slot);
   if (tid < STEM_BUILDERS) {
     // the three zero chunks (k = 168..191) of every pixel never change: chunks 5,6,7 of slab 2, both buffers
     for (int q = tid; q < 2 * 128 * 3; q += STEM_BUILDERS) {
@@ -1011,13 +560,9 @@ __global__ void __launch_bounds__(STEM_TC_THREADS, 1) stem_tc_kernel(const __gri
     }
     fence_proxy_async();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   pdl_launch_dependents();  // the next kernel may begin its prologue
   pdl_wait();               // activations of the previous kernel are complete and visible
-  uint32_t tmem_base;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
   const int tiles_per_img = p.tiles_h * p.tiles_w;
   const int num_tiles = p.n_img * tiles_per_img;
 
@@ -1083,77 +628,38 @@ __global__ void __launch_bounds__(STEM_TC_THREADS, 1) stem_tc_kernel(const __gri
         eph ^= 1u;
       }
     }
-  } else if (warp == 8) {
-    if (lane == 0) {
+  } else {
+    const bool leader = tid == STEM_BUILDERS;
+    if (leader) {
       mbar_arrive_expect_tx(bar_w, S_B_BYTES);
       for (int kb = 0; kb < 3; ++kb) tma_load_2d(sB + kb * 64 * 128, &p.w_map, bar_w, kb * 64, 0);
-      mbar_wait(bar_w, 0);
-      constexpr uint32_t idesc = make_idesc_f16(128, 64);
-      int buf = 0;
-      uint32_t ph = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(t_empty(buf), ph ^ 1u);  // accumulator stage drained
-        mbar_wait(a_full(buf), ph);        // operand tile assembled
-        tc_fence_after();
-#pragma unroll
-        for (int kb = 0; kb < 3; ++kb) {
-          const uint64_t da = make_sw128_kmajor_desc(sA + buf * S_A_BYTES + kb * A_TILE_BYTES);
-          const uint64_t db = make_sw128_kmajor_desc(sB + kb * 64 * 128);
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_f16(tmem_base + buf * 64, desc_advance_k(da, k), desc_advance_k(db, k), idesc, (kb | k) ? 1u : 0u);
-        }
-        umma_commit(a_empty(buf));
-        umma_commit(t_full(buf));
-        if (++buf == 2) {
-          buf = 0;
-          ph ^= 1u;
-        }
-      }
     }
-  } else {
-    const int quarter = warp & 3;  // warps 9..12 -> quarters 1,2,3,0
-    const int px = quarter * 32 + lane;
-    const bool leader = (warp == 9 && lane == 0);
+    mbar_wait(bar_w, 0);
+    float acc[2][32];
     int buf = 0;
     uint32_t ph = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int img = tile / tiles_per_img, tr = tile - img * tiles_per_img;
       const int oh0 = (tr / p.tiles_w) * S_TH, ow0 = (tr % p.tiles_w) * S_TW;
-      mbar_wait(t_full(buf), ph);
-      tc_fence_after();
-      uint32_t r[64];
-      const uint32_t t0 = tmem_base + buf * 64 + (static_cast<uint32_t>(quarter * 32) << 16);
-      tmem_ld16(t0, *reinterpret_cast<uint32_t(*)[16]>(&r[0]));
-      tmem_ld16(t0 + 16, *reinterpret_cast<uint32_t(*)[16]>(&r[16]));
-      tmem_ld16(t0 + 32, *reinterpret_cast<uint32_t(*)[16]>(&r[32]));
-      tmem_ld16(t0 + 48, *reinterpret_cast<uint32_t(*)[16]>(&r[48]));
+      mbar_wait(a_full(buf), ph);  // operand tile assembled
+      wgmma_fence();
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int kb = 0; kb < 3; ++kb) {
+          const uint64_t da = make_sw128_kmajor_desc(sA + buf * S_A_BYTES + kb * A_TILE_BYTES + h * A_HALF_BYTES);
+          const uint64_t db = make_sw128_kmajor_desc(sB + kb * 64 * 128);
+#pragma unroll
+          for (int k = 0; k < 4; ++k) wgmma_f16<64>(acc[h], desc_advance_k(da, k), desc_advance_k(db, k), (kb | k) ? 1u : 0u);
+        }
+      wgmma_commit();
+      wgmma_wait<0>();
+      if (leader) mbar_arrive(a_empty(buf));
       if (leader) tma_store_wait_read<1>();  // staging slab `buf` was stored two tiles ago
       named_bar_sync(3, 128);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(t_empty(buf));
-      uint8_t* slab = gbase + 2 * S_A_BYTES + S_B_BYTES + buf * A_TILE_BYTES + px * 128;
+      uint8_t* slab = gbase + 2 * S_A_BYTES + S_B_BYTES + buf * A_TILE_BYTES;
 #pragma unroll
-      for (int c = 0; c < 8; ++c) {
-        uint4 o;
-        __half2* po = reinterpret_cast<__half2*>(&o);
-        const float4 bA = *reinterpret_cast<const float4*>(bias_s + c * 8);
-        const float4 bB = *reinterpret_cast<const float4*>(bias_s + c * 8 + 4);
-        const float bv[8] = {bA.x, bA.y, bA.z, bA.w, bB.x, bB.y, bB.z, bB.w};
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          float a0 = __uint_as_float(r[c * 8 + 2 * q]) + bv[2 * q];
-          float a1 = __uint_as_float(r[c * 8 + 2 * q + 1]) + bv[2 * q + 1];
-          if (p.relu) {
-            a0 = fmaxf(a0, 0.f);
-            a1 = fmaxf(a1, 0.f);
-          }
-          po[q] = __floats2half2_rn(a0, a1);
-        }
-        *reinterpret_cast<uint4*>(slab + ((c ^ (px & 7)) << 4)) = o;
-      }
+      for (int h = 0; h < 2; ++h) store_subtile_f16(acc[h], slab, 64 * h + 16 * (warp & 3), bias_s, 0, p.relu, 0);
       fence_proxy_async();
       named_bar_sync(3, 128);
       if (leader) {
@@ -1167,13 +673,6 @@ __global__ void __launch_bounds__(STEM_TC_THREADS, 1) stem_tc_kernel(const __gri
     }
     if (leader) tma_store_wait<0>();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 8) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc<128>(tmem_base);
-  }
 }
 
 // =======================================================================================
@@ -1181,19 +680,19 @@ __global__ void __launch_bounds__(STEM_TC_THREADS, 1) stem_tc_kernel(const __gri
 //
 // The input is first packed to zero-bordered NHWC4 fp16 (stem_pack_input_kernel: [N][H+6][136][4], 8 bytes per
 // pixel, 3 border pixels left/top).  In that layout the 7-pixel window of output column ox starts 16 bytes after
-// the window of ox-1 (stride 2 x 8 bytes), which is exactly the row pitch of a K-major NO-SWIZZLE UMMA core
+// the window of ox-1 (stride 2 x 8 bytes), which is exactly the row pitch of a K-major NO-SWIZZLE wgmma core
 // matrix (8 rows, 16 bytes apart).  So the im2col operand is never built: shared memory holds raw input rows
 // (cut into 8 overlapping 192-byte pieces of 8 output columns each by one TMA box with overlapping strides) and
 // the A descriptor (LBO = 16 B, SBO = 192 B) walks the windows in place.  Per output-row pair the CTA loads
 // 10 input-row slots (15 KiB) instead of a 56 KiB im2col tile; K = 7 kernel rows x (8 px x 4 ch) = 224.
 // Even/odd input rows sit in separate slot runs so that "+1 slot" = "+2 input rows" = the second output row
-// (rows 64..127 of the M = 128 tile).
+// (rows 64..127 of the M = 128 tile, the second MMA warpgroup).
 //
 // The epilogue writes the conv tile (2 output rows x 64 columns x 64 ch, fp16) to a triple-buffered smem tile and
 // pools it together with the last row of the previous tile; only the pooled tensor goes to HBM.  A CTA walks a
 // contiguous range of row pairs; a range that starts inside an image first recomputes the row pair above it.
 // =======================================================================================
-static constexpr int S3_THREADS = 448;                 // TMA warp, MMA warp, 8 epilogue warps, 4 pool warps
+static constexpr int S3_THREADS = 512;                 // TMA warpgroup, 2 MMA + epilogue warpgroups, 4 pool warps
 static constexpr int S3_STAGES = 4;
 static constexpr int S3_PIECE = 256;                   // bytes: 8 windows (stride 2 px) of 8 px need 176; 256 keeps core matrices 128 B-aligned
 static constexpr int S3_SLOT = 8 * S3_PIECE;           // one input row cut into 8 pieces
@@ -1267,11 +766,8 @@ __global__ void __launch_bounds__(S3_THREADS, 1) stem_pool_kernel(const __grid_c
   const uint32_t bar_w = bars;
   auto full_bar = [&](int s) { return bars + 8u * (1 + s); };
   auto empty_bar = [&](int s) { return bars + 8u * (1 + S3_STAGES + s); };
-  auto tfull_bar = [&](int s) { return bars + 8u * (1 + 2 * S3_STAGES + s); };
-  auto tempty_bar = [&](int s) { return bars + 8u * (3 + 2 * S3_STAGES + s); };
-  auto sfull_bar = [&](int s) { return bars + 8u * (5 + 2 * S3_STAGES + s); };   // conv tile written (8 warps)
-  auto sempty_bar = [&](int s) { return bars + 8u * (8 + 2 * S3_STAGES + s); };  // conv tile no longer needed (4 warps)
-  const uint32_t tmem_slot = bars + 8u * (11 + 2 * S3_STAGES);
+  auto sfull_bar = [&](int s) { return bars + 8u * (1 + 2 * S3_STAGES + s); };   // conv tile written (8 warps)
+  auto sempty_bar = [&](int s) { return bars + 8u * (4 + 2 * S3_STAGES + s); };  // conv tile no longer needed (4 warps)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   if (tid < 64) bias_s[tid] = p.bias[tid];
@@ -1279,11 +775,7 @@ __global__ void __launch_bounds__(S3_THREADS, 1) stem_pool_kernel(const __grid_c
     mbar_init(bar_w, 1);
     for (int s = 0; s < S3_STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(tfull_bar(s), 1);
-      mbar_init(tempty_bar(s), 8);
+      mbar_init(empty_bar(s), 2);  // one arrive per MMA warpgroup
     }
     for (int s = 0; s < 3; ++s) {
       mbar_init(sfull_bar(s), 8);
@@ -1292,14 +784,9 @@ __global__ void __launch_bounds__(S3_THREADS, 1) stem_pool_kernel(const __grid_c
     fence_barrier_init();
     tma_prefetch_desc(&p.x_map);
   }
-  if (warp == 1) tmem_alloc<128>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   pdl_launch_dependents();
   pdl_wait();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
 
   // contiguous, balanced range of row pairs; a range that starts inside an image recomputes the pair above it
   const int num_tiles = p.n_img * p.hp;
@@ -1308,8 +795,8 @@ __global__ void __launch_bounds__(S3_THREADS, 1) stem_pool_kernel(const __grid_c
   const int t_end = t_begin + per + ((int)blockIdx.x < rem ? 1 : 0);
   const int t_first = (t_begin < t_end && (t_begin % p.hp) != 0) ? t_begin - 1 : t_begin;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    if (tid == 0) {
       mbar_arrive_expect_tx(bar_w, S3_W_BYTES);
       bulk_copy_g2s(sW, p.w, S3_W_BYTES, bar_w);
       int stage = 0;
@@ -1327,98 +814,50 @@ __global__ void __launch_bounds__(S3_THREADS, 1) stem_pool_kernel(const __grid_c
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_f16(128, 64);
-      mbar_wait(bar_w, 0);
-      tc_fence_after();
-      int stage = 0, as = 0;
-      uint32_t phase = 0, aphase = 0;
-      for (int t = t_first; t < t_end; ++t) {
-        mbar_wait(tempty_bar(as), aphase ^ 1u);
-        mbar_wait(full_bar(stage), phase);
-        tc_fence_after();
-        const uint32_t a0 = sA + stage * S3_STAGE_BYTES;
-        const uint32_t acc = tmem_base + as * 64;
+  } else if (warp < 12) {
+    // ---- MMA warpgroups: wg computes output row wg of the pair (tile rows [64 wg, 64 wg + 64)), then
+    // +bias (+ReLU) -> fp16 -> conv tile in shared memory (ring of 3) ----
+    const int wg = (tid >> 7) - 1;
+    const int row0 = 64 * wg + 16 * (warp & 3);
+    mbar_wait(bar_w, 0);
+    float acc[32];
+    int stage = 0, buf = 0;
+    uint32_t phase = 0, bphase = 0;
+    for (int t = t_first; t < t_end; ++t) {
+      mbar_wait(full_bar(stage), phase);
+      // output row 1 reads its kernel rows one slot (= two input rows) further
+      const uint32_t a0 = sA + stage * S3_STAGE_BYTES + wg * S3_SLOT;
+      wgmma_fence();
 #pragma unroll
-        for (int r = 0; r < 7; ++r) {
-          // kernel row r of output row 0 = padded input row 4py + r: slot r/2 of the even or odd run; rows 64..127
-          // of the tile (output row 1) land one slot further (SBO * 8 = one slot)
-          const uint32_t arow = a0 + ((r & 1) * 5 + (r >> 1)) * S3_SLOT;
+      for (int r = 0; r < 7; ++r) {
+        // kernel row r of output row 0 = padded input row 4py + r: slot r/2 of the even or odd run
+        const uint32_t arow = a0 + ((r & 1) * 5 + (r >> 1)) * S3_SLOT;
 #pragma unroll
-          for (int kk = 0; kk < 2; ++kk) {
-            const uint64_t da = make_noswizzle_kmajor_desc(arow + 32 * kk, 16, S3_PIECE);
-            const uint64_t db = make_noswizzle_kmajor_desc(sW + (r * 4 + 2 * kk) * 1024, 1024, 128);
-            umma_f16(acc, da, db, idesc, (r > 0 || kk > 0) ? 1u : 0u);
-          }
-        }
-        umma_commit(empty_bar(stage));
-        umma_commit(tfull_bar(as));
-        if (++stage == S3_STAGES) {
-          stage = 0;
-          phase ^= 1u;
-        }
-        if (++as == 2) {
-          as = 0;
-          aphase ^= 1u;
+        for (int kk = 0; kk < 2; ++kk) {
+          const uint64_t da = make_noswizzle_kmajor_desc(arow + 32 * kk, 16, S3_PIECE);
+          const uint64_t db = make_noswizzle_kmajor_desc(sW + (r * 4 + 2 * kk) * 1024, 1024, 128);
+          wgmma_f16<64>(acc, da, db, (r > 0 || kk > 0) ? 1u : 0u);
         }
       }
-    }
-  } else if (warp < 10) {
-    // ---- epilogue warps: TMEM -> +bias (+ReLU) -> fp16 -> conv tile in shared memory (ring of 3) ----
-    const int ew = warp - 2;
-    const int quarter = warp & 3, chalf = ew >> 2;
-    const int px = quarter * 32 + lane;  // tile row: output row px / 64, column px % 64
-    int as = 0, buf = 0;
-    uint32_t aphase = 0, bphase = 0;
-    float bs[32];  // this thread's 32 channels never change: bias lives in registers (no per-tile LDS)
-#pragma unroll
-    for (int j = 0; j < 32; ++j) bs[j] = bias_s[chalf * 32 + j];
-    for (int t = t_first; t < t_end; ++t) {
-      mbar_wait(tfull_bar(as), aphase);
-      tc_fence_after();
-      uint32_t r0[16], r1[16];
-      const uint32_t taddr = tmem_base + as * 64 + chalf * 32 + (static_cast<uint32_t>(quarter * 32) << 16);
-      tmem_ld16(taddr, r0);
-      tmem_ld16(taddr + 16, r1);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(as));
-      uint8_t* tl = tile_g + buf * S3_TILE_BYTES;
-      uint32_t h[16];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        float v0 = __uint_as_float(r0[2 * j]) + bs[2 * j], v1 = __uint_as_float(r0[2 * j + 1]) + bs[2 * j + 1];
-        float v2 = __uint_as_float(r1[2 * j]) + bs[16 + 2 * j], v3 = __uint_as_float(r1[2 * j + 1]) + bs[16 + 2 * j + 1];
-        if (p.relu) {
-          v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); v2 = fmaxf(v2, 0.f); v3 = fmaxf(v3, 0.f);
-        }
-        const __half2 a = __floats2half2_rn(v0, v1), b = __floats2half2_rn(v2, v3);
-        h[j] = *reinterpret_cast<const uint32_t*>(&a);
-        h[8 + j] = *reinterpret_cast<const uint32_t*>(&b);
+      wgmma_commit();
+      wgmma_wait<0>();
+      if ((tid & 127) == 0) mbar_arrive(empty_bar(stage));
+      if (++stage == S3_STAGES) {
+        stage = 0;
+        phase ^= 1u;
       }
       mbar_wait(sempty_bar(buf), bphase ^ 1u);  // the pool warps are done with the tile that lived here
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const int chunk = chalf * 4 + q;
-        *reinterpret_cast<uint4*>(tl + px * 128 + ((chunk ^ (px & 7)) << 4)) =
-            make_uint4(h[4 * q], h[4 * q + 1], h[4 * q + 2], h[4 * q + 3]);
-      }
+      store_subtile_f16(acc, tile_g + buf * S3_TILE_BYTES, row0, bias_s, 0, p.relu, 0);
       __syncwarp();
       if (lane == 0) mbar_arrive(sfull_bar(buf));
       if (++buf == 3) {
         buf = 0;
         bphase ^= 1u;
       }
-      if (++as == 2) {
-        as = 0;
-        aphase ^= 1u;
-      }
     }
   } else {
     // ---- pool warps: 3x3/2 max over the conv tile and the last row of the previous one -> HBM ----
-    const int pt = tid - 320;  // 0..127
+    const int pt = tid - 384;  // 0..127
     int buf = 0;
     uint32_t bphase = 0;
     for (int t = t_first; t < t_end; ++t) {
@@ -1461,13 +900,6 @@ __global__ void __launch_bounds__(S3_THREADS, 1) stem_pool_kernel(const __grid_c
         bphase ^= 1u;
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc<128>(tmem_base);
   }
 }
 
@@ -1651,26 +1083,6 @@ static int launch_c64(const void* x, int n, int h, int w, const void* weight, co
   return 0;
 }
 
-template <int BN, int VAR>
-static int launch_conv_pair_v(const ConvKernelParams& p, cudaStream_t st) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    CTL_CUDA(cudaFuncSetAttribute(conv_gemm_pair_kernel<BN, VAR>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  (int)PairCfg<BN, VAR>::SMEM));
-    attr_set = true;
-  }
-  const long long tiles = (long long)(p.m_tiles / 2) * p.n_tiles;
-  const int clusters = (int)std::min<long long>(tiles, sm_count() / 2);
-  CTL_CUDA(launch_k(conv_gemm_pair_kernel<BN, VAR>, dim3(2 * clusters), dim3(CONV_THREADS), PairCfg<BN, VAR>::SMEM, st, p));
-  CTL_LAUNCH_CHECK();
-  return 0;
-}
-
-template <int BN>
-static int launch_conv_pair(const ConvKernelParams& p, cudaStream_t st) {
-  return p.has_residual ? launch_conv_pair_v<BN, 2>(p, st) : launch_conv_pair_v<BN, 1>(p, st);
-}
-
 // Fills the tile geometry, the output / residual / weight maps and dispatches.  The caller has filled the A maps,
 // the taps and k_blocks; `ktot` = row length of the weight matrix [Cout][ktot].
 static int finish_and_launch(ConvKernelParams& p, int n, int Ho, int Wo, int cout, int ktot, const void* weight,
@@ -1699,17 +1111,12 @@ static int finish_and_launch(ConvKernelParams& p, int n, int Ho, int Wo, int cou
                                 ostr, obox, CU_TENSOR_MAP_SWIZZLE_128B)))
       return rc;
   }
-  // CTA pairs for every 256- / 128-channel-tile layer with an even tile count; CTL_CONV_PAIR=0 forces the single-CTA
-  // kernel (A/B runs)
-  static const int pair_mode = [] { const char* e = getenv("CTL_CONV_PAIR"); return e ? atoi(e) : -1; }();
-  const bool use_pair = (BN == 256 || BN == 128) && (p.m_tiles % 2 == 0) && p.m_tiles >= 2 && pair_mode != 0;
   const uint64_t bdims[2] = {(uint64_t)ktot, (uint64_t)cout};
   const uint64_t bstr[2] = {2, (uint64_t)ktot * 2};
-  const uint32_t bbox[2] = {CBK, (uint32_t)(use_pair ? BN / 2 : BN)};  // a pair CTA stages half of the weight tile
+  const uint32_t bbox[2] = {CBK, (uint32_t)BN};
   if ((rc = encode_tensor_map(&p.b_map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 2, weight, bdims, bstr, bbox,
                               CU_TENSOR_MAP_SWIZZLE_128B)))
     return rc;
-  if (use_pair) return BN == 256 ? launch_conv_pair<256>(p, st) : launch_conv_pair<128>(p, st);
   if (BN == 256) return launch_conv<256>(p, st);
   if (BN == 128) return launch_conv<128>(p, st);
   return launch_conv<64>(p, st);

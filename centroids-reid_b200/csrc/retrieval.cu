@@ -1,19 +1,21 @@
-// Query x gallery distances on 5th-gen tensor cores with streamed top-k / CMC / mAP epilogues.
+// Query x gallery distances on Hopper tensor cores (wgmma) with streamed top-k / CMC / mAP epilogues.
 //
 // Replaces utils/reid_metric.py:25-33,51-59,112-136, utils/eval_reid.py:25-92 and
 // inference/get_similar.py:104-128 of the reference (see include/ctl_b200.h).
 //
 // Arithmetic.  The reference computes q.g in fp32.  Here every fp32 row x is split exactly as
 //     x * s = hi + 2^-11 * lo        (s: per-row power of two, hi/lo: fp16)
-// and q.g = (hi_q.hi_g + 2^-11 (hi_q.lo_g + lo_q.hi_g)) / (s_q s_g): three fp16 tcgen05.mma
-// passes with fp32 accumulation into TWO TMEM accumulators (the 2^-11 terms never get swamped
+// and q.g = (hi_q.hi_g + 2^-11 (hi_q.lo_g + lo_q.hi_g)) / (s_q s_g): three fp16 wgmma
+// passes with fp32 accumulation into TWO register accumulators (the 2^-11 terms never get swamped
 // by the leading term).  Dropped: 2^-22 lo.lo -- i.e. >= 22 significant bits per product,
 // fp32-equivalent, and EXACT whenever the operands have <= 11 significant bits (the
 // dyadic-grid fixtures on which rank parity is asserted bit-exact).
 //
-// One persistent CTA per SM, 6 warps: TMA producer / MMA issuer / 4 epilogue warps; 3-stage
-// smem ring of {q_hi, q_lo, g_hi, g_lo} 128x64 fp16 tiles (SWIZZLE_128B), double-buffered TMEM
-// accumulators (2 x (128 + 128) columns) so the epilogue of tile i overlaps the MMAs of i+1.
+// One persistent CTA per SM, 3 warpgroups: a TMA producer and two consumers; 2-stage smem ring of
+// {q_hi, q_lo, g_hi, g_lo} 128x64 fp16 tiles (SWIZZLE_128B).  Consumer warpgroup wg multiplies
+// query rows [64 wg, 64 wg + 64) of the tile (two m64n128 accumulators in registers), folds them
+// into one fp32 dot product per element, stages its rows in shared memory and runs the epilogue
+// on them, one thread per (query row, 64-column half); the producer fills the ring meanwhile.
 #include <limits.h>
 #include <math_constants.h>
 #include <math.h>
@@ -23,17 +25,19 @@
 #include <algorithm>
 
 #include "common.h"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace ctl {
 
-static constexpr int BM = 128;      // queries per tile (TMEM lanes)
-static constexpr int BN = 128;      // gallery rows per tile (TMEM columns per accumulator)
+static constexpr int BM = 128;      // queries per tile (2 consumer warpgroups x 64 rows)
+static constexpr int BN = 128;      // gallery rows per tile
 static constexpr int BK = 64;       // fp16 elements per k-block = one 128-byte swizzle row
-static constexpr int STAGES = 3;
+static constexpr int STAGES = 2;
 static constexpr int TILE_BYTES = BM * BK * 2;          // 16 KiB
 static constexpr int STAGE_BYTES = 4 * TILE_BYTES;      // q_hi, q_lo, g_hi, g_lo
-static constexpr int GEMM_THREADS = 320;  // TMA warp, MMA warp, 8 epilogue warps
+static constexpr int GEMM_THREADS = 384;  // producer warpgroup + 2 consumer warpgroups
+static constexpr uint32_t GEMM_PRODUCER_REGS = 40, GEMM_CONSUMER_REGS = 232;
+static constexpr int ACC_BYTES = BM * BN * 4;  // the tile's fp32 dot products, one 512-byte row per query
 static constexpr int GROUP_W = 16;                      // columns per group-min
 static constexpr int META_BYTES = 2 * BN * (4 + 4 + 4 + 8 + 4);  // double-buffered per-tile column metadata
 static constexpr int THR_MAX = 32, THR_STRIDE = 36;         // positives per query held in shared memory (16-byte rows)
@@ -41,9 +45,9 @@ static constexpr int THR_BYTES = BM * THR_STRIDE * 4;
 static constexpr int CNT_STRIDE = THR_MAX / 2 + 1;          // bucket counters of one query row: 2 x 16 bit per word
 static constexpr int CNT_BYTES = BM * CNT_STRIDE * 4;
 static constexpr int FAR_LEVELS = 1;  // buckets of the count pass resolved by plain compares against the farthest positives
-                                      // (measured on config 3: 1 level 0.514 ms, 3 levels 0.531 ms, none 0.568 ms per pass)
+                                      // (config 3 retrieval step on one H100: none 5.57 ms, 1 level 5.51 ms, 2 levels 5.79 ms)
 static constexpr int UNIT_R = 4;  // count passes: gallery tiles a CTA runs back to back for ONE query tile
-static constexpr size_t GEMM_SMEM = STAGES * STAGE_BYTES + META_BYTES + THR_BYTES + CNT_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+static constexpr size_t GEMM_SMEM = STAGES * STAGE_BYTES + ACC_BYTES + META_BYTES + THR_BYTES + CNT_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 static_assert(GEMM_SMEM <= 227 * 1024, "dist_gemm_kernel shared memory");
 static_assert(UNIT_R * BN < 65536, "16-bit bucket counters of a unit");
 
@@ -209,8 +213,8 @@ struct GemmMaps {
   CUtensorMap q_hi, q_lo, g_hi, g_lo;
 };
 
-// The ONE place a distance is formed from the accumulators: every pass must produce
-// bit-identical values for the same (query, gallery) pair.
+// The ONE place a distance is formed from the accumulators (dot_from_acc, then dist_from_dot): every
+// pass must produce bit-identical values for the same (query, gallery) pair.
 // d[j] for a runtime j without spilling the array to local memory: a 4-level select tree (15 FSEL)
 __device__ __forceinline__ float select16(const float (&d)[16], int j) {
   float a[8], b[4], c[2];
@@ -223,9 +227,10 @@ __device__ __forceinline__ float select16(const float (&d)[16], int j) {
   return (j & 8) ? c[1] : c[0];
 }
 
-__device__ __forceinline__ float dist_from_acc(float acc0, float acc1, float q_is, float g_is, float qq, float gg,
-                                               int cosine) {
-  float dot = __fmaf_rn(acc1, 4.8828125e-4f /* 2^-11 */, acc0);
+__device__ __forceinline__ float dot_from_acc(float acc0, float acc1) {
+  return __fmaf_rn(acc1, 4.8828125e-4f /* 2^-11 */, acc0);
+}
+__device__ __forceinline__ float dist_from_dot(float dot, float q_is, float g_is, float qq, float gg, int cosine) {
   dot = __fmul_rn(__fmul_rn(dot, q_is), g_is);
   if (cosine & 1) return fmaxf(fabsf(__fsub_rn(1.f, dot)), 1e-12f);
   const float sqd = __fmaf_rn(-2.f, dot, __fadd_rn(qq, gg));
@@ -264,19 +269,24 @@ __device__ __forceinline__ void unit_coords(const GemmPass& p, int w, int& mt, i
   }
 }
 
+// Shared-memory word of element (row, col) of the staged dot-product tile: 16-byte chunks of a row XOR-swizzled by
+// (2 row + chunk / 16) & 7, so neither the accumulator stores nor the epilogue's row reads conflict on a bank.
+__device__ __forceinline__ int acc_word(int row, int col) {
+  const int chunk = col >> 2;
+  return row * BN + ((chunk ^ ((2 * row + (chunk >> 4)) & 7)) << 2) + (col & 3);
+}
+
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
     dist_gemm_kernel(const __grid_constant__ GemmMaps maps, const GemmPass p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t meta_base = smem_base + STAGES * STAGE_BYTES;
+  const uint32_t acc_base = smem_base + STAGES * STAGE_BYTES;
+  const uint32_t meta_base = acc_base + ACC_BYTES;
   const uint32_t thr_base = meta_base + META_BYTES;
   const uint32_t bar_base = thr_base + THR_BYTES + CNT_BYTES;
-  // barriers: full[STAGES], empty[STAGES], tmem_full[2], tmem_empty[2], tmem ptr
+  // barriers: full[STAGES], empty[STAGES]
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + s); };
-  auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + 2 + s); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 4);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -287,30 +297,20 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(tfull_bar(s), 1);
-      mbar_init(tempty_bar(s), 8);
+      mbar_init(empty_bar(s), 2);  // one arrive per consumer warpgroup
     }
     fence_barrier_init();
-  }
-  if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&maps.q_hi);
     tma_prefetch_desc(&maps.q_lo);
     tma_prefetch_desc(&maps.g_hi);
     tma_prefetch_desc(&maps.g_lo);
   }
-  if (warp == 1) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    setmaxnreg_dec<GEMM_PRODUCER_REGS>();
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
@@ -332,69 +332,28 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
           }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_f16(BM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int as = 0;
-      uint32_t aphase = 0;
-      for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
-        int mt, nt0, ncnt;
-        unit_coords(p, w, mt, nt0, ncnt);
-        for (int t = 0; t < ncnt; ++t) {
-        mbar_wait(tempty_bar(as), aphase ^ 1u);
-        tc_fence_after();
-        const uint32_t acc0 = tmem_base + as * 256;
-        const uint32_t acc1 = acc0 + 128;
-        for (int kb = 0; kb < k_blocks; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          const uint32_t base = smem_base + stage * STAGE_BYTES;
-          const uint64_t d_qh = make_sw128_kmajor_desc(base + 0 * TILE_BYTES);
-          const uint64_t d_ql = make_sw128_kmajor_desc(base + 1 * TILE_BYTES);
-          const uint64_t d_gh = make_sw128_kmajor_desc(base + 2 * TILE_BYTES);
-          const uint64_t d_gl = make_sw128_kmajor_desc(base + 3 * TILE_BYTES);
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint32_t acc = (kb > 0 || k > 0) ? 1u : 0u;
-            umma_f16(acc0, desc_advance_k(d_qh, k), desc_advance_k(d_gh, k), idesc, acc);
-            umma_f16(acc1, desc_advance_k(d_qh, k), desc_advance_k(d_gl, k), idesc, acc);
-            umma_f16(acc1, desc_advance_k(d_ql, k), desc_advance_k(d_gh, k), idesc, 1u);
-          }
-          umma_commit(empty_bar(stage));  // smem slot free once these MMAs have read it
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-        umma_commit(tfull_bar(as));  // accumulators complete
-        if (++as == 2) {
-          as = 0;
-          aphase ^= 1u;
-        }
-        }
-      }
-    }
   } else {
-    // ===================== epilogue: 8 warps, two per 32-lane TMEM quarter (64 columns each) =====
+    // ===================== consumers: MMA + epilogue, one thread per (query row, 64-column half) =====
     // Per-tile column metadata (|g|^2, 1/scale, pid, camera mask of the 128 gallery rows) is staged
     // once in shared memory; every thread then reads it by broadcast instead of 4 global loads per
     // element.
-    const int ew = warp - 2;
-    const int et = threadIdx.x - 64;  // 0..255
-    const int quarter = warp & 3;
-    const int chalf = ew >> 2;        // columns [64*chalf, 64*chalf + 64) of the tile
-    const int row_in_tile = quarter * 32 + lane;
+    setmaxnreg_inc<GEMM_CONSUMER_REGS>();
+    const int wg = (threadIdx.x >> 7) - 1;
+    const bool wg_leader = (threadIdx.x & 127) == 0;
+    const int wrow0 = 64 * wg + 16 * (warp & 3);  // first of the 16 tile rows this warp multiplies and drains
+    float* acc_s = reinterpret_cast<float*>(smem_raw + (acc_base - smem_u32(smem_raw)));
+    int stage = 0;
+    uint32_t phase = 0;
+    const int ew = warp - 4;          // 0..7
+    const int et = threadIdx.x - 128;  // 0..255
+    const int chalf = lane & 1;       // columns [64*chalf, 64*chalf + 64) of the tile
+    const int row_in_tile = wrow0 + (lane >> 1);
     float* cm_sq = reinterpret_cast<float*>(smem_raw + (meta_base - smem_u32(smem_raw)));  // [2][128]
     float* cm_is = cm_sq + 2 * BN;
     int* cm_pid = reinterpret_cast<int*>(cm_is + 2 * BN);
     unsigned long long* cm_mask = reinterpret_cast<unsigned long long*>(cm_pid + 2 * BN);
     unsigned int* cm_idx = reinterpret_cast<unsigned int*>(cm_mask + 2 * BN);  // index written into the keys
     uint32_t* thr_s = reinterpret_cast<uint32_t*>(smem_raw + (thr_base - smem_u32(smem_raw)));
-    int as = 0;
-    uint32_t aphase = 0;
     int it = 0;
     long long pc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     long long tprev = clock64();
@@ -482,18 +441,59 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
       }
       const int nps = min(npos, THR_MAX);
       CTL_STAMP(0)
-      mbar_wait(tfull_bar(as), aphase);
-      tc_fence_after();
+      {
+        // acc0 = q_hi.g_hi, acc1 = q_hi.g_lo + q_lo.g_hi over this warpgroup's 64 query rows x 128 gallery rows
+        float acc0[BN / 2], acc1[BN / 2];
+        int held = -1;  // ring slot still read by the wgmma group in flight
+        for (int kb = 0; kb < k_blocks; ++kb) {
+          mbar_wait(full_bar(stage), phase);
+          const uint32_t base = smem_base + stage * STAGE_BYTES;
+          const uint64_t d_qh = make_sw128_kmajor_desc(base + 0 * TILE_BYTES + wg * (TILE_BYTES / 2));
+          const uint64_t d_ql = make_sw128_kmajor_desc(base + 1 * TILE_BYTES + wg * (TILE_BYTES / 2));
+          const uint64_t d_gh = make_sw128_kmajor_desc(base + 2 * TILE_BYTES);
+          const uint64_t d_gl = make_sw128_kmajor_desc(base + 3 * TILE_BYTES);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < BK / 16; ++k) {
+            const uint32_t acc = (kb > 0 || k > 0) ? 1u : 0u;
+            wgmma_f16<BN>(acc0, desc_advance_k(d_qh, k), desc_advance_k(d_gh, k), acc);
+            wgmma_f16<BN>(acc1, desc_advance_k(d_qh, k), desc_advance_k(d_gl, k), acc);
+            wgmma_f16<BN>(acc1, desc_advance_k(d_ql, k), desc_advance_k(d_gh, k), 1u);
+          }
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (held >= 0 && wg_leader) mbar_arrive(empty_bar(held));
+          held = stage;
+          if (++stage == STAGES) {
+            stage = 0;
+            phase ^= 1u;
+          }
+        }
+        wgmma_wait<0>();
+        if (held >= 0 && wg_leader) mbar_arrive(empty_bar(held));
+        // this warp's 16 rows -> shared memory (only this warp reads them back)
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int r = wrow0 + (lane >> 2) + 8 * h, col = 8 * j + 2 * (lane & 3);
+            *reinterpret_cast<float2*>(acc_s + acc_word(r, col)) =
+                make_float2(dot_from_acc(acc0[4 * j + 2 * h], acc1[4 * j + 2 * h]),
+                            dot_from_acc(acc0[4 * j + 2 * h + 1], acc1[4 * j + 2 * h + 1]));
+          }
+        __syncwarp();
+      }
       CTL_STAMP(1)
       named_bar_sync(1, 256);  // metadata slice published
       CTL_STAMP(2)
-      const uint32_t t0 = tmem_base + as * 256 + (static_cast<uint32_t>(quarter * 32) << 16) + chalf * 64;
 #pragma unroll 1
       for (int c = 0; c < 4; ++c) {
-        uint32_t r0[16], r1[16];
-        tmem_ld16(t0 + c * 16, r0);
-        tmem_ld16(t0 + 128 + c * 16, r1);
-        tmem_ld_wait();
+        float r0[16];
+#pragma unroll
+        for (int q4 = 0; q4 < 4; ++q4) {
+          const float4 v = *reinterpret_cast<const float4*>(acc_s + acc_word(row_in_tile, chalf * 64 + c * 16 + 4 * q4));
+          r0[4 * q4] = v.x; r0[4 * q4 + 1] = v.y; r0[4 * q4 + 2] = v.z; r0[4 * q4 + 3] = v.w;
+        }
         CTL_STAMP(3)
         const int cl0 = chalf * 64 + c * 16;  // column inside the tile
         const int col0 = nt * BN + cl0;
@@ -516,7 +516,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
           }
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
-            dist[j] = dist_from_acc(__uint_as_float(r0[j]), __uint_as_float(r1[j]), qis, gis[j], qq, gsq[j], p.cosine);
+            dist[j] = dist_from_dot(r0[j], qis, gis[j], qq, gsq[j], p.cosine);
             const bool ok = row_ok && (col0 + j < p.ng);
             m_valid |= (ok ? 1u : 0u) << j;
             gmin = fminf(gmin, ok ? dist[j] : CUDART_INF_F);
@@ -605,8 +605,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
                 exact = lo > 0 && thr_row[lo - 1] == kd;
               }
               if (exact) lo_i = bucket_search_global(p.thr_keys + (size_t)row * p.max_pos, npos, key);
-              // buckets below THR_MAX: 16-bit counters of this row in shared memory (flushed once per work item) --
-              // round 2 measured the count pass epilogue-bound on ~27 M global REDs per pass (wait_acc 30 k of 850 k clk)
+              // buckets below THR_MAX: 16-bit counters of this row in shared memory (flushed once per work item) instead
+              // of one global RED per counted row (tens of millions per pass at config 3)
               if (lo_i < THR_MAX) atomicAdd(cnt_row + (lo_i >> 1), 1u << ((lo_i & 1) * 16));
               else atomicAdd(p.buckets + (size_t)row * (p.max_pos + 1) + lo_i, 1);
             }
@@ -615,18 +615,12 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
         if (p.gmin && row_ok && col0 < p.ng) p.gmin[(size_t)row * p.n_groups + (col0 >> 4)] = gmin;
         CTL_STAMP(4)
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(as));
+      __syncwarp();  // this warp's staged rows are read: the next tile may overwrite them
       CTL_STAMP(5)
-      if (++as == 2) {
-        as = 0;
-        aphase ^= 1u;
-      }
       }  // gallery tiles of the work item
       if (thr_in_smem) {
         named_bar_sync(2, 256);  // every warp is done with this work item's thresholds and counters
-        // flush: the two warps of a row quarter take alternate counter words of the row and leave them zero.  The next
+        // flush: the two threads of a row take alternate counter words of the row and leave them zero.  The next
         // work item's first metadata barrier orders these writes (and the new thresholds) before any use.
         if (row_ok) {
           int* dst = p.buckets + (size_t)row * (p.max_pos + 1);
@@ -642,21 +636,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
         CTL_STAMP(6)
       }
     }
-    if (p.prof && (threadIdx.x == 64 || threadIdx.x == 64 + 5 * 32 + 7)) {
-      long long* dst = p.prof + ((size_t)blockIdx.x * 2 + (threadIdx.x == 64 ? 0 : 1)) * 8;
+    if (p.prof && (threadIdx.x == 128 || threadIdx.x == 128 + 5 * 32 + 7)) {
+      long long* dst = p.prof + ((size_t)blockIdx.x * 2 + (threadIdx.x == 128 ? 0 : 1)) * 8;
       for (int i = 0; i < 8; ++i) dst[i] = pc[i];
     }
 #undef CTL_STAMP
-  }
-  if (p.prof && warp == 2 && lane == 0) {
-    // (registers of the epilogue leader; other roles write nothing)
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
   }
 }
 
@@ -686,8 +670,7 @@ __device__ __forceinline__ void bitonic_sort_smem(T* s, int n_pow2) {
 // tau[q] = k-th smallest of the (merged) group minima: an upper bound of the k-th smallest
 // distance, with at most merge*GROUP_W*(k-1) rows strictly below it.
 // Radix select on the order-preserving uint32 keys (4 passes of 8 bits, shared-memory histogram + warp scan): the k-th
-// smallest needs no sort -- round 1 sorted all n_merged keys with a bitonic network (55 block-wide stages for 1024 keys,
-// 128 us for 3368 queries; this form: ~20 us).
+// smallest needs no sort (a bitonic network over all n_merged keys takes 55 block-wide stages for 1024 keys).
 __global__ void __launch_bounds__(256) select_tau_kernel(const float* __restrict__ gmin, int n_groups, int merge, int k,
                                                          int n_pow2, float* __restrict__ tau) {
   extern __shared__ uint32_t skeys[];
@@ -910,7 +893,7 @@ static int launch_gemm_pass(const void* q_planes, int64_t nq, const void* g_plan
   }
   static const int unit_r_env = [] {
     const char* e = getenv("CTL_DIST_UNIT_R");  // experiments: gallery tiles per work item of the count pass
-    const int v = e ? atoi(e) : 1;  // measured (round 2): no gain from longer items once the thresholds are staged cheaply
+    const int v = e ? atoi(e) : 1;  // config 3 step on one H100: 5.51 ms (1), 5.50 ms (2), 5.74 ms (4) -- no gain
     return v >= 1 && v <= UNIT_R ? v : UNIT_R;
   }();
   p.unit_r = p.buckets ? unit_r_env : 1;

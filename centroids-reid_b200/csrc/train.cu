@@ -1,10 +1,10 @@
 // Training-side kernels of the trunk (reference: autograd through modelling/backbones/resnet.py:67-87,122-133
 // in train mode -- torch.nn.Conv2d weight gradients, BatchNorm2d batch statistics and their backward).
 //
-// 1. conv2d weight gradient as a tcgen05 GEMM over the pixel dimension:
+// 1. conv2d weight gradient as a wgmma GEMM over the pixel dimension:
 //      dW[co][tap][ci] = sum_pixels dy[pixel][co] * x[pixel + tap][ci]
 //    Both operands are the SAME TMA boxes the forward uses ([128 pixels][64 channels], 128-byte rows,
-//    SWIZZLE_128B) -- read by the tensor core as MN-major operands (instruction-descriptor bits 15/16):
+//    SWIZZLE_128B) -- read by the tensor core as MN-major (transposed) operands:
 //    rows are the K (pixel) dimension, the 64 channels of a row the M / N dimension.  The reduction is long
 //    (N*Ho*Wo pixels) and the output small, so the pixel range is split across CTAs; fp32 partial tiles are
 //    reduced in a fixed order by a second kernel (deterministic, no atomics).
@@ -14,7 +14,7 @@
 #include <algorithm>
 
 #include "common.h"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace ctl {
 
@@ -23,17 +23,20 @@ struct ConvTapW {
   int dh, dw;
 };
 
-static constexpr int WG_THREADS = 192;            // TMA warp, MMA warp, 4 epilogue warps
+// producer warpgroup (one TMA thread) + two consumer warpgroups: warpgroup g owns output channels
+// [64 g, 64 g + 64) of the 128-channel cout tile (= dy box g) and the whole N = cin-per-item width
+static constexpr int WG_THREADS = 384;
 static constexpr int WG_BOX_BYTES = 128 * 64 * 2;  // one [128 px][64 ch] box
-// two shapes of the work item: N (cin per item) up to 128 with a 3-stage ring, or up to 256 with a 2-stage ring
-// (one dy tile then feeds twice the MMA work: less TMA fill per flop, but a shallower pipeline; CTL_WGRAD_WIDE)
-template <bool WIDE>
+static constexpr uint32_t WG_PRODUCER_REGS = 40, WG_CONSUMER_REGS = 232;
+// N (cin per work item) = 64, 128 or 256: the wider the item, the more MMA work one dy tile feeds (less TMA fill per
+// flop), the shallower the ring that fits in shared memory (CTL_WGRAD_WIDE selects 256)
+template <int BNW>
 struct WgCfg {
-  static constexpr int XBOXES = WIDE ? 4 : 2;
-  static constexpr int STAGES = WIDE ? 2 : 3;
+  static constexpr int XBOXES = BNW / 64;
+  static constexpr int STAGES = BNW == 256 ? 2 : (BNW == 128 ? 3 : 4);
   static constexpr int STAGE_BYTES = (2 + XBOXES) * WG_BOX_BYTES;  // dy: 2 boxes (128 cout) + x boxes
-  static constexpr int ACC_COLS = WIDE ? 256 : 128;
   static constexpr size_t SMEM = 1024 + STAGES * STAGE_BYTES + 256;
+  static_assert(SMEM <= 227 * 1024, "conv_wgrad_kernel shared memory");
 };
 
 struct WgradParams {
@@ -42,7 +45,7 @@ struct WgradParams {
   ConvTapW taps[9];
   int n_taps, cin, cout;
   int TW, TH, tiles_w, tiles_h, m_tiles;
-  int bnw;         // cin per work item: 64, 128 or (wide kernel) 256
+  int bnw;         // cin per work item: 64, 128 or 256
   int cin_chunks;  // cin / bnw
   int cout_tiles;  // ceil(cout / 128)
   int n_items;     // cout_tiles * n_taps * cin_chunks
@@ -51,55 +54,30 @@ struct WgradParams {
   float* part;     // [splits][cout_pad][n_taps * cin]
 };
 
-// MN-major SWIZZLE_128B operand: 128-byte rows = 64 M/N elements, consecutive rows = consecutive K; `lbo` = byte
-// distance between 64-element M/N blocks, 8-row K groups 1024 bytes apart.
-__device__ __forceinline__ uint64_t make_sw128_mnmajor_desc(uint32_t smem_addr, uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-
-template <bool WIDE>
+template <int BNW>
 __global__ void __launch_bounds__(WG_THREADS, 1) conv_wgrad_kernel(const __grid_constant__ WgradParams p) {
-  constexpr int WG_STAGES = WgCfg<WIDE>::STAGES, WG_STAGE_BYTES = WgCfg<WIDE>::STAGE_BYTES, ACC_COLS = WgCfg<WIDE>::ACC_COLS;
+  constexpr int WG_STAGES = WgCfg<BNW>::STAGES, WG_STAGE_BYTES = WgCfg<BNW>::STAGE_BYTES;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t bar_base = smem_base + WG_STAGES * WG_STAGE_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (WG_STAGES + s); };
-  auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * WG_STAGES + s); };
-  auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * WG_STAGES + 2 + s); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * WG_STAGES + 4);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < WG_STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(tfull_bar(s), 1);
-      mbar_init(tempty_bar(s), 4);
+      mbar_init(empty_bar(s), 2);  // one arrive per consumer warpgroup
     }
     fence_barrier_init();
     tma_prefetch_desc(&p.dy_map);
     for (int i = 0; i < 4; ++i) tma_prefetch_desc(&p.x_map[i]);
   }
-  if (warp == 1) tmem_alloc<2 * ACC_COLS>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   pdl_launch_dependents();
   pdl_wait();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
 
   const int n_units = p.n_items * p.splits;
-  const int xboxes = p.bnw / 64;
   const int tiles_per_img = p.tiles_w * p.tiles_h;
   // unit -> (work item, pixel-tile range)
   auto unit_range = [&](int u, int& item, int& t0, int& t1) {
@@ -115,8 +93,9 @@ __global__ void __launch_bounds__(WG_THREADS, 1) conv_wgrad_kernel(const __grid_
     chunk = r - tap * p.cin_chunks;
   };
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    setmaxnreg_dec<WG_PRODUCER_REGS>();
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
@@ -131,11 +110,11 @@ __global__ void __launch_bounds__(WG_THREADS, 1) conv_wgrad_kernel(const __grid_
           const int h0 = th * p.TH, w0 = tw * p.TW;
           mbar_wait(empty_bar(stage), phase ^ 1u);
           const uint32_t dst = smem_base + stage * WG_STAGE_BYTES;
-          mbar_arrive_expect_tx(full_bar(stage), (2 + xboxes) * WG_BOX_BYTES);
+          mbar_arrive_expect_tx(full_bar(stage), WG_STAGE_BYTES);
           tma_load_4d(dst, &p.dy_map, full_bar(stage), ct * 128, w0, h0, img);
           tma_load_4d(dst + WG_BOX_BYTES, &p.dy_map, full_bar(stage), ct * 128 + 64, w0, h0, img);  // OOB channels -> 0
-          for (int j = 0; j < xboxes; ++j)
-            tma_load_4d(dst + (2 + j) * WG_BOX_BYTES, &p.x_map[tap.map], full_bar(stage), chunk * p.bnw + 64 * j,
+          for (int j = 0; j < BNW / 64; ++j)
+            tma_load_4d(dst + (2 + j) * WG_BOX_BYTES, &p.x_map[tap.map], full_bar(stage), chunk * BNW + 64 * j,
                         w0 + tap.dw, h0 + tap.dh, img);
           if (++stage == WG_STAGES) {
             stage = 0;
@@ -151,80 +130,51 @@ __global__ void __launch_bounds__(WG_THREADS, 1) conv_wgrad_kernel(const __grid_
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_f16(128, (uint32_t)p.bnw) | (1u << 15) | (1u << 16);  // A and B MN-major
-      int stage = 0, as = 0;
-      uint32_t phase = 0, aphase = 0;
-      for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
-        int item, t0, t1;
-        unit_range(u, item, t0, t1);
-        mbar_wait(tempty_bar(as), aphase ^ 1u);
-        tc_fence_after();
-        const uint32_t acc = tmem_base + as * ACC_COLS;
-        for (int t = t0; t < t1; ++t) {
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          const uint32_t a0 = smem_base + stage * WG_STAGE_BYTES, b0 = a0 + 2 * WG_BOX_BYTES;
-#pragma unroll
-          for (int k = 0; k < 8; ++k) {  // 16 pixels (rows) per MMA
-            const uint64_t da = make_sw128_mnmajor_desc(a0 + k * 2048, WG_BOX_BYTES);
-            const uint64_t db = make_sw128_mnmajor_desc(b0 + k * 2048, WG_BOX_BYTES);
-            umma_f16(acc, da, db, idesc, (t > t0 || k > 0) ? 1u : 0u);
-          }
-          umma_commit(empty_bar(stage));
-          if (++stage == WG_STAGES) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-        umma_commit(tfull_bar(as));
-        if (++as == 2) {
-          as = 0;
-          aphase ^= 1u;
-        }
-      }
-    }
   } else {
-    const int quarter = warp & 3;
-    const int row = quarter * 32 + lane;  // cout inside the tile == TMEM lane
+    // ===== consumers: D[64 cout][BNW cin] += dy^T x over the unit's pixels (both operands MN-major: rows of a box
+    // are the K = pixel dimension), then the fp32 partial tile goes straight from the registers to `part` =====
+    setmaxnreg_inc<WG_CONSUMER_REGS>();
+    const int wg = (threadIdx.x >> 7) - 1;
+    const bool wg_leader = (threadIdx.x & 127) == 0;
+    const int row0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // cout inside the 128-channel tile
     const int ktot = p.n_taps * p.cin;
-    int as = 0;
-    uint32_t aphase = 0;
+    float acc[BNW / 2];
+    int stage = 0;
+    uint32_t phase = 0;
     for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
       int item, t0, t1, ct, tapi, chunk;
       unit_range(u, item, t0, t1);
       item_coords(item, ct, tapi, chunk);
       const int split = u - item * p.splits;
-      mbar_wait(tfull_bar(as), aphase);
-      tc_fence_after();
-      float* dst = p.part + ((size_t)split * p.cout_pad + ct * 128 + row) * ktot + tapi * p.cin + chunk * p.bnw;
-      const uint32_t taddr = tmem_base + as * ACC_COLS + (static_cast<uint32_t>(quarter * 32) << 16);
-      for (int c = 0; c < p.bnw; c += 16) {
-        uint32_t r[16];
-        tmem_ld16(taddr + c, r);
-        tmem_ld_wait();
+      int held = -1;
+      for (int t = t0; t < t1; ++t) {
+        mbar_wait(full_bar(stage), phase);
+        const uint32_t a0 = smem_base + stage * WG_STAGE_BYTES + wg * WG_BOX_BYTES, b0 = smem_base + stage * WG_STAGE_BYTES + 2 * WG_BOX_BYTES;
+        wgmma_fence();
 #pragma unroll
-        for (int q = 0; q < 4; ++q)
-          *reinterpret_cast<float4*>(dst + c + 4 * q) =
-              make_float4(__uint_as_float(r[4 * q]), __uint_as_float(r[4 * q + 1]), __uint_as_float(r[4 * q + 2]),
-                          __uint_as_float(r[4 * q + 3]));
+        for (int k = 0; k < 8; ++k) {  // 16 pixels (rows) per MMA
+          const uint64_t da = make_sw128_mnmajor_desc(a0 + k * 2048, WG_BOX_BYTES);
+          const uint64_t db = make_sw128_mnmajor_desc(b0 + k * 2048, WG_BOX_BYTES);
+          wgmma_f16<BNW, 1, 1>(acc, da, db, (t > t0 || k > 0) ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (held >= 0 && wg_leader) mbar_arrive(empty_bar(held));
+        held = stage;
+        if (++stage == WG_STAGES) {
+          stage = 0;
+          phase ^= 1u;
+        }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(as));
-      if (++as == 2) {
-        as = 0;
-        aphase ^= 1u;
-      }
+      wgmma_wait<0>();
+      if (held >= 0 && wg_leader) mbar_arrive(empty_bar(held));
+      float* dst = p.part + ((size_t)split * p.cout_pad + ct * 128 + row0) * ktot + tapi * p.cin + chunk * BNW + 2 * (lane & 3);
+#pragma unroll
+      for (int j = 0; j < BNW / 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          *reinterpret_cast<float2*>(dst + (size_t)(8 * h) * ktot + 8 * j) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc<2 * ACC_COLS>(tmem_base);
   }
 }
 
@@ -349,7 +299,7 @@ static int wgrad_plan(int n, int h, int w, int cin, int cout, int ksize, int str
 //    fixed order in double precision (deterministic, no atomics).
 // =======================================================================================
 static constexpr int BN_THREADS = 256;
-static constexpr int BN_MAX_BLOCKS = 592;  // 148 SMs x 4
+static constexpr int BN_MAX_BLOCKS = 528;  // 132 SMs x 4
 
 static int bn_batched() {
   static const int v = [] { const char* e = getenv("CTL_BN_FINALIZE_BATCHED"); return e ? atoi(e) : 1; }();
@@ -1150,18 +1100,19 @@ int ctl_conv2d_wgrad_nhwc_f16_ex(const void* x, int32_t n, int32_t h, int32_t w,
   }
   static bool attr_set = false;
   if (!attr_set) {
-    CTL_CUDA(cudaFuncSetAttribute(conv_wgrad_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  (int)WgCfg<false>::SMEM));
-    CTL_CUDA(cudaFuncSetAttribute(conv_wgrad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  (int)WgCfg<true>::SMEM));
+    CTL_CUDA(cudaFuncSetAttribute(conv_wgrad_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WgCfg<64>::SMEM));
+    CTL_CUDA(cudaFuncSetAttribute(conv_wgrad_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WgCfg<128>::SMEM));
+    CTL_CUDA(cudaFuncSetAttribute(conv_wgrad_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WgCfg<256>::SMEM));
     attr_set = true;
   }
   cudaStream_t st = (cudaStream_t)stream;
   const int grid = std::min(p.n_items * p.splits, sm_count());
   if (p.bnw == 256)
-    CTL_CUDA(launch_k(conv_wgrad_kernel<true>, dim3(grid), dim3(WG_THREADS), WgCfg<true>::SMEM, st, p));
+    CTL_CUDA(launch_k(conv_wgrad_kernel<256>, dim3(grid), dim3(WG_THREADS), WgCfg<256>::SMEM, st, p));
+  else if (p.bnw == 128)
+    CTL_CUDA(launch_k(conv_wgrad_kernel<128>, dim3(grid), dim3(WG_THREADS), WgCfg<128>::SMEM, st, p));
   else
-    CTL_CUDA(launch_k(conv_wgrad_kernel<false>, dim3(grid), dim3(WG_THREADS), WgCfg<false>::SMEM, st, p));
+    CTL_CUDA(launch_k(conv_wgrad_kernel<64>, dim3(grid), dim3(WG_THREADS), WgCfg<64>::SMEM, st, p));
   if (param_layout != 0 || out_scale != 1.f) {
     const size_t np = (size_t)cout * cin;
     const int rgrid = (int)std::min<size_t>((np + 255) / 256, (size_t)sm_count() * 8);

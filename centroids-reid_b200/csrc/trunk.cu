@@ -17,7 +17,7 @@
 #include <vector>
 
 #include "common.h"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace ctl {
 

@@ -7,7 +7,7 @@ Same names, arguments and on-disk formats:
   * `results.npy`     pickled dict  query_path -> {"indices", "paths", "distances"}   (get_similar.py:121-137)
   * `query_embeddings.npy`, `query_paths.npy`
 
-What changes underneath: `_inference` runs the B200 trunk engine (`modelling.baseline.embed`), `run_inference` keeps
+What changes underneath: `_inference` runs the H100 trunk engine (`modelling.baseline.embed`), `run_inference` keeps
 the embeddings on the device and copies them to the host ONCE (the reference does one `.cpu().numpy()` per image,
 inference_utils.py:123-125), `calculate_centroids` is the segmented-mean kernel, and `get_similar` streams
 query x gallery distances into a per-query top-k without materialising the [Q, G] matrix or its argsort

@@ -1,6 +1,6 @@
 """Drop-in for losses/triplet_loss.py of the reference: normalize, euclidean_dist,
 cosine_dist, hard_example_mining, TripletLoss, CrossEntropyLabelSmooth -- same names,
-arguments and return values, computed by the sm_100a kernels behind include/ctl_b200.h.
+arguments and return values, computed by the sm_90a kernels behind include/ctl_b200.h.
 """
 from __future__ import annotations
 

@@ -1,1 +1,1 @@
-"""ResNet50 / ResNet50-IBN-A trunks: reference-layout parameters + the B200 inference engine."""
+"""ResNet50 / ResNet50-IBN-A trunks: reference-layout parameters + the H100 inference engine."""

@@ -1,9 +1,9 @@
-"""B200 inference engine of the ResNet50(-IBN-A) trunk.
+"""H100 inference engine of the ResNet50(-IBN-A) trunk.
 
 Packs a reference-layout state_dict (keys of modelling/backbones/resnet.py:90-120 /
 resnet_ibn_a.py:77-124) into kernel operands -- NHWC / [Cout][kh][kw][Cin] fp16 weights with the
 eval-mode BatchNorm folded in, fp32 biases -- and runs the forward as a sequence of fused
-conv+BN(+residual)(+ReLU) tcgen05 launches (csrc/conv.cu) through the C ABI.
+conv+BN(+residual)(+ReLU) wgmma launches (csrc/conv.cu) through the C ABI.
 
 Forward semantics follow ResNet.forward (resnet.py:122-133: NO ReLU after the stem) and
 ResNet_IBN.forward (resnet_ibn_a.py:126-141: ReLU after the stem; IBN as bn1 of layer1-3),

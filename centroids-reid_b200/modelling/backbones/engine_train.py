@@ -1,9 +1,9 @@
-"""Train-mode ResNet-50 trunk on the B200 kernels: forward with batch-statistics BatchNorm and the full backward
+"""Train-mode ResNet-50 trunk on the H100 kernels: forward with batch-statistics BatchNorm and the full backward
 (what autograd does through modelling/backbones/resnet.py:67-87,122-133 + baseline.py:91-96 in the reference).
 
-Per conv+BN of the forward:   conv (tcgen05 implicit GEMM, raw fp16 output y)  ->  batch statistics  ->
+Per conv+BN of the forward:   conv (wgmma implicit GEMM, raw fp16 output y)  ->  batch statistics  ->
 z = [relu](gamma * xhat + beta [+ shortcut])  (fp16).  The backward walks the blocks in reverse:
-BN/ReLU backward (masked grad g, dgamma, dbeta, dy), weight gradient (tcgen05 GEMM over the pixel dimension),
+BN/ReLU backward (masked grad g, dgamma, dbeta, dy), weight gradient (wgmma GEMM over the pixel dimension),
 data gradient = the forward conv kernel on dy with the transposed / flipped weights (stride-2 layers through
 zero-insertion upsampling), shortcut gradients folded into conv1's data gradient through the kernel's residual
 input.  Activations and activation gradients are fp16, every reduction and all parameter gradients fp32.

@@ -1,10 +1,10 @@
 """Drop-in for modelling/baseline.py: Baseline(cfg).forward(x) -> (base_out, global_feat).
 
-Parameters live in reference-layout modules (`self.base.*`); eval-mode forward runs the B200
+Parameters live in reference-layout modules (`self.base.*`); eval-mode forward runs the H100
 engine, whose packed operands are rebuilt lazily whenever the parameters change
 (`invalidate()`; call it after `opt.step()` / `load_state_dict`).  Train-mode forward (ResNet-50) runs the
 training engine (batch-statistics BatchNorm, running statistics updated in place) and is differentiable:
-`global_feat.backward()` fills `.grad` of every trunk parameter through the B200 backward kernels.
+`global_feat.backward()` fills `.grad` of every trunk parameter through the H100 backward kernels.
 """
 from __future__ import annotations
 
@@ -22,7 +22,7 @@ _LAYERS = {"resnet50": ((3, 4, 6, 3), False), "resnet101": ((3, 4, 23, 3), False
 
 
 class _TrunkTrainFn(torch.autograd.Function):
-    """global_feat = trunk(x; parameters) with the B200 training engine; backward returns the parameter gradients
+    """global_feat = trunk(x; parameters) with the H100 training engine; backward returns the parameter gradients
     (the input crops get no gradient, like the reference's data tensors)."""
 
     @staticmethod
@@ -52,7 +52,7 @@ class Baseline(nn.Module):
         super().__init__()
         name = cfg.MODEL.NAME
         if name not in _LAYERS:
-            raise NotImplementedError(f"MODEL.NAME={name!r}: the B200 trunk covers the bottleneck ResNets {sorted(_LAYERS)}")
+            raise NotImplementedError(f"MODEL.NAME={name!r}: the H100 trunk covers the bottleneck ResNets {sorted(_LAYERS)}")
         layers, ibn = _LAYERS[name]
         self.model_name = name
         self.use_mixed_precision = cfg.USE_MIXED_PRECISION

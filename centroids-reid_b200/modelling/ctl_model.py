@@ -1,6 +1,6 @@
 """Drop-in for the tensor part of modelling/bases.py (ModelBase) and train_ctl_model.py
 (CTLModel.training_step): same attribute names (backbone, bn, fc_query, center_loss,
-contrastive_loss, xent), same hook signatures, the arithmetic on the B200 kernels.
+contrastive_loss, xent), same hook signatures, the arithmetic on the H100 kernels.
 
 pytorch_lightning is not a dependency of this package (and is absent from the build image): the class
 derives from pl.LightningModule when PL is importable and from nn.Module otherwise.  Under PL the
@@ -180,7 +180,7 @@ class CTLModel(_Base):
         x, class_labels, camid, is_real = batch
         opts = self._step_optimizers()
         if opts is None:
-            _, features = self.backbone(x)  # train mode: B200 training engine (differentiable w.r.t. the trunk parameters)
+            _, features = self.backbone(x)  # train mode: H100 training engine (differentiable w.r.t. the trunk parameters)
             return self.training_step_from_features(features, class_labels, is_real)
         opt, opt_center = opts
         epoch = int(getattr(getattr(self, "trainer", None), "current_epoch", 0) or 0)

@@ -1,7 +1,7 @@
 """Multi-GPU plumbing of the training step (SURVEY 8e): the reference trains data-parallel over pids under
 PyTorch-Lightning DDP -- rank r owns `np.array_split(pids, world)[r]` (datasets/samplers/distributed_pids_sampler.py:71),
 losses are computed on the local P x K batch only, and ONE gradient all-reduce (mean) over all parameters follows
-the backward.  The B200 trunk produces every parameter gradient at the end of its single backward call, so there
+the backward.  The H100 trunk produces every parameter gradient at the end of its single backward call, so there
 is nothing to overlap bucket by bucket: the gradients are packed into a few large flat fp32 buckets and reduced
 with torch.distributed (NCCL on GPUs; gloo in the CPU tests).  Wrapping the module in torch DDP works too (its hooks
 fire on the same `.grad`s); this helper is the dependency-free form.

@@ -58,8 +58,8 @@ def pid_order(pids) -> np.ndarray:
 def pid_order_pays(nq: int, ng: int) -> bool:
     """topk_and_eval: identity-ordered planes trade a cheaper pass 1 (tile list: ~30 % of the matrix) for a lumpier pass 2
     (the positives and nearest rows of a query tile sit in a few gallery tiles, and the looser subset threshold lengthens
-    the candidate lists).  Measured on a B200: 3368 x 15913 -> 1.41 ms sorted vs 1.30 ms in caller order;
-    16384 x 25000 -> 7.9 ms vs 9.8 ms.  evaluate_streamed (no candidates) gains at both sizes."""
+    the candidate lists); the threshold is where sorting paid off in earlier measurements of this kernel pair and has
+    not been re-measured on the H100 build."""
     return int(nq) * int(ng) >= 150_000_000
 
 

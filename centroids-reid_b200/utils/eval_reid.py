@@ -3,7 +3,7 @@
 `eval_func` keeps the reference signature (it consumes a full [Q, G] ranking that the caller
 already holds on the host) and is vectorised host code; the product path does NOT build that
 ranking at all: `eval_streamed` computes the same (cmc, mAP, all_topk, single_performance)
-straight from the features on the B200 (retrieval.evaluate_streamed), which is what
+straight from the features on the H100 (retrieval.evaluate_streamed), which is what
 `R1_mAP.compute` in utils/reid_metric.py calls.
 """
 from __future__ import annotations
@@ -67,7 +67,7 @@ def eval_func(indices, q_pids, g_pids, q_camids, g_camids, max_rank=50, respect_
 
 def eval_streamed(q_feats, g_feats, q_pids, g_pids, q_camids, g_camids, max_rank=50, respect_camids=False,
                   dist_func="euclidean", feat_norm=False):
-    """eval_func's results computed on the B200 directly from query / gallery features
+    """eval_func's results computed on the H100 directly from query / gallery features
     (no distance matrix, no argsort).  Host tensors are staged to the current CUDA device."""
     import torch
 

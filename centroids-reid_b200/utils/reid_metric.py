@@ -1,5 +1,5 @@
 """Drop-in for utils/reid_metric.py of the reference (get_euclidean, get_cosine,
-get_dist_func, R1_mAP) on the B200 distance kernel.
+get_dist_func, R1_mAP) on the H100 distance kernel.
 
 The distance functions return the full [m, n] matrix like the reference (on the device of
 the inputs; host inputs are staged through the GPU and returned on the host).  R1_mAP.compute
@@ -73,7 +73,7 @@ class R1_mAP:
         g_pids = np.asarray(pids[nq:])
         q_camids, g_camids = camids[:nq], camids[nq:]
         if getattr(self.hparms.TEST, "VISUALIZE", "no") == "yes":
-            raise NotImplementedError("ranked-result visualisation (utils/visrank.py) is outside the B200 hot path")
+            raise NotImplementedError("ranked-result visualisation (utils/visrank.py) is outside the H100 hot path")
         # reid_metric.py:113-136: F.normalize -> dist -> argsort -> eval_func(.., 50, ..), fused.
         # (the reference hard-codes max_rank=50 in the eval_func call, :134-136)
         # both operands are stored in identity order: the collect pass then skips every tile that cannot hold a positive

@@ -1,4 +1,4 @@
-/* libctl_b200.so -- C ABI of the B200-native centroid-triplet re-ID hot path.
+/* libctl_b200.so -- C ABI of the H100-native centroid-triplet re-ID hot path.
  *
  * The reference (mikwieczorek/centroids-reid @ a1825b7) is pure Python: the path it exposes
  * is a Python module/class API called by PyTorch-Lightning hooks, there is no FFI of its
@@ -14,10 +14,10 @@
  *     synchronises unless stated;
  *   - return value: 0 = ok, negative = CTL_ERR_* (argument / capacity error),
  *     positive = cudaError_t; ctl_last_error() returns a thread-local description;
- *   - there is NO CPU fallback: without an sm_100 device every compute entry point fails.
+ *   - there is NO CPU fallback: without an sm_90 device every compute entry point fails.
  */
-#ifndef CTL_B200_H_
-#define CTL_B200_H_
+#ifndef CTL_H100_H_
+#define CTL_H100_H_
 
 #include <stddef.h>
 #include <stdint.h>
@@ -39,7 +39,7 @@ typedef void* ctl_stream_t; /* cudaStream_t */
 
 const char* ctl_last_error(void);
 int ctl_abi_version(void);
-/* 0 when the current device is sm_100 (B200); CTL_ERR_NO_DEVICE otherwise. */
+/* 0 when the current device is sm_90 (H100); CTL_ERR_NO_DEVICE otherwise. */
 int ctl_device_check(void);
 
 /* ------------------------------------------------------------------------------------------
@@ -464,4 +464,4 @@ int ctl_augment_batch_u8(const void* images_u8_nhwc, int32_t n, int32_t h, int32
 #ifdef __cplusplus
 }
 #endif
-#endif /* CTL_B200_H_ */
+#endif /* CTL_H100_H_ */

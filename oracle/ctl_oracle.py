@@ -523,7 +523,7 @@ def embed_forward(x, sd, bn_sd, **kw):
 
 def trunk_forward_fp16sim(x, sd, last_stride=1, ibn=False, layers=R50_LAYERS):
     """Same-precision checker for the fp16 engine: trunk_forward(eval) with the rounding points
-    of the B200 path made explicit -- eval BatchNorm folded into fp16 weights, fp32
+    of the H100 path made explicit -- eval BatchNorm folded into fp16 weights, fp32
     accumulation, every stored activation rounded to fp16 (the reference under AMP has the same
     class of rounding, SURVEY A.3; an fp16 trunk cannot meet 1e-4 against the fp32 reference, so
     parity of the trunk is defined against this function and reported against the fp32 one)."""
@@ -584,7 +584,7 @@ class _RoundHalfSTE(torch.autograd.Function):
 def trunk_train_fp16sim(x, sd, dfeat=None, last_stride=1, layers=R50_LAYERS, momentum=0.1, forced=None, ibn=False,
                         round_fp16=True):
     """Train-mode trunk (ResNet.forward resnet.py:122-133 with BatchNorm2d batch statistics, Bottleneck.forward
-    :67-87) in float64 with the B200 training path's rounding points: fp16 crops and conv weights, every stored
+    :67-87) in float64 with the H100 training path's rounding points: fp16 crops and conv weights, every stored
     activation (conv output, BN/ReLU output) rounded to fp16, statistics / BN arithmetic / GAP in full precision.
     Returns (global_feat, grads, running) where grads maps state_dict names -> d(sum(global_feat * dfeat))/d(param)
     and running holds the updated running statistics.  ibn=True: the IBN-a variant (resnet_ibn_a.py:18-32,54-74,126-141:

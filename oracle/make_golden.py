@@ -2,6 +2,7 @@
 reference (/root/reference, through oracle/ref_import.py) on seeded synthetic inputs.
 
     python -m oracle.make_golden [--only loss,retrieval,trunk,trunk_train,trunk_autocast,masks,centroids,market]
+    python -m oracle.make_golden --only bench_autocast     (on a GPU: tests/golden/bench_autocast_*.npz)
 
 The reference has no tests and no golden vectors of its own (SURVEY.md section 4); these
 files are what pins the oracle restatement (oracle/ctl_oracle.py) and, through it, the
@@ -357,9 +358,122 @@ def gen_trunk_autocast(ref):
     np.savez_compressed(os.path.join(GOLD, "trunk_autocast.npz"), **out)
 
 
+def gen_random_erasing(ref):
+    """The reference's RandomErasing (datasets/transforms/random_erasing.py) on one normalised 32x20 crop, driven by
+    `random.seed(s)` for s = 0..4 (tests/test_oracle_golden.py replays the same draws)."""
+    import importlib.util
+    import random
+
+    from oracle.ref_import import REFERENCE_ROOT
+
+    path = os.path.join(REFERENCE_ROOT, "datasets", "transforms", "random_erasing.py")
+    spec = importlib.util.spec_from_file_location("ref_random_erasing", path)
+    mod = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(mod)
+    mean, std = (0.485, 0.456, 0.406), (0.229, 0.224, 0.225)
+    H, W = 32, 20
+    img = torch.from_numpy(np.random.default_rng(1).integers(0, 256, (1, H, W, 3), dtype=np.uint8))
+    norm = (img[0].permute(2, 0, 1).float() / 255.0 - torch.tensor(mean)[:, None, None]) / torch.tensor(std)[:, None, None]
+    out = {"image": img.numpy()}
+    for seed in range(5):
+        random.seed(seed)
+        out[f"erased_{seed}"] = mod.RandomErasing(probability=1.0, mean=mean)(norm.clone()).numpy()
+    np.savez_compressed(os.path.join(GOLD, "random_erasing.npz"), **out)
+
+
+TRIPLET_VARIANTS = ((None, "euclidean"), (0.3, "cosine"), (None, "cosine"))
+
+
+def gen_triplet_variants(ref):
+    """The reference's TripletLoss(margin=None) / dist_func='cosine' (losses/triplet_loss.py:44-65,127-137,157-158):
+    loss and input gradient on the batch of tests/test_losses_gpu.py::test_triplet_loss_soft_margin_and_cosine_variants."""
+    feats, labels, _ = O.synth_batch(10, 4, 384, 100, seed=4, pad_fraction=0.2)
+    feats = feats * 0.3 + 0.05
+    out = {"in_checksum": checksum(feats)}
+    for margin, dist in TRIPLET_VARIANTS:
+        fr = feats.clone().requires_grad_(True)
+        lr, _, _ = ref.triplet_loss.TripletLoss(margin, dist)(fr, labels)
+        lr.backward()
+        out[f"{margin}_{dist}_loss"] = np.array(float(lr))
+        out[f"{margin}_{dist}_grad"] = fr.grad.numpy()
+    np.savez_compressed(os.path.join(GOLD, "triplet_variants.npz"), **out)
+
+
+BENCH_EVAL_CASES = (("r50", False, (256, 128), 256), ("ibn", True, (320, 320), 128))
+BENCH_TRAIN_CASES = (("r50", False, (256, 128), 16, 16), ("ibn", True, (320, 320), 32, 4))
+BENCH_ROW_STRIDE = 16      # stored feature rows: every 16th image of the batch
+BENCH_GRAD_SAMPLE = 512    # stored elements per parameter gradient (evenly strided)
+
+
+def bench_grad_sample(t):
+    f = t.detach().flatten()
+    return f[:: max(1, f.numel() // BENCH_GRAD_SAMPLE)][:BENCH_GRAD_SAMPLE]
+
+
+def gen_bench_autocast(ref):
+    """The reference's own trunk ON THE GPU at the bench shapes (tests/test_reference_autocast_gpu.py), under CUDA fp16
+    autocast and in fp32: eval features of every 16th image; for one training step, the features of every 16th image and,
+    per parameter, an evenly strided sample of its autocast and fp32 gradients plus their full norms and full cosine.
+    Needs a CUDA device (run once where oracle/_ref is present)."""
+    assert torch.cuda.is_available(), "bench_autocast runs the reference on cuda:0"
+    for tag, ibn, hw, bs in BENCH_EVAL_CASES:
+        sd = O.make_trunk_state(seed=7, ibn=ibn)
+        x = torch.randn(bs, 3, *hw, generator=torch.Generator().manual_seed(77))
+        cfg = default_cfg(ref)
+        cfg.MODEL.NAME = "resnet50_ibn_a" if ibn else "resnet50"
+        base = ref.baseline.Baseline(cfg)
+        base.base.load_state_dict(sd, strict=True)
+        base = base.cuda().eval()
+        with torch.no_grad():
+            _, f32 = base(x.cuda())
+            with torch.autocast("cuda", dtype=torch.float16):
+                _, amp = base(x.cuda())
+        rows = slice(None, None, BENCH_ROW_STRIDE)
+        np.savez_compressed(os.path.join(GOLD, f"bench_autocast_eval_{tag}.npz"), in_checksum=checksum(x),
+                            feat_fp32=f32[rows].float().cpu().numpy(), feat_amp=amp[rows].float().cpu().numpy())
+        del base
+        torch.cuda.empty_cache()
+    scale = 1024.0
+    for tag, ibn, hw, P, K in BENCH_TRAIN_CASES:
+        n = P * K
+        sd = O.make_trunk_state(seed=17, ibn=ibn)
+        gen = torch.Generator().manual_seed(5)
+        x = torch.randn(n, 3, *hw, generator=gen)
+        dfeat = torch.randn(n, 2048, generator=gen) * 1e-3
+        cfg = default_cfg(ref)
+        cfg.MODEL.NAME = "resnet50_ibn_a" if ibn else "resnet50"
+        base = ref.baseline.Baseline(cfg)
+        base.base.load_state_dict(sd, strict=True)
+        base = base.cuda().train()
+        xc, dc = x.cuda(), dfeat.cuda()
+        with torch.autocast("cuda", dtype=torch.float16):
+            _, rfeat = base(xc)
+        ((rfeat.float() * dc).sum() * scale).backward()
+        rgrads = {k: (p.grad / scale) for k, p in base.base.named_parameters() if p.grad is not None}
+        rfeat = rfeat.detach().float()
+        base.zero_grad(set_to_none=True)
+        base.base.load_state_dict(sd, strict=True)
+        _, rfeat32 = base(xc)
+        (rfeat32 * dc).sum().backward()
+        rgrads32 = {k: p.grad.clone() for k, p in base.base.named_parameters() if p.grad is not None}
+        names = sorted(rgrads)
+        out = {"in_checksum": checksum(torch.cat((x.flatten(), dfeat.flatten()))),
+               "feat_amp": rfeat[::BENCH_ROW_STRIDE].cpu().numpy(), "names": np.array(names)}
+        for k in names:
+            a, b = rgrads[k].double(), rgrads32[k].double()
+            out[f"amp/{k}"] = bench_grad_sample(rgrads[k]).float().cpu().numpy()
+            out[f"fp32/{k}"] = bench_grad_sample(rgrads32[k]).float().cpu().numpy()
+            out[f"stats/{k}"] = np.array([float(a.norm()), float(b.norm()), float((a * b).sum() / (a.norm() * b.norm() + 1e-300))])
+        np.savez_compressed(os.path.join(GOLD, f"bench_autocast_train_{tag}.npz"), **out)
+        del base
+        torch.cuda.empty_cache()
+        print(f"bench autocast {tag}: {len(names)} gradients stored")
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--only", default="loss,loss_variants,masks,retrieval,centroids,trunk,trunk_train,trunk_autocast,market")
+    ap.add_argument("--only", default="loss,loss_variants,masks,retrieval,centroids,trunk,trunk_train,trunk_autocast,"
+                    "random_erasing,triplet_variants,market")
     args = ap.parse_args()
     only = set(args.only.split(","))
     os.makedirs(GOLD, exist_ok=True)
@@ -383,6 +497,12 @@ def main():
         gen_trunk_train(ref)
     if "trunk_autocast" in only:
         gen_trunk_autocast(ref)
+    if "triplet_variants" in only:
+        gen_triplet_variants(ref)
+    if "random_erasing" in only:
+        gen_random_erasing(ref)
+    if "bench_autocast" in only:  # not in the default set: needs a GPU
+        gen_bench_autocast(ref)
     if "market" in only:
         # BASELINE config 3 shape; the reference's per-query python loop takes ~80 s here
         gen_retrieval(ref, "market", 3368, 15913, 751, 3.0, 0, store_dist=False)

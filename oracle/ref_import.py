@@ -12,11 +12,10 @@ defaults (``use_gpu=True`` with hard ``.cuda()`` calls, losses/center_loss.py:21
 losses/triplet_loss.py:187,202) are switched to ``use_gpu=False`` -- that is the only
 behavioural patch, and it does not touch any arithmetic.
 
-/root/reference does not exist on the GPU box.  There the module imports the verbatim copy
-``oracle/_ref`` made by ``oracle/vendor_ref.py`` (git-ignored, shipped with the snapshot); it is
-used only by ``bench.py --impl reference`` / the ``cpu_baseline`` legs (the reference timed on the
-host cores) and by ``tests/test_reference_autocast_gpu.py`` (the reference under CUDA autocast as
-the same-precision checker).  Tests that need it skip with a message when the copy is absent.
+Where /root/reference is absent the module imports the verbatim copy ``oracle/_ref`` made by
+``oracle/vendor_ref.py`` (git-ignored); that is used only by ``bench.py --impl reference`` / the
+``cpu_baseline`` legs (the reference timed on the host cores) and by ``oracle/make_golden.py``.
+No test imports the reference: tests compare against tests/golden/.
 """
 from __future__ import annotations
 
@@ -31,7 +30,7 @@ _VENDORED = os.path.join(os.path.dirname(os.path.abspath(__file__)), "_ref")  # 
 def _default_root():
     if os.path.isfile("/root/reference/train_ctl_model.py"):
         return "/root/reference"
-    return _VENDORED  # the GPU box: the verbatim copy that travelled with the snapshot
+    return _VENDORED  # the verbatim copy made by oracle/vendor_ref.py
 
 
 REFERENCE_ROOT = os.environ.get("CTL_REFERENCE_ROOT") or _default_root()
@@ -191,7 +190,7 @@ def load_reference():
     if not reference_available():
         raise RuntimeError(
             f"reference tree not found at {REFERENCE_ROOT}; the golden vectors under "
-            "tests/golden/ are what travels to the GPU box"
+            "tests/golden/ hold what the tests compare against"
         )
     _install_stubs()
     # The reference is used as a flat source tree with its root on sys.path

@@ -1,7 +1,7 @@
 """pytest configuration: registers the `gpu` marker and puts the repo root on sys.path.
 
 `-m "not gpu"` (CPU, build container): oracle vs golden vectors, host logic, C-ABI symbol
-checks, world_size-2 gloo tests.   `-m gpu` (B200 box): CUDA path vs oracle / goldens.
+checks, world_size-2 gloo tests.   `-m gpu` (H100): CUDA path vs oracle / goldens.
 """
 import os
 import sys
@@ -16,7 +16,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100)")
 
 
 @pytest.fixture(scope="session")

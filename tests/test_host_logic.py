@@ -166,7 +166,7 @@ def test_ctl_model_under_a_lightning_like_base(monkeypatch):
 
 def test_no_undefined_names_in_the_python_sources():
     """GPU-only branches (sharded retrieval, NCCL paths) are not executed by the CPU suite: a static scan keeps a typo in them
-    from surviving until the GPU box (tools/undefined_names.py: names loaded in a function that are bound nowhere)."""
+    from surviving until a GPU run (tools/undefined_names.py: names loaded in a function that are bound nowhere)."""
     import subprocess
     import sys
     from pathlib import Path

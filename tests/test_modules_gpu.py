@@ -1,4 +1,4 @@
-"""GPU: the reference-named module surface (Baseline, CTLModel hooks) on the B200 engine."""
+"""GPU: the reference-named module surface (Baseline, CTLModel hooks) on the H100 engine."""
 import numpy as np
 import pytest
 import torch
@@ -53,7 +53,7 @@ def test_ctl_model_hooks():
     scale = float(ref.abs().max())
     assert float((out["emb"].cpu() - ref).abs().max()) <= 1e-2 * scale  # fp16 trunk vs fp32 oracle
     model.train()
-    assert model.backbone(x.cuda())[1].requires_grad  # train mode: differentiable B200 training engine
+    assert model.backbone(x.cuda())[1].requires_grad  # train mode: differentiable H100 training engine
     # training_step tail from prescribed features == the reference's training_step golden (train mode, like the reference)
     name = "p8k4_pad"
     g = load_golden(f"loss_{name}.npz")

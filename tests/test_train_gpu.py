@@ -185,7 +185,7 @@ def _rel(a, b):
 
 
 def test_trunk_train_step_against_float64_autograd():
-    """Train-mode ResNet-50 forward + full backward on the B200 kernels vs float64 autograd of the same network
+    """Train-mode ResNet-50 forward + full backward on the H100 kernels vs float64 autograd of the same network
     with the engine's fp16 rounding points (oracle.trunk_train_fp16sim).
 
     (1) independent forward: features within 2e-2; gradients agree in direction and size (ReLU masks are

@@ -210,7 +210,7 @@ def test_full_trunk_matches_checker_and_reference_golden(tag, ibn, hw):
 @pytest.mark.gpu
 @pytest.mark.parametrize("shape", [(3, 64, 48), (2, 256, 128), (40, 64, 32), (5, 128, 64), (1, 8, 8)])
 def test_stem_pool_fused(shape):
-    """conv1 + folded bn1 (+ReLU) + maxpool in one kernel (UMMA windows over raw input rows) against the fp16-operand
+    """conv1 + folded bn1 (+ReLU) + maxpool in one kernel (wgmma windows over raw input rows) against the fp16-operand
     convolution followed by max_pool2d; ranges that start inside an image and cross images are both exercised."""
     from ctl_b200 import _native as N
     from ctl_b200.modelling.backbones.engine import pack_stem_fused

@@ -1,4 +1,4 @@
-"""Time the fused stem (pack + conv/pool kernels) alone (GPU box)."""
+"""Time the fused stem (pack + conv/pool kernels) alone (needs a GPU)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -1,4 +1,4 @@
-"""GPU box: time the training trunk (forward + backward) at the BASELINE config-2 batch (256 x 3 x 256 x 128)."""
+"""Needs a GPU: time the training trunk (forward + backward) at the BASELINE config-2 batch (256 x 3 x 256 x 128)."""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -1,4 +1,4 @@
-"""Quick device-side timing of the trunk engine (GPU box)."""
+"""Quick device-side timing of the trunk engine (needs a GPU)."""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -1,4 +1,4 @@
-"""Debug helper (GPU box): distance matrix of tiny / structured inputs vs torch, with a
+"""Debug helper (needs a GPU): distance matrix of tiny / structured inputs vs torch, with a
 pattern dump when something is off."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

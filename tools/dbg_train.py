@@ -1,4 +1,4 @@
-"""GPU box, test-side debugging aid (executes the oracle like tests/ do): per-parameter gradient error of the training
+"""Needs a GPU; test-side debugging aid (executes the oracle like tests/ do): per-parameter gradient error of the training
 trunk vs the float64 oracle, for several loss scales."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -1,4 +1,4 @@
-"""GPU-box host probe: CPU model, thread count and the accuracy of torch's CPU fp32 matmul."""
+"""Host probe: CPU model, thread count and the accuracy of torch's CPU fp32 matmul."""
 import os, torch
 print("cpu_count", os.cpu_count(), "torch threads", torch.get_num_threads())
 try:

@@ -1,4 +1,4 @@
-"""Per-launch CUDA-event times of one trunk forward (GPU box): name, us, TFLOP/s, GB/s."""
+"""Per-launch CUDA-event times of one trunk forward (needs a GPU): name, us, TFLOP/s, GB/s."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -1,4 +1,4 @@
-"""GPU box: wall-time breakdown of one retrieval step (3368 x 15913 x 2048, top-100 + CMC/mAP)."""
+"""Needs a GPU: wall-time breakdown of one retrieval step (3368 x 15913 x 2048, top-100 + CMC/mAP)."""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
@@ -47,7 +47,7 @@ buckets = torch.zeros(nq, ids.max_pos + 1, dtype=torch.int32, device="cuda")
 print("pass count                %.3f ms" % gpu_ms(N.PassDesc(thr_keys=pos_keys.data_ptr(), thr_count=pos_count.data_ptr(), buckets=buckets.data_ptr(), **idk)))
 tau = torch.full((nq,), 1.9, device="cuda"); cand = torch.empty(nq, 4096, dtype=torch.int64, device="cuda"); cc = torch.zeros(nq, dtype=torch.int32, device="cuda")
 print("pass cand(tau=1.9)+count  %.3f ms" % gpu_ms(N.PassDesc(tau=tau.data_ptr(), cand_keys=cand.data_ptr(), cand_count=cc.data_ptr(), cand_cap=4096, overflow=ovf.data_ptr(), thr_keys=pos_keys.data_ptr(), thr_count=pos_count.data_ptr(), buckets=buckets.data_ptr(), **idk)))
-PH = ["tile_setup", "wait_acc", "bar_meta", "tmem_wait", "element_loop", "tile_end", "-", "-"]
+PH = ["tile_setup", "mma_and_stage", "bar_meta", "acc_read", "element_loop", "tile_end", "-", "-"]
 def phases(name, desc):
     prof = torch.zeros(148 * 2 * 8, dtype=torch.int64, device="cuda")
     L.ctl_debug_set_dist_profile(prof.data_ptr())

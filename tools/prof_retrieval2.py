@@ -1,4 +1,4 @@
-"""GPU box: where one retrieval step (3368 x 15913 x 2048, top-100 + CMC/mAP) spends its time -- host enqueue vs device,
+"""Needs a GPU: where one retrieval step (3368 x 15913 x 2048, top-100 + CMC/mAP) spends its time -- host enqueue vs device,
 exact vs one-product (cheap) tiles, epilogue phases of the cheap pass."""
 import ctypes as C
 import os

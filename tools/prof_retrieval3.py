@@ -1,4 +1,4 @@
-"""GPU box: epilogue phase counters of pass 2 (candidates + bucket counts) in caller order vs identity order."""
+"""Needs a GPU: epilogue phase counters of pass 2 (candidates + bucket counts) in caller order vs identity order."""
 import ctypes as C
 import os
 import sys
@@ -16,7 +16,7 @@ feats, pids, cams = synth.synth_retrieval(NQ, NG, 751, D, 3.0, 0)
 q, g = feats[:NQ].cuda(), feats[NQ:].cuda()
 args = (pids[:NQ], pids[NQ:], cams[:NQ], cams[NQ:])
 L = N.lib()
-PH = ["tile_setup", "wait_acc", "bar_meta", "tmem_wait", "element_loop", "tile_end"]
+PH = ["tile_setup", "mma_and_stage", "bar_meta", "acc_read", "element_loop", "tile_end"]
 
 
 def run(name, qp, gp, ids, gmap):

@@ -1,4 +1,4 @@
-"""GPU box: topk_and_eval at a config-5 shard shape (16384 x 25000 x 2048) -- caller order vs identity order + tile lists."""
+"""Needs a GPU: topk_and_eval at a config-5 shard shape (16384 x 25000 x 2048) -- caller order vs identity order + tile lists."""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
