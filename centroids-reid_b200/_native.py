@@ -78,7 +78,6 @@ SIGNATURES = {
     "ctl_eval_finalize": (C.c_int, [_p, _p, _i64, _i32, _p, _p, _p]),
     "ctl_eval_finalize_packed": (C.c_int, [_p, _p, _i64, _i32, _p, _p, _p, _p, _p]),
     "ctl_dist_pass": (C.c_int, [_p, _i64, _p, _i64, _i32, _i32, C.POINTER(PassDesc), _p]),
-    "ctl_debug_set_dist_profile": (None, [_p]),
     "ctl_topk_plan": (C.c_int, [_i64, _i32, C.POINTER(_i32), C.POINTER(_i32), C.POINTER(_i32), C.POINTER(_i32)]),
     "ctl_select_tau": (C.c_int, [_p, _i64, _i32, _i32, _i32, _p, _p]),
     "ctl_dist_worklist_bytes": (_sz, [_i64, _i64]),
@@ -109,7 +108,6 @@ SIGNATURES = {
     "ctl_train_workspace_bytes": (_sz, [_p, _i32, _i32, _i32]),
     "ctl_train_forward": (C.c_int, [_p, _p, _i32, _i32, _i32, _p, _p, _sz, _p]),
     "ctl_train_backward": (C.c_int, [_p, _p, C.c_float, _p, _sz, _p]),
-    "ctl_stem_conv7x7": (C.c_int, [_p, _i32, _i32, _i32, _p, _p, _i32, _p, _p]),
     "ctl_stem_conv7x7_tc": (C.c_int, [_p, _i32, _i32, _i32, _p, _p, _i32, _p, _p]),
     "ctl_stem_pad_bytes": (C.c_size_t, [_i32, _i32, _i32]),
     "ctl_stem_pool_fused": (C.c_int, [_p, _i32, _i32, _i32, _p, _p, _p, _i32, _p, _p]),

@@ -308,7 +308,7 @@ struct C64Params {
   CUtensorMap w_map;    // [64][576] weights, box {64, 64}
   CUtensorMap out_map;  // NHWC output, box {64, 8, 16, 1}
   const float* bias;
-  int n_img, H, W, tiles_h, tiles_w, relu, use_base_offset;
+  int n_img, H, W, tiles_h, tiles_w, relu;
 };
 
 __global__ void __launch_bounds__(CONV_THREADS, 1) conv3x3_c64_kernel(const __grid_constant__ C64Params p) {
@@ -391,8 +391,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv3x3_c64_kernel(const __gr
       for (int t = 0; t < 9; ++t) {
         const int r = t / 3, s = t - 3 * r;
         const uint32_t a0 = slab + (r * 16 + s) * 128;
-        uint64_t da = make_sw128_kmajor_desc(a0, 2048);
-        if (p.use_base_offset) da |= static_cast<uint64_t>((a0 >> 7) & 7u) << 49;
+        const uint64_t da = make_sw128_kmajor_desc(a0, 2048);
         const uint64_t db = make_sw128_kmajor_desc(w_sm + t * 64 * 128);
 #pragma unroll
         for (int k = 0; k < 4; ++k) wgmma_f16<64>(acc, desc_advance_k(da, k), desc_advance_k(db, k), (t | k) ? 1u : 0u);
@@ -416,79 +415,6 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv3x3_c64_kernel(const __gr
       }
     }
     if (leader) tma_store_wait<0>();
-  }
-}
-
-// ---------------------------------------------------------------------------------------
-// stem: conv 7x7 / 2, pad 3, 3 -> 64 (+ folded BN, optional ReLU) from NCHW fp32 to NHWC fp16
-// (modelling/backbones/resnet.py:93-97,122-125 -- NO ReLU; resnet_ibn_a.py:84-86,126-129 -- ReLU)
-// Direct convolution on the CUDA cores: K = 147 with Cin = 3 does not map on TMA channel slabs.
-// Block: 8 x 32 output pixels x 64 channels, 256 threads, each 8 pixels (along w) x 8 channels.
-// ---------------------------------------------------------------------------------------
-static constexpr int ST_TH = 8, ST_TW = 32;
-static constexpr int ST_PH = 2 * ST_TH + 5, ST_PW = 2 * ST_TW + 5;  // 21 x 69 input patch
-static constexpr size_t STEM_SMEM = (size_t)(147 * 64 + 3 * ST_PH * (ST_PW + 1)) * sizeof(float);
-
-__global__ void __launch_bounds__(256) stem_conv_kernel(const float* __restrict__ x, int H, int W,
-                                                        const float* __restrict__ wt /*[147][64], k=(c*7+r)*7+s*/,
-                                                        const float* __restrict__ bias, int relu,
-                                                        __half* __restrict__ out, int Ho, int Wo) {
-  extern __shared__ float ssm[];
-  float* sw = ssm;                 // [147][64]
-  float* sp = ssm + 147 * 64;      // [3][ST_PH][ST_PW + 1]
-  const int n = blockIdx.z, oh0 = blockIdx.y * ST_TH, ow0 = blockIdx.x * ST_TW;
-  for (int i = threadIdx.x; i < 147 * 64; i += 256) sw[i] = wt[i];
-  const int ih0 = 2 * oh0 - 3, iw0 = 2 * ow0 - 3;
-  for (int i = threadIdx.x; i < 3 * ST_PH * ST_PW; i += 256) {
-    const int c = i / (ST_PH * ST_PW), rem = i % (ST_PH * ST_PW), ph = rem / ST_PW, pw = rem % ST_PW;
-    const int ih = ih0 + ph, iw = iw0 + pw;
-    float v = 0.f;
-    if (ih >= 0 && ih < H && iw >= 0 && iw < W) v = x[(((size_t)n * 3 + c) * H + ih) * W + iw];
-    sp[(c * ST_PH + ph) * (ST_PW + 1) + pw] = v;
-  }
-  __syncthreads();
-  const int cg = threadIdx.x & 7;    // 8 channels
-  const int pg = threadIdx.x >> 3;   // 32 pixel groups: row = pg / 4, 8 consecutive columns
-  const int orow = pg >> 2, ocol0 = (pg & 3) * 8;
-  float acc[8][8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i)
-#pragma unroll
-    for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
-  for (int c = 0; c < 3; ++c)
-    for (int r = 0; r < 7; ++r) {
-      const float* prow = sp + (c * ST_PH + 2 * orow + r) * (ST_PW + 1) + 2 * ocol0;
-#pragma unroll
-      for (int s = 0; s < 7; ++s) {
-        const float4 w0 = *reinterpret_cast<const float4*>(sw + ((c * 7 + r) * 7 + s) * 64 + cg * 8);
-        const float4 w1 = *reinterpret_cast<const float4*>(sw + ((c * 7 + r) * 7 + s) * 64 + cg * 8 + 4);
-        const float wv[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float xv = prow[2 * i + s];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) acc[i][j] = __fmaf_rn(xv, wv[j], acc[i][j]);
-        }
-      }
-    }
-  const int oh = oh0 + orow;
-  if (oh >= Ho) return;
-  float b[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) b[j] = bias[cg * 8 + j];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int ow = ow0 + ocol0 + i;
-    if (ow >= Wo) continue;
-    uint4 o;
-    __half2* ph2 = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      float a0 = acc[i][2 * j] + b[2 * j], a1 = acc[i][2 * j + 1] + b[2 * j + 1];
-      if (relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); }
-      ph2[j] = __floats2half2_rn(a0, a1);
-    }
-    *reinterpret_cast<uint4*>(out + (((size_t)n * Ho + oh) * Wo + ow) * 64 + cg * 8) = o;
   }
 }
 
@@ -1061,7 +987,6 @@ static int launch_c64(const void* x, int n, int h, int w, const void* weight, co
   p.tiles_h = (h + 15) / 16;
   p.tiles_w = (w + 7) / 8;
   p.relu = relu;
-  p.use_base_offset = 0;  // see the kernel comment: shifted views need no base_offset
   int rc;
   const uint64_t dims[4] = {64, (uint64_t)w, (uint64_t)h, (uint64_t)n};
   const uint64_t strd[4] = {2, 128, (uint64_t)w * 128, (uint64_t)h * w * 128};
@@ -1169,11 +1094,8 @@ int ctl_conv2d_nhwc_f16(const void* x, int32_t n, int32_t h, int32_t w, int32_t 
   if (rc) return rc;
   const int pad = ksize == 3 ? 1 : 0;
   const int Ho = (h + 2 * pad - ksize) / stride + 1, Wo = (w + 2 * pad - ksize) / stride + 1;
-  {
-    static const int c64_mode = [] { const char* e = getenv("CTL_CONV_C64"); return e ? atoi(e) : 1; }();
-    if (c64_mode && ksize == 3 && stride == 1 && cin == 64 && cout == 64 && !residual && relu_from == 0)
-      return launch_c64(x, n, h, w, weight, bias, out, relu, (cudaStream_t)stream);
-  }
+  if (ksize == 3 && stride == 1 && cin == 64 && cout == 64 && !residual && relu_from == 0)
+    return launch_c64(x, n, h, w, weight, bias, out, relu, (cudaStream_t)stream);
   ConvKernelParams p = {};
   pick_tile(Ho, Wo, &p.TH, &p.TW);
   p.tiles_h = (Ho + p.TH - 1) / p.TH;
@@ -1223,25 +1145,6 @@ int ctl_conv1x1_dual_nhwc_f16(const void* x1, int32_t cin1, const void* x2, int3
   p.taps[1] = ConvTap{1, 0, 0, cin1, cin2 / 64};
   p.k_blocks = (cin1 + cin2) / 64;
   return finish_and_launch(p, n, Ho, Wo, cout, cin1 + cin2, weight_cat, bias, nullptr, out, relu, 0, (cudaStream_t)stream);
-}
-
-int ctl_stem_conv7x7(const float* x_nchw, int32_t n, int32_t h, int32_t w, const float* weight_k64, const float* bias,
-                     int32_t relu, void* out_nhwc_f16, ctl_stream_t stream) {
-  CTL_CHECK_ARG(x_nchw && weight_k64 && bias && out_nhwc_f16, "null pointer");
-  CTL_CHECK_ARG(n >= 1 && h >= 7 && w >= 7, "bad input shape");
-  int rc = ctl_device_check();
-  if (rc) return rc;
-  const int Ho = (h + 6 - 7) / 2 + 1, Wo = (w + 6 - 7) / 2 + 1;
-  static bool attr_set = false;
-  if (!attr_set) {
-    CTL_CUDA(cudaFuncSetAttribute(stem_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)STEM_SMEM));
-    attr_set = true;
-  }
-  dim3 grid((Wo + ST_TW - 1) / ST_TW, (Ho + ST_TH - 1) / ST_TH, n);
-  stem_conv_kernel<<<grid, 256, STEM_SMEM, (cudaStream_t)stream>>>(x_nchw, h, w, weight_k64, bias, relu,
-                                                                  static_cast<__half*>(out_nhwc_f16), Ho, Wo);
-  CTL_LAUNCH_CHECK();
-  return 0;
 }
 
 int ctl_stem_conv7x7_tc(const float* x_nchw, int32_t n, int32_t h, int32_t w, const void* weight_k192_f16,

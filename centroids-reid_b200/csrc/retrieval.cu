@@ -46,10 +46,9 @@ static constexpr int CNT_STRIDE = THR_MAX / 2 + 1;          // bucket counters o
 static constexpr int CNT_BYTES = BM * CNT_STRIDE * 4;
 static constexpr int FAR_LEVELS = 1;  // buckets of the count pass resolved by plain compares against the farthest positives
                                       // (config 3 retrieval step on one H100: none 5.57 ms, 1 level 5.51 ms, 2 levels 5.79 ms)
-static constexpr int UNIT_R = 4;  // count passes: gallery tiles a CTA runs back to back for ONE query tile
 static constexpr size_t GEMM_SMEM = STAGES * STAGE_BYTES + ACC_BYTES + META_BYTES + THR_BYTES + CNT_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 static_assert(GEMM_SMEM <= 227 * 1024, "dist_gemm_kernel shared memory");
-static_assert(UNIT_R * BN < 65536, "16-bit bucket counters of a unit");
+static_assert(BN < 65536, "16-bit bucket counters of a tile");
 
 // ---------------------------------------------------------------------------------------
 // (distance, index) keys: ascending uint64 order == ascending (distance, index)
@@ -204,9 +203,7 @@ struct GemmPass {
   // A pass that only collects the positives and a threshold needs the tiles that can hold a positive plus a subset for
   // the group minima -- with both operands stored in identity order that is a fraction of the matrix.
   const int* work;
-  int unit_r;           // gallery tiles per work item of a full pass (set by launch_gemm_pass)
   const int* g_map;     // optional: gallery row -> index written into the keys (rows stored in another order)
-  long long* prof;  // debug: [grid][8] epilogue cycle counters (tools/prof_retrieval.py)
 };
 
 struct GemmMaps {
@@ -249,24 +246,17 @@ __device__ __noinline__ int bucket_search_global(const unsigned long long* __res
   return lo;
 }
 
-// Work item w of a pass -> query tile mt, first gallery tile nt0, number of gallery tiles run back to back.
-//   full pass: (query tile, `unit_r` consecutive gallery tiles), query tiles fastest -- the CTAs that run concurrently
-//              touch ~5 gallery-tile groups x all query tiles, so each operand tile is fetched from HBM about once.
-//              unit_r > 1 for the count pass: the per-row state of a query tile (sorted thresholds in shared memory,
-//              bucket counters) is set up and flushed once per unit instead of once per tile;
-//   tile list: one listed tile, id = nt * m_tiles + mt.
-__device__ __forceinline__ void unit_coords(const GemmPass& p, int w, int& mt, int& nt0, int& cnt) {
-  if (p.work) {
-    const int id = p.work[1 + w];
-    nt0 = id / p.m_tiles;
-    mt = id - nt0 * p.m_tiles;
-    cnt = 1;
-  } else {
-    const int g = w / p.m_tiles;
-    mt = w - g * p.m_tiles;
-    nt0 = g * p.unit_r;
-    cnt = min(p.unit_r, p.n_tiles - nt0);
-  }
+// Work item w of a pass -> query tile mt, gallery tile nt; tile id = nt * m_tiles + mt.
+//   full pass: tile id w, query tiles fastest -- the CTAs that run concurrently touch ~5 gallery tiles x all query
+//              tiles, so each operand tile is fetched from HBM about once.  One tile per work item in every pass: longer
+//              items for the count pass (the per-row thresholds and counters set up and flushed once per several gallery
+//              tiles) gave no gain (config 3 retrieval step on one H100, measured while the epilogue still spilled
+//              registers: 5.51 ms (1 tile), 5.50 ms (2), 5.74 ms (4));
+//   tile list: the listed tile work[1 + w].
+__device__ __forceinline__ void tile_coords(const GemmPass& p, int w, int& mt, int& nt) {
+  const int id = p.work ? p.work[1 + w] : w;
+  nt = id / p.m_tiles;
+  mt = id - nt * p.m_tiles;
 }
 
 // Shared-memory word of element (row, col) of the staged dot-product tile: 16-byte chunks of a row XOR-swizzled by
@@ -290,8 +280,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  // every role walks the same sequence of work items (unit_coords)
-  const int num_work = p.work ? p.work[0] : p.m_tiles * ((p.n_tiles + p.unit_r - 1) / p.unit_r);
+  // every role walks the same sequence of work items (tile_coords)
+  const int num_work = p.work ? p.work[0] : p.m_tiles * p.n_tiles;
   const int k_blocks = (p.d + BK - 1) / BK;
 
   if (threadIdx.x == 0) {
@@ -314,22 +304,21 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
       int stage = 0;
       uint32_t phase = 0;
       for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
-        int mt, nt0, ncnt;
-        unit_coords(p, w, mt, nt0, ncnt);
-        for (int nt = nt0; nt < nt0 + ncnt; ++nt)
-          for (int kb = 0; kb < k_blocks; ++kb) {
-            mbar_wait(empty_bar(stage), phase ^ 1u);
-            const uint32_t dst = smem_base + stage * STAGE_BYTES;
-            mbar_arrive_expect_tx(full_bar(stage), STAGE_BYTES);
-            tma_load_2d(dst + 0 * TILE_BYTES, &maps.q_hi, full_bar(stage), kb * BK, mt * BM);
-            tma_load_2d(dst + 1 * TILE_BYTES, &maps.q_lo, full_bar(stage), kb * BK, mt * BM);
-            tma_load_2d(dst + 2 * TILE_BYTES, &maps.g_hi, full_bar(stage), kb * BK, nt * BN);
-            tma_load_2d(dst + 3 * TILE_BYTES, &maps.g_lo, full_bar(stage), kb * BK, nt * BN);
-            if (++stage == STAGES) {
-              stage = 0;
-              phase ^= 1u;
-            }
+        int mt, nt;
+        tile_coords(p, w, mt, nt);
+        for (int kb = 0; kb < k_blocks; ++kb) {
+          mbar_wait(empty_bar(stage), phase ^ 1u);
+          const uint32_t dst = smem_base + stage * STAGE_BYTES;
+          mbar_arrive_expect_tx(full_bar(stage), STAGE_BYTES);
+          tma_load_2d(dst + 0 * TILE_BYTES, &maps.q_hi, full_bar(stage), kb * BK, mt * BM);
+          tma_load_2d(dst + 1 * TILE_BYTES, &maps.q_lo, full_bar(stage), kb * BK, mt * BM);
+          tma_load_2d(dst + 2 * TILE_BYTES, &maps.g_hi, full_bar(stage), kb * BK, nt * BN);
+          tma_load_2d(dst + 3 * TILE_BYTES, &maps.g_lo, full_bar(stage), kb * BK, nt * BN);
+          if (++stage == STAGES) {
+            stage = 0;
+            phase ^= 1u;
           }
+        }
       }
     }
   } else {
@@ -355,14 +344,6 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     unsigned int* cm_idx = reinterpret_cast<unsigned int*>(cm_mask + 2 * BN);  // index written into the keys
     uint32_t* thr_s = reinterpret_cast<uint32_t*>(smem_raw + (thr_base - smem_u32(smem_raw)));
     int it = 0;
-    long long pc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    long long tprev = clock64();
-#define CTL_STAMP(i)                \
-  if (p.prof) {                     \
-    const long long _t = clock64(); \
-    pc[i] += _t - tprev;            \
-    tprev = _t;                     \
-  }
     uint32_t* cnt_s = thr_s + BM * THR_STRIDE;  // [BM][CNT_STRIDE]: 2 x 16-bit bucket counters per word
     const bool thr_in_smem = p.buckets != nullptr;
     const int n_stage = min(p.max_pos, THR_MAX);
@@ -370,9 +351,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     uint32_t* cnt_row = cnt_s + row_in_tile * CNT_STRIDE;
     if (thr_in_smem)  // the counters start at zero; every flush leaves them at zero again
       for (int i = et; i < BM * CNT_STRIDE; i += 256) cnt_s[i] = 0u;
-    for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
-      int mt, nt0, ncnt;
-      unit_coords(p, w, mt, nt0, ncnt);
+    for (int w = blockIdx.x; w < num_work; w += gridDim.x, ++it) {
+      int mt, nt;
+      tile_coords(p, w, mt, nt);
       // ---- per work item: the state of this thread's query row ----
       const int row = mt * BM + row_in_tile;
       const bool row_ok = row < p.nq;
@@ -401,8 +382,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
       }
       // The distance halves of each row's first THR_MAX sorted positives are staged in shared memory (row stride 36
       // words: 16-byte rows, conflict-free LDS.128), so the bucket of a gallery row comes from shared memory instead of a
-      // dependent chain of L2 loads; deeper positives (rare) and exact distance ties use the 64-bit global search.  Staged once per work
-      // item (UNIT_R gallery tiles of the same query tile); the first tile's metadata barrier publishes it.
+      // dependent chain of L2 loads; deeper positives (rare) and exact distance ties use the 64-bit global search.  The
+      // metadata barrier publishes the staged rows.
       if (thr_in_smem) {
         const int rows_here = min(BM, p.nq - mt * BM);
         const unsigned long long* src = p.thr_keys + (size_t)mt * BM * p.max_pos;
@@ -426,7 +407,6 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 #pragma unroll
         for (int i = 0; i < BM / 8; ++i) thr_s[(ew + 8 * i) * THR_STRIDE + lane] = v0[i];
       }
-      for (int nt = nt0; nt < nt0 + ncnt; ++nt, ++it) {
       const int mb = (it & 1) * BN;  // double-buffered metadata slice
       if (et < BN) {
         const int col = nt * BN + et;
@@ -440,7 +420,6 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
         }
       }
       const int nps = min(npos, THR_MAX);
-      CTL_STAMP(0)
       {
         // acc0 = q_hi.g_hi, acc1 = q_hi.g_lo + q_lo.g_hi over this warpgroup's 64 query rows x 128 gallery rows
         float acc0[BN / 2], acc1[BN / 2];
@@ -483,9 +462,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
           }
         __syncwarp();
       }
-      CTL_STAMP(1)
       named_bar_sync(1, 256);  // metadata slice published
-      CTL_STAMP(2)
 #pragma unroll 1
       for (int c = 0; c < 4; ++c) {
         float r0[16];
@@ -494,7 +471,6 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
           const float4 v = *reinterpret_cast<const float4*>(acc_s + acc_word(row_in_tile, chalf * 64 + c * 16 + 4 * q4));
           r0[4 * q4] = v.x; r0[4 * q4 + 1] = v.y; r0[4 * q4 + 2] = v.z; r0[4 * q4 + 3] = v.w;
         }
-        CTL_STAMP(3)
         const int cl0 = chalf * 64 + c * 16;  // column inside the tile
         const int col0 = nt * BN + cl0;
         // ---- phase 1, branch-free: the 16 distances and the masks of the (rare) elements that need more ----
@@ -613,15 +589,12 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
           }
         }
         if (p.gmin && row_ok && col0 < p.ng) p.gmin[(size_t)row * p.n_groups + (col0 >> 4)] = gmin;
-        CTL_STAMP(4)
       }
       __syncwarp();  // this warp's staged rows are read: the next tile may overwrite them
-      CTL_STAMP(5)
-      }  // gallery tiles of the work item
       if (thr_in_smem) {
         named_bar_sync(2, 256);  // every warp is done with this work item's thresholds and counters
         // flush: the two threads of a row take alternate counter words of the row and leave them zero.  The next
-        // work item's first metadata barrier orders these writes (and the new thresholds) before any use.
+        // work item's metadata barrier orders these writes (and the new thresholds) before any use.
         if (row_ok) {
           int* dst = p.buckets + (size_t)row * (p.max_pos + 1);
           for (int wd = chalf; wd < THR_MAX / 2; wd += 2) {
@@ -633,14 +606,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
             }
           }
         }
-        CTL_STAMP(6)
       }
     }
-    if (p.prof && (threadIdx.x == 128 || threadIdx.x == 128 + 5 * 32 + 7)) {
-      long long* dst = p.prof + ((size_t)blockIdx.x * 2 + (threadIdx.x == 128 ? 0 : 1)) * 8;
-      for (int i = 0; i < 8; ++i) dst[i] = pc[i];
-    }
-#undef CTL_STAMP
   }
 }
 
@@ -768,7 +735,7 @@ __global__ void __launch_bounds__(WL_THREADS) dist_worklist_kernel(const int* __
     const int tile = t0 + threadIdx.x;
     int keep = 0;
     if (tile < num_tiles) {
-      const int nt = tile / m_tiles, mt = tile - nt * m_tiles;  // tile id = nt * m_tiles + mt (unit_coords)
+      const int nt = tile / m_tiles, mt = tile - nt * m_tiles;  // tile id = nt * m_tiles + mt (tile_coords)
       const int2 a = s_rng[mt], b = s_rng[m_tiles + nt];
       keep = (!(b.y < a.x || b.x > a.y)) || (keep_stride > 0 && nt % keep_stride == 0);
     }
@@ -891,13 +858,7 @@ static int launch_gemm_pass(const void* q_planes, int64_t nq, const void* g_plan
     CTL_CUDA(cudaFuncSetAttribute(dist_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GEMM_SMEM));
     attr_set = true;
   }
-  static const int unit_r_env = [] {
-    const char* e = getenv("CTL_DIST_UNIT_R");  // experiments: gallery tiles per work item of the count pass
-    const int v = e ? atoi(e) : 1;  // config 3 step on one H100: 5.51 ms (1), 5.50 ms (2), 5.74 ms (4) -- no gain
-    return v >= 1 && v <= UNIT_R ? v : UNIT_R;
-  }();
-  p.unit_r = p.buckets ? unit_r_env : 1;
-  const long long items = (long long)p.m_tiles * ((p.n_tiles + p.unit_r - 1) / p.unit_r);
+  const long long items = (long long)p.m_tiles * p.n_tiles;
   const int grid = (int)std::min<long long>(items, sm_count());
   dist_gemm_kernel<<<grid, GEMM_THREADS, GEMM_SMEM, stream>>>(maps, p);
   CTL_LAUNCH_CHECK();
@@ -930,8 +891,6 @@ static int sort_rows(unsigned long long* keys, const int* counts, int64_t rows, 
   CTL_LAUNCH_CHECK();
   return 0;
 }
-
-static long long* g_dist_prof = nullptr;
 
 static int next_pow2(int v) {
   int p = 1;
@@ -1185,8 +1144,6 @@ int ctl_eval_finalize_packed(const int32_t* buckets, const int32_t* pos_count, i
   return 0;
 }
 
-void ctl_debug_set_dist_profile(long long* device_buffer) { g_dist_prof = device_buffer; }
-
 int ctl_dist_pass(const void* q_planes, int64_t nq, const void* g_planes, int64_t ng, int32_t d, int32_t flags,
                   const ctl_pass_desc* desc, ctl_stream_t stream) {
   CTL_CHECK_ARG(desc != nullptr, "null pass descriptor");
@@ -1218,7 +1175,6 @@ int ctl_dist_pass(const void* q_planes, int64_t nq, const void* g_planes, int64_
   CTL_CHECK_ARG(!e.buckets || (e.thr_keys && e.thr_count), "count needs the sorted positives");
   p.overflow = e.overflow;
   p.g_off = e.g_index_offset;
-  p.prof = g_dist_prof;
   CTL_CHECK_ARG(e.g_index_offset >= 0 && e.g_index_offset + ng < (1ll << 32), "gallery index out of uint32 range");
   CTL_CHECK_ARG(!e.tile_list || !(e.dist_out || e.cand_keys || e.buckets),
                 "a tile list drops tiles: not for the full matrix, the candidates or the bucket counts");

@@ -28,12 +28,12 @@ struct ConvTapW {
 static constexpr int WG_THREADS = 384;
 static constexpr int WG_BOX_BYTES = 128 * 64 * 2;  // one [128 px][64 ch] box
 static constexpr uint32_t WG_PRODUCER_REGS = 40, WG_CONSUMER_REGS = 232;
-// N (cin per work item) = 64, 128 or 256: the wider the item, the more MMA work one dy tile feeds (less TMA fill per
-// flop), the shallower the ring that fits in shared memory (CTL_WGRAD_WIDE selects 256)
+// N (cin per work item) = 64 or 128: the wider the item, the more MMA work one dy tile feeds (less TMA fill per
+// flop), the shallower the ring that fits in shared memory
 template <int BNW>
 struct WgCfg {
   static constexpr int XBOXES = BNW / 64;
-  static constexpr int STAGES = BNW == 256 ? 2 : (BNW == 128 ? 3 : 4);
+  static constexpr int STAGES = BNW == 128 ? 3 : 4;
   static constexpr int STAGE_BYTES = (2 + XBOXES) * WG_BOX_BYTES;  // dy: 2 boxes (128 cout) + x boxes
   static constexpr size_t SMEM = 1024 + STAGES * STAGE_BYTES + 256;
   static_assert(SMEM <= 227 * 1024, "conv_wgrad_kernel shared memory");
@@ -45,7 +45,7 @@ struct WgradParams {
   ConvTapW taps[9];
   int n_taps, cin, cout;
   int TW, TH, tiles_w, tiles_h, m_tiles;
-  int bnw;         // cin per work item: 64, 128 or 256
+  int bnw;         // cin per work item: 64 or 128
   int cin_chunks;  // cin / bnw
   int cout_tiles;  // ceil(cout / 128)
   int n_items;     // cout_tiles * n_taps * cin_chunks
@@ -280,8 +280,7 @@ static int wgrad_plan(int n, int h, int w, int cin, int cout, int ksize, int str
   p->n_taps = ksize * ksize;
   p->cin = cin;
   p->cout = cout;
-  static const int wide_mode = [] { const char* e = getenv("CTL_WGRAD_WIDE"); return e ? atoi(e) : 0; }();
-  p->bnw = (wide_mode && cin % 256 == 0) ? 256 : (cin % 128 == 0 ? 128 : 64);
+  p->bnw = cin % 128 == 0 ? 128 : 64;
   p->cin_chunks = cin / p->bnw;
   p->cout_tiles = (cout + 127) / 128;
   p->cout_pad = p->cout_tiles * 128;
@@ -300,11 +299,6 @@ static int wgrad_plan(int n, int h, int w, int cin, int cout, int ksize, int str
 // =======================================================================================
 static constexpr int BN_THREADS = 256;
 static constexpr int BN_MAX_BLOCKS = 528;  // 132 SMs x 4
-
-static int bn_batched() {
-  static const int v = [] { const char* e = getenv("CTL_BN_FINALIZE_BATCHED"); return e ? atoi(e) : 1; }();
-  return v;
-}
 
 struct BnGeom {
   int groups;         // C / 8
@@ -412,36 +406,28 @@ __global__ void __launch_bounds__(BN_THREADS) bn_stats_kernel(const __half* __re
 // Sum of the per-block partials of 32 channels: 32 warps split the block index (stride 32), partial sums are combined in
 // a fixed order (deterministic).  Returns the two totals of channel `c` to the threads with part == 0.
 __device__ __forceinline__ void bn_sum_partials(const float* __restrict__ part, int blocks, int C, int c, int part_id,
-                                                double (*sh)[2][32], double& s0, double& s1, int batched) {  // sh[32][2][32]
+                                                double (*sh)[2][32], double& s0, double& s1) {  // sh[32][2][32]
   // the partials are loaded in groups of 4 INDEPENDENT loads (5 memory round trips instead of a chain of up to 19
-  // dependent ones -- the finalize kernels were pure latency, ~15 us each, 127 launches per training step) and summed in
-  // the same fixed order as before (bit-identical results).  A first version loaded all 19 at once: 64 registers x 1024
-  // threads = the whole register file of an SM, and the kernel showed sporadic 20-80 ms stalls -- keep the footprint low.
+  // dependent ones -- the finalize kernels are pure latency, 127 launches per training step) and summed in a fixed
+  // order (deterministic).  Loading all 19 at once takes 64 registers x 1024 threads = the whole register file of an
+  // SM, and the kernel then showed sporadic 20-80 ms stalls -- keep the footprint low.
   constexpr int MAXQ = (BN_MAX_BLOCKS + 31) / 32, GRP = 4;
   double a = 0.0, b = 0.0;
-  if (!batched) {  // round-1 form: a chain of dependent loads (CTL_BN_FINALIZE_BATCHED=0)
-    if (c < C)
-      for (int blk = part_id; blk < blocks; blk += 32) {
-        a += (double)part[(size_t)blk * 2 * C + c];
-        b += (double)part[(size_t)blk * 2 * C + C + c];
-      }
-  } else {
 #pragma unroll 1
-    for (int q0 = 0; q0 < MAXQ; q0 += GRP) {
-      float va[GRP], vb[GRP];
+  for (int q0 = 0; q0 < MAXQ; q0 += GRP) {
+    float va[GRP], vb[GRP];
 #pragma unroll
-      for (int j = 0; j < GRP; ++j) {
-        const int blk = part_id + 32 * (q0 + j);
-        const bool ok = c < C && blk < blocks;
-        va[j] = ok ? part[(size_t)blk * 2 * C + c] : 0.f;
-        vb[j] = ok ? part[(size_t)blk * 2 * C + C + c] : 0.f;
-      }
+    for (int j = 0; j < GRP; ++j) {
+      const int blk = part_id + 32 * (q0 + j);
+      const bool ok = c < C && blk < blocks;
+      va[j] = ok ? part[(size_t)blk * 2 * C + c] : 0.f;
+      vb[j] = ok ? part[(size_t)blk * 2 * C + C + c] : 0.f;
+    }
 #pragma unroll
-      for (int j = 0; j < GRP; ++j) {
-        if (c < C && part_id + 32 * (q0 + j) < blocks) {
-          a += (double)va[j];
-          b += (double)vb[j];
-        }
+    for (int j = 0; j < GRP; ++j) {
+      if (c < C && part_id + 32 * (q0 + j) < blocks) {
+        a += (double)va[j];
+        b += (double)vb[j];
       }
     }
   }
@@ -463,13 +449,13 @@ __global__ void __launch_bounds__(1024) bn_finalize_kernel(const float* __restri
                                                           float eps, float momentum, float* __restrict__ running_mean,
                                                           float* __restrict__ running_var, float* __restrict__ mean,
                                                           float* __restrict__ invstd, float* __restrict__ scale,
-                                                          float* __restrict__ shift, int batched) {
+                                                          float* __restrict__ shift) {
   pdl_launch_dependents();
   pdl_wait();
   __shared__ double sh[32][2][32];
   const int c = blockIdx.x * 32 + (threadIdx.x & 31), part_id = threadIdx.x >> 5;
   double s, ss;
-  bn_sum_partials(part, blocks, C, c, part_id, sh, s, ss, batched);
+  bn_sum_partials(part, blocks, C, c, part_id, sh, s, ss);
   if (part_id != 0 || c >= C) return;
   const double m = s / count;
   double var = ss / count - m * m;
@@ -588,13 +574,13 @@ __global__ void __launch_bounds__(1024) bn_bwd_finalize_kernel(const float* __re
                                                               const float* __restrict__ gamma, const float* __restrict__ mean,
                                                               const float* __restrict__ invstd, float grad_unscale,
                                                               float* __restrict__ dgamma, float* __restrict__ dbeta,
-                                                              float* __restrict__ coef, int batched) {
+                                                              float* __restrict__ coef) {
   pdl_launch_dependents();
   pdl_wait();
   __shared__ double sh[32][2][32];
   const int c = blockIdx.x * 32 + (threadIdx.x & 31), part_id = threadIdx.x >> 5;
   double sg, sgx;
-  bn_sum_partials(part, blocks, C, c, part_id, sh, sg, sgx, batched);
+  bn_sum_partials(part, blocks, C, c, part_id, sh, sg, sgx);
   if (part_id != 0 || c >= C) return;
   dbeta[c] = (float)sg * grad_unscale;
   dgamma[c] = (float)sgx * grad_unscale;
@@ -1102,14 +1088,11 @@ int ctl_conv2d_wgrad_nhwc_f16_ex(const void* x, int32_t n, int32_t h, int32_t w,
   if (!attr_set) {
     CTL_CUDA(cudaFuncSetAttribute(conv_wgrad_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WgCfg<64>::SMEM));
     CTL_CUDA(cudaFuncSetAttribute(conv_wgrad_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WgCfg<128>::SMEM));
-    CTL_CUDA(cudaFuncSetAttribute(conv_wgrad_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WgCfg<256>::SMEM));
     attr_set = true;
   }
   cudaStream_t st = (cudaStream_t)stream;
   const int grid = std::min(p.n_items * p.splits, sm_count());
-  if (p.bnw == 256)
-    CTL_CUDA(launch_k(conv_wgrad_kernel<256>, dim3(grid), dim3(WG_THREADS), WgCfg<256>::SMEM, st, p));
-  else if (p.bnw == 128)
+  if (p.bnw == 128)
     CTL_CUDA(launch_k(conv_wgrad_kernel<128>, dim3(grid), dim3(WG_THREADS), WgCfg<128>::SMEM, st, p));
   else
     CTL_CUDA(launch_k(conv_wgrad_kernel<64>, dim3(grid), dim3(WG_THREADS), WgCfg<64>::SMEM, st, p));
@@ -1169,8 +1152,7 @@ int ctl_bn_train_forward_nhwc_f16(const void* y, int64_t rows, int32_t c, int32_
   CTL_CUDA(launch_k(bn_stats_kernel, dim3(g.blocks), dim3(BN_THREADS), sm, st, static_cast<const __half*>(y), (long long)rows,
                     (int)c, (int)pitch, g.rows_per_block, g.lanes, part));
   CTL_CUDA(launch_k(bn_finalize_kernel, dim3((c + 31) / 32), dim3(1024), 0, st, (const float*)part, g.blocks, (int)c,
-                    (double)rows, gamma, beta, eps, momentum, running_mean, running_var, save_mean, save_invstd, scale, shift,
-                    bn_batched()));
+                    (double)rows, gamma, beta, eps, momentum, running_mean, running_var, save_mean, save_invstd, scale, shift));
   CTL_CUDA(launch_k(bn_apply_kernel, dim3(row_grid(rows, g.lanes)), dim3(BN_THREADS), 0, st, static_cast<const __half*>(y),
                     (long long)rows, (int)c, (int)pitch, g.lanes, (const float*)scale, (const float*)shift, static_cast<const __half*>(residual),
                     (int)relu, static_cast<__half*>(out)));
@@ -1196,7 +1178,7 @@ int ctl_bn_train_backward_nhwc_f16(const void* dz, const void* z, const void* y,
                     static_cast<const __half*>(z), static_cast<const __half*>(y), (long long)rows, (int)c, (int)pitch, g.rows_per_block,
                     g.lanes, save_mean, save_invstd, static_cast<__half*>(g_out), part));
   CTL_CUDA(launch_k(bn_bwd_finalize_kernel, dim3((c + 31) / 32), dim3(1024), 0, st, (const float*)part, g.blocks, (int)c,
-                    (double)rows, gamma, save_mean, save_invstd, grad_unscale, dgamma, dbeta, coef, bn_batched()));
+                    (double)rows, gamma, save_mean, save_invstd, grad_unscale, dgamma, dbeta, coef));
   const __half* gsrc = z ? static_cast<const __half*>(g_out) : static_cast<const __half*>(dz);
   CTL_CUDA(launch_k(bn_bwd_apply_kernel, dim3(row_grid(rows, g.lanes)), dim3(BN_THREADS), 0, st, gsrc, static_cast<const __half*>(y),
                     (long long)rows, (int)c, (int)pitch, g.lanes, (const float*)coef, static_cast<__half*>(dy)));

@@ -12,7 +12,6 @@ bn(backbone(x)) of modelling/bases.py:169-177.
 """
 from __future__ import annotations
 
-import os
 from typing import Dict, Optional
 
 import torch
@@ -97,7 +96,6 @@ class TrunkEngine:
                     blk["dual_b"] = (c3.b + cd.b).contiguous()
                 self.blocks.append(blk)
         self.out_channels = self.blocks[-1]["conv3"].cout
-        self.fuse_shortcut = os.environ.get("CTL_FUSE_SHORTCUT", "1") == "1"  # A/B switch (two-launch form when 0)
         self.profile = None  # set to a list to record (kernel, flops, bytes, start_evt, end_evt) per launch
         self.launches_per_forward = 0
         self.head = None
@@ -166,7 +164,7 @@ class TrunkEngine:
         if images_u8.dim() != 4 or images_u8.shape[3] != 3 or images_u8.dtype != torch.uint8:
             raise ValueError(f"expected uint8 [B, H, W, 3], got {images_u8.dtype} {tuple(images_u8.shape)}")
         n, H, W, _ = images_u8.shape
-        if not (H % 4 == 0 and W % 2 == 0 and W <= 128 and os.environ.get("CTL_STEM_FUSED", "1") == "1"):
+        if not (H % 4 == 0 and W % 2 == 0 and W <= 128):
             from ...datasets.transforms import normalize_batch
 
             return self.forward(normalize_batch(images_u8, pixel_mean, pixel_std), want_base, want_emb)
@@ -190,7 +188,7 @@ class TrunkEngine:
         h, w = (H + 6 - 7) // 2 + 1, (W + 6 - 7) // 2 + 1
         hp, wp = (h + 2 - 3) // 2 + 1, (w + 2 - 3) // 2 + 1
         a = torch.empty(n, hp, wp, 64, dtype=torch.float16, device=self.device)
-        if H % 4 == 0 and W % 2 == 0 and W <= 128 and os.environ.get("CTL_STEM_FUSED", "1") == "1":
+        if H % 4 == 0 and W % 2 == 0 and W <= 128:
             # conv1 + bn1 (+ReLU) + maxpool in one pass; only the pooled tensor is written
             pad = self._stem_pad.get((n, H, W))
             if pad is None:
@@ -227,7 +225,7 @@ class TrunkEngine:
                     N.check(L.ctl_instnorm_relu_nhwc_f16(o1.data_ptr(), n, h1 * w1, blk["conv1"].cout, half,
                                                          g.data_ptr(), b.data_ptr(), BN_EPS, N.stream_ptr()))
             o2, h2, w2 = self._conv(o1, n, h1, w1, blk["conv2"])
-            if "down" in blk and self.fuse_shortcut and h % blk["down"].stride == 0 and w % blk["down"].stride == 0:
+            if "down" in blk and h % blk["down"].stride == 0 and w % blk["down"].stride == 0:
                 a, h, w = self._dual(o2, a, n, h, w, h2, w2, blk)
                 continue
             res = a

@@ -15,7 +15,6 @@ GradScaler in the reference's PL trainer) and un-scaled in fp32.  `ibn=True` run
 """
 from __future__ import annotations
 
-import os
 from typing import Dict, List, Optional
 
 import torch
@@ -300,11 +299,7 @@ class TrunkTrainer:
         """weight gradient of s.conv and (optionally) the data gradient w.r.t. s.a (+ residual)."""
         wt = params[s.conv + ".weight"].detach()
         cout, cin, k = wt.shape[0], wt.shape[1], s.k
-        if os.environ.get("CTL_WGRAD_NCHW", "1") == "1":
-            grads[s.conv + ".weight"] = self._wgrad(s.a, s.shape_in, dy, cout, k, s.stride, param_layout=True)
-        else:  # round-1 form (bisect aid): operand layout + torch permute / mul
-            dw = self._wgrad(s.a, s.shape_in, dy, cout, k, s.stride)
-            grads[s.conv + ".weight"] = dw.permute(0, 3, 1, 2).mul(1.0 / self.grad_scale)
+        grads[s.conv + ".weight"] = self._wgrad(s.a, s.shape_in, dy, cout, k, s.stride, param_layout=True)
         if not need_dx:
             return None
         n, h, w = s.shape_in

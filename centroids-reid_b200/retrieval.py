@@ -332,10 +332,8 @@ def _finalize_and_read_back(buckets, count, nq, max_pos, ovf):
 
 def _tile_lists_enabled(qp: Planes, gp: Planes) -> bool:
     """Tile lists (ctl_pass_desc.tile_list) pay off when BOTH operands are stored in identity order (then few tiles can
-    hold a positive); off with CTL_RETRIEVAL_TILE_LISTS=0 (bisect aid)."""
-    import os
-
-    return os.environ.get("CTL_RETRIEVAL_TILE_LISTS", "1") != "0" and qp.order is not None and gp.order is not None
+    hold a positive)."""
+    return qp.order is not None and gp.order is not None
 
 
 def _tile_list(qp: Planes, gp: Planes, ids: "EncodedIds", keep_stride: int) -> Optional[torch.Tensor]:

@@ -141,8 +141,6 @@ typedef struct ctl_pass_desc {
 } ctl_pass_desc;
 int ctl_dist_pass(const void* q_planes, int64_t nq, const void* g_planes, int64_t ng, int32_t d, int32_t flags,
                   const ctl_pass_desc* desc, ctl_stream_t stream);
-/* debug aid: per-CTA epilogue cycle counters [grid][2][8] written by the following ctl_dist_pass calls */
-void ctl_debug_set_dist_profile(long long* device_buffer);
 /* top-k plan for (ng, k): emit_all != 0 means "skip pass 1, tau = +inf". */
 int ctl_topk_plan(int64_t ng, int32_t k, int32_t* emit_all, int32_t* n_groups, int32_t* merge, int32_t* cand_cap);
 int ctl_select_tau(const float* gmin, int64_t nq, int32_t n_groups, int32_t merge, int32_t k, float* tau,
@@ -239,7 +237,6 @@ int ctl_xent_smooth_step(const float* logits, int32_t b, int32_t c, const int32_
  *              ReLU (if relu != 0) is applied to output channels >= relu_from only (IBN: the
  *              InstanceNorm half of bn1 is left raw for ctl_instnorm_relu);
  *   stem     : conv 7x7/2 pad 3 (3 -> 64) + folded BN [+ ReLU] from NCHW fp32 to NHWC fp16;
- *              weight_k64 = [147][64] fp32 with k = (c*7 + r)*7 + s;
  *   maxpool  : 3x3 / 2, pad 1;
  *   gap_bn   : feat = mean over H*W (fp32), emb = feat * bn_scale + bn_shift (eval BatchNorm1d);
  *   instnorm : per-(image, channel) InstanceNorm(affine) + ReLU in place on channels [0, half).
@@ -256,8 +253,6 @@ int ctl_conv2d_nhwc_f16(const void* x, int32_t n, int32_t h, int32_t w, int32_t 
 int ctl_conv1x1_dual_nhwc_f16(const void* x1, int32_t cin1, const void* x2, int32_t h2, int32_t w2, int32_t cin2,
                               int32_t stride2, int32_t n, const void* weight_cat, const float* bias, void* out,
                               int32_t cout, int32_t relu, ctl_stream_t stream);
-int ctl_stem_conv7x7(const float* x_nchw, int32_t n, int32_t h, int32_t w, const float* weight_k64, const float* bias,
-                     int32_t relu, void* out_nhwc_f16, ctl_stream_t stream);
 /* tensor-core stem: weight_k192_f16 = [64][192] fp16, k = (c*7 + r)*8 + s (s = 7 and k >= 168 zero) */
 int ctl_stem_conv7x7_tc(const float* x_nchw, int32_t n, int32_t h, int32_t w, const void* weight_k192_f16,
                         const float* bias, int32_t relu, void* out_nhwc_f16, ctl_stream_t stream);

@@ -164,6 +164,30 @@ def test_ctl_model_under_a_lightning_like_base(monkeypatch):
         importlib.reload(M)
 
 
+def test_runtime_switches_are_the_known_ones():
+    """Every environment variable the package reads.  An A/B switch left in a kernel or engine is a second code path
+    nobody runs; a new read must be added here on purpose."""
+    allowed = {
+        ("csrc/common.h", "CTL_PDL"),  # rules out launch-overlap ordering when diagnosing a fault
+        ("modelling/baseline.py", "CTL_TRAIN_GRAPHS"),
+        ("modelling/baseline.py", "CTL_DYNAMIC_LOSS_SCALE"),
+        ("modelling/ctl_model.py", "CTL_VALIDATE_BATCH"),
+    }
+    pkg = os.path.join(ROOT, "centroids-reid_b200")
+    found = set()
+    for dirpath, _, names in os.walk(pkg):
+        for name in names:
+            if not name.endswith((".py", ".cu", ".cuh", ".h")):
+                continue
+            path = os.path.join(dirpath, name)
+            rel = os.path.relpath(path, pkg).replace(os.sep, "/")
+            for line in open(path, encoding="utf-8"):
+                if "getenv(" in line or "os.environ" in line:
+                    m = re.search(r"(?:getenv\(|os\.environ(?:\.get\(|\[))\s*[\"'](\w+)[\"']", line)
+                    found.add((rel, m.group(1) if m else line.strip()))
+    assert found == allowed, found ^ allowed
+
+
 def test_no_undefined_names_in_the_python_sources():
     """GPU-only branches (sharded retrieval, NCCL paths) are not executed by the CPU suite: a static scan keeps a typo in them
     from surviving until a GPU run (tools/undefined_names.py: names loaded in a function that are bound nowhere)."""

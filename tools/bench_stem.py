@@ -19,4 +19,4 @@ e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=Tr
 e0.record()
 for i in range(20): run(i)
 e1.record(); torch.cuda.synchronize()
-print(f"dbg={os.environ.get('CTL_STEM_DEBUG','0')}: pack+stem_pool {e0.elapsed_time(e1)/20*1e3:.1f} us")
+print(f"pack+stem_pool {e0.elapsed_time(e1)/20*1e3:.1f} us")

@@ -47,15 +47,4 @@ buckets = torch.zeros(nq, ids.max_pos + 1, dtype=torch.int32, device="cuda")
 print("pass count                %.3f ms" % gpu_ms(N.PassDesc(thr_keys=pos_keys.data_ptr(), thr_count=pos_count.data_ptr(), buckets=buckets.data_ptr(), **idk)))
 tau = torch.full((nq,), 1.9, device="cuda"); cand = torch.empty(nq, 4096, dtype=torch.int64, device="cuda"); cc = torch.zeros(nq, dtype=torch.int32, device="cuda")
 print("pass cand(tau=1.9)+count  %.3f ms" % gpu_ms(N.PassDesc(tau=tau.data_ptr(), cand_keys=cand.data_ptr(), cand_count=cc.data_ptr(), cand_cap=4096, overflow=ovf.data_ptr(), thr_keys=pos_keys.data_ptr(), thr_count=pos_count.data_ptr(), buckets=buckets.data_ptr(), **idk)))
-PH = ["tile_setup", "mma_and_stage", "bar_meta", "acc_read", "element_loop", "tile_end", "-", "-"]
-def phases(name, desc):
-    prof = torch.zeros(148 * 2 * 8, dtype=torch.int64, device="cuda")
-    L.ctl_debug_set_dist_profile(prof.data_ptr())
-    N.check(L.ctl_dist_pass(qp.ptr, nq, gp.ptr, ng, 2048, qp.flags, C.byref(desc), N.stream_ptr()))
-    torch.cuda.synchronize()
-    L.ctl_debug_set_dist_profile(None)
-    pm = prof.view(148, 2, 8).double().mean(0)
-    print(name, "| thread A:", ", ".join(f"{PH[i]}={pm[0, i].item():.0f}" for i in range(6)), "| thread B:", ", ".join(f"{PH[i]}={pm[1, i].item():.0f}" for i in range(6)))
-phases("gmin", N.PassDesc(gmin=gmin.data_ptr()))
-phases("count", N.PassDesc(thr_keys=pos_keys.data_ptr(), thr_count=pos_count.data_ptr(), buckets=buckets.data_ptr(), **idk))
 print("dist_matrix (1 pass)     %.3f ms" % T(lambda: R.dist_matrix(q, g)))
