@@ -113,7 +113,8 @@ __global__ void loss_scale_update_kernel(float* __restrict__ state, int* __restr
     scale *= backoff;
     *tracker = 0;
   } else if (++(*tracker) >= interval) {
-    scale *= growth;
+    const float grown = scale * growth;
+    if (isfinite(grown)) scale = grown;  // like GradScaler: a growth that would overflow keeps the current scale
     *tracker = 0;
   }
   state[0] = scale;

@@ -358,10 +358,16 @@ __device__ __forceinline__ void bn_block_store(float (&acc)[NQ][8], int group, i
   }
 }
 
-// pass A of the forward: per-block sum and sum of squares of y
+// pass A of the forward: per-block sum and sum of squares of y - p, p = the channel's value in one row (`pivot`).
+// Summing y and y^2 directly and forming E[y^2] - mean^2 cancels catastrophically when |mean| >> std (fp32 partials of
+// y^2 lose the variance); shifted by a sample of the channel the sums stay of the order of the variance.  The fp32
+// partial error is still amplified by 1 + (p - mean)^2 / var: about 1-10 for a sample of a bell-shaped channel, but a pivot
+// row that is a far outlier of its channel brings the cancellation back (unlike the Welford InstanceNorm statistics
+// below, which are robust; here they would need the (count, mean, M2) triples carried through bn_block_store and the
+// double-precision finalize).
 __global__ void __launch_bounds__(BN_THREADS) bn_stats_kernel(const __half* __restrict__ y, long long rows, int C, int pitch,
                                                               long long rows_per_block, int lanes,
-                                                              float* __restrict__ part) {
+                                                              const __half* __restrict__ pivot, float* __restrict__ part) {
   pdl_launch_dependents();
   pdl_wait();
   extern __shared__ float sred[];
@@ -371,6 +377,8 @@ __global__ void __launch_bounds__(BN_THREADS) bn_stats_kernel(const __half* __re
 #pragma unroll
   for (int i = 0; i < 8; ++i) acc[0][i] = acc[1][i] = 0.f;
   if (lane_row < lanes) {
+    float piv[8];
+    unpack8(*reinterpret_cast<const uint4*>(pivot + group * 8), piv);
     const long long r0 = (long long)blockIdx.x * rows_per_block, r1 = min(rows, r0 + rows_per_block);
     long long r = r0 + lane_row;
     for (; r + 3LL * lanes < r1; r += 4LL * lanes) {  // four independent 16-byte loads in flight per thread
@@ -383,8 +391,9 @@ __global__ void __launch_bounds__(BN_THREADS) bn_stats_kernel(const __half* __re
         unpack8(v[u], f);
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-          acc[0][i] += f[i];
-          acc[1][i] = fmaf(f[i], f[i], acc[1][i]);
+          const float d = f[i] - piv[i];
+          acc[0][i] += d;
+          acc[1][i] = fmaf(d, d, acc[1][i]);
         }
       }
     }
@@ -393,8 +402,9 @@ __global__ void __launch_bounds__(BN_THREADS) bn_stats_kernel(const __half* __re
       unpack8(*reinterpret_cast<const uint4*>(y + r * pitch + group * 8), f);
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
-        acc[0][i] += f[i];
-        acc[1][i] = fmaf(f[i], f[i], acc[1][i]);
+        const float d = f[i] - piv[i];
+        acc[0][i] += d;
+        acc[1][i] = fmaf(d, d, acc[1][i]);
       }
     }
   }
@@ -443,8 +453,10 @@ __device__ __forceinline__ void bn_sum_partials(const float* __restrict__ part, 
 }
 
 // finalize of the forward: batch mean / biased variance -> invstd, scale = gamma*invstd, shift = beta - mean*scale;
-// running statistics updated like torch (momentum, unbiased variance).  grid = C / 32 blocks of 1024 threads.
+// running statistics updated like torch (momentum, unbiased variance).  The partials are sums of y - pivot
+// (bn_stats_kernel); the pivot row is read here again.  grid = C / 32 blocks of 1024 threads.
 __global__ void __launch_bounds__(1024) bn_finalize_kernel(const float* __restrict__ part, int blocks, int C, double count,
+                                                          const __half* __restrict__ pivot,
                                                           const float* __restrict__ gamma, const float* __restrict__ beta,
                                                           float eps, float momentum, float* __restrict__ running_mean,
                                                           float* __restrict__ running_var, float* __restrict__ mean,
@@ -457,8 +469,9 @@ __global__ void __launch_bounds__(1024) bn_finalize_kernel(const float* __restri
   double s, ss;
   bn_sum_partials(part, blocks, C, c, part_id, sh, s, ss);
   if (part_id != 0 || c >= C) return;
-  const double m = s / count;
-  double var = ss / count - m * m;
+  const double d = s / count;  // mean - pivot
+  const double m = (double)__half2float(pivot[c]) + d;
+  double var = ss / count - d * d;
   if (var < 0.0) var = 0.0;
   const float is = (float)(1.0 / sqrt(var + (double)eps));
   mean[c] = (float)m;
@@ -652,6 +665,42 @@ __device__ __forceinline__ void in_block_reduce(float (&acc)[2][8], float* sred 
   __syncthreads();
 }
 
+// Block reduction of per-thread (count, mean, M2 = sum of squared deviations) of 8 channels by Chan's pairwise update,
+// in a fixed tree order (deterministic).  Returns the block's mean and M2 to every thread.
+__device__ __forceinline__ void in_block_welford(float cnt, float (&mean)[8], float (&m2)[8], float* sred /* [256][16] */,
+                                                 float* scnt /* [256] */) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    sred[threadIdx.x * 16 + i] = mean[i];
+    sred[threadIdx.x * 16 + 8 + i] = m2[i];
+  }
+  scnt[threadIdx.x] = cnt;
+  __syncthreads();
+  for (int off = 128; off > 0; off >>= 1) {
+    const int t = threadIdx.x;
+    if (t < off && scnt[t + off] > 0.f) {
+      const float na = scnt[t], nb = scnt[t + off], nab = na + nb, wb = nb * __frcp_rn(nab);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const float ma = sred[t * 16 + i], d = sred[(t + off) * 16 + i] - ma;
+        sred[t * 16 + i] = fmaf(d, wb, ma);
+        sred[t * 16 + 8 + i] += sred[(t + off) * 16 + 8 + i] + d * d * na * wb;
+      }
+      scnt[t] = nab;
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    mean[i] = sred[i];
+    m2[i] = sred[8 + i];
+  }
+  __syncthreads();
+}
+
+// statistics in ONE pass over the instance with Welford's update per thread and Chan's combination across threads (the
+// update PyTorch's own normalisation kernels use), not E[y^2] - mean^2, which cancels catastrophically in fp32 when
+// |mean| >> std
 __global__ void __launch_bounds__(256) in_train_forward_kernel(const __half* __restrict__ y, int HW, int pitch, int half,
                                                                const float* __restrict__ gamma, const float* __restrict__ beta,
                                                                float eps, float* __restrict__ save_mean,
@@ -659,31 +708,34 @@ __global__ void __launch_bounds__(256) in_train_forward_kernel(const __half* __r
   pdl_launch_dependents();
   pdl_wait();
   __shared__ float sred[256 * 16];
+  __shared__ float scnt[256];
   const int g = blockIdx.x, n = blockIdx.y;
   const size_t base = (size_t)n * HW * pitch + g * 8;
-  float acc[2][8], tot[2][8];
+  float cnt = 0.f, m[8], m2[8];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) acc[0][i] = acc[1][i] = 0.f;
+  for (int i = 0; i < 8; ++i) m[i] = m2[i] = 0.f;
   for (int r = threadIdx.x; r < HW; r += blockDim.x) {
     float f[8];
     unpack8(*reinterpret_cast<const uint4*>(y + base + (size_t)r * pitch), f);
+    cnt += 1.f;
+    const float inv = __frcp_rn(cnt);
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-      acc[0][i] += f[i];
-      acc[1][i] = fmaf(f[i], f[i], acc[1][i]);
+      const float d = f[i] - m[i];
+      m[i] = fmaf(d, inv, m[i]);
+      m2[i] = fmaf(d, f[i] - m[i], m2[i]);
     }
   }
-  in_block_reduce(acc, sred, tot);
+  in_block_welford(cnt, m, m2, sred, scnt);
   float sc[8], sh[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
-    const float m = tot[0][i] / HW;
-    const float var = fmaxf(tot[1][i] / HW - m * m, 0.f);
+    const float var = m2[i] / HW;
     const float is = rsqrtf(var + eps);
     sc[i] = gamma[g * 8 + i] * is;
-    sh[i] = beta[g * 8 + i] - m * sc[i];
+    sh[i] = beta[g * 8 + i] - m[i] * sc[i];
     if (threadIdx.x == 0) {
-      save_mean[(size_t)n * half + g * 8 + i] = m;
+      save_mean[(size_t)n * half + g * 8 + i] = m[i];
       save_invstd[(size_t)n * half + g * 8 + i] = is;
     }
   }
@@ -1149,10 +1201,14 @@ int ctl_bn_train_forward_nhwc_f16(const void* y, int64_t rows, int32_t c, int32_
   float* shift = scale + c;
   cudaStream_t st = (cudaStream_t)stream;
   const size_t sm = (size_t)g.lanes * 2 * c * sizeof(float);
+  // the pivot is the slice's last row.  Any row serves equally well numerically; the row changes the last bits of the
+  // statistics and, through the ReLU masks, of every training gradient -- see the margin note on
+  // tests/test_reference_autocast_gpu.py::test_training_step_at_bench_shape_vs_reference_cuda_autocast
+  const __half* pivot = static_cast<const __half*>(y) + (size_t)(rows - 1) * pitch;
   CTL_CUDA(launch_k(bn_stats_kernel, dim3(g.blocks), dim3(BN_THREADS), sm, st, static_cast<const __half*>(y), (long long)rows,
-                    (int)c, (int)pitch, g.rows_per_block, g.lanes, part));
+                    (int)c, (int)pitch, g.rows_per_block, g.lanes, pivot, part));
   CTL_CUDA(launch_k(bn_finalize_kernel, dim3((c + 31) / 32), dim3(1024), 0, st, (const float*)part, g.blocks, (int)c,
-                    (double)rows, gamma, beta, eps, momentum, running_mean, running_var, save_mean, save_invstd, scale, shift));
+                    (double)rows, pivot, gamma, beta, eps, momentum, running_mean, running_var, save_mean, save_invstd, scale, shift));
   CTL_CUDA(launch_k(bn_apply_kernel, dim3(row_grid(rows, g.lanes)), dim3(BN_THREADS), 0, st, static_cast<const __half*>(y),
                     (long long)rows, (int)c, (int)pitch, g.lanes, (const float*)scale, (const float*)shift, static_cast<const __half*>(residual),
                     (int)relu, static_cast<__half*>(out)));

@@ -59,6 +59,12 @@ def test_eval_embedding_at_bench_shape_vs_reference_cuda_autocast(tag, ibn, hw, 
     assert e_f32 <= max(3.0 * own, 1.5e-3)
 
 
+# Margin note (measured on an H100 80GB HBM3): at config 4 the norm check of the IBN-a InstanceNorm bias gradients sits
+# close to its 6 % bound.  Those gradients are sums over ~800k positions that almost cancel, so last-bit changes to any
+# training kernel move them through the ReLU masks: the reference's own autocast run is up to 4.5 % from its fp32 run on
+# them, and of two equally valid BatchNorm pivot rows the first put layer1.0.bn1.IN.bias at 6.7 % while the last (the
+# committed kernel) passes.  A failure here after a change of rounding is not by itself a wrong kernel;
+# check the change against float64 first (tests/test_train_kernels_gpu.py), and do not pick numerics by this outcome.
 @pytest.mark.parametrize("tag,ibn,hw,P,K", [("r50 cfg2", False, (256, 128), 16, 16), ("ibn cfg4/gpu", True, (320, 320), 32, 4)])
 def test_training_step_at_bench_shape_vs_reference_cuda_autocast(tag, ibn, hw, P, K):
     from ctl_b200.modelling.backbones.engine_train import TrunkTrainer
