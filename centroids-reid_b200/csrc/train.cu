@@ -28,6 +28,7 @@ struct ConvTapW {
 static constexpr int WG_THREADS = 384;
 static constexpr int WG_BOX_BYTES = 128 * 64 * 2;  // one [128 px][64 ch] box
 static constexpr uint32_t WG_PRODUCER_REGS = 40, WG_CONSUMER_REGS = 232;
+static constexpr int WG_CHAIN_TILES = 8;  // pixel tiles per wgmma accumulation chain: 64 k16 steps (see the consumer)
 // N (cin per work item) = 64 or 128: the wider the item, the more MMA work one dy tile feeds (less TMA fill per
 // flop), the shallower the ring that fits in shared memory
 template <int BNW>
@@ -138,7 +139,17 @@ __global__ void __launch_bounds__(WG_THREADS, 1) conv_wgrad_kernel(const __grid_
     const bool wg_leader = (threadIdx.x & 127) == 0;
     const int row0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // cout inside the 128-channel tile
     const int ktot = p.n_taps * p.cin;
-    float acc[BNW / 2];
+    // wgmma's fp32 accumulation does not round like IEEE addition: on same-sign terms its error grows with the chain
+    // length C (about C * 2^-24 * sum |terms|, measured on an H100), not with sqrt(C).  So a unit runs as chains of
+    // WG_CHAIN_TILES pixel tiles (8 k16 steps each), and each finished chain is added to `sum` with ordinary FADDs.
+    float acc[BNW / 2], sum[BNW / 2];
+    auto fold = [&](bool first) {  // sum (+)= acc once the chain's wgmma groups have completed
+#pragma unroll
+      for (int i = 0; i < BNW / 2; ++i) {
+        asm volatile("" : "+f"(acc[i])::"memory");  // keep the reads after wgmma_wait
+        sum[i] = first ? acc[i] : sum[i] + acc[i];
+      }
+    };
     int stage = 0;
     uint32_t phase = 0;
     for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
@@ -148,6 +159,7 @@ __global__ void __launch_bounds__(WG_THREADS, 1) conv_wgrad_kernel(const __grid_
       const int split = u - item * p.splits;
       int held = -1;
       for (int t = t0; t < t1; ++t) {
+        const int c = (t - t0) % WG_CHAIN_TILES;  // tile index inside the current chain
         mbar_wait(full_bar(stage), phase);
         const uint32_t a0 = smem_base + stage * WG_STAGE_BYTES + wg * WG_BOX_BYTES, b0 = smem_base + stage * WG_STAGE_BYTES + 2 * WG_BOX_BYTES;
         wgmma_fence();
@@ -155,7 +167,7 @@ __global__ void __launch_bounds__(WG_THREADS, 1) conv_wgrad_kernel(const __grid_
         for (int k = 0; k < 8; ++k) {  // 16 pixels (rows) per MMA
           const uint64_t da = make_sw128_mnmajor_desc(a0 + k * 2048, WG_BOX_BYTES);
           const uint64_t db = make_sw128_mnmajor_desc(b0 + k * 2048, WG_BOX_BYTES);
-          wgmma_f16<BNW, 1, 1>(acc, da, db, (t > t0 || k > 0) ? 1u : 0u);
+          wgmma_f16<BNW, 1, 1>(acc, da, db, (c > 0 || k > 0) ? 1u : 0u);
         }
         wgmma_commit();
         wgmma_wait<1>();
@@ -165,15 +177,20 @@ __global__ void __launch_bounds__(WG_THREADS, 1) conv_wgrad_kernel(const __grid_
           stage = 0;
           phase ^= 1u;
         }
+        if (c == WG_CHAIN_TILES - 1 && t + 1 < t1) {
+          wgmma_wait<0>();
+          fold(t - t0 < WG_CHAIN_TILES);
+        }
       }
       wgmma_wait<0>();
       if (held >= 0 && wg_leader) mbar_arrive(empty_bar(held));
+      fold(t1 - t0 <= WG_CHAIN_TILES);
       float* dst = p.part + ((size_t)split * p.cout_pad + ct * 128 + row0) * ktot + tapi * p.cin + chunk * BNW + 2 * (lane & 3);
 #pragma unroll
       for (int j = 0; j < BNW / 8; ++j)
 #pragma unroll
         for (int h = 0; h < 2; ++h)
-          *reinterpret_cast<float2*>(dst + (size_t)(8 * h) * ktot + 8 * j) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+          *reinterpret_cast<float2*>(dst + (size_t)(8 * h) * ktot + 8 * j) = make_float2(sum[4 * j + 2 * h], sum[4 * j + 2 * h + 1]);
     }
   }
 }
@@ -288,6 +305,11 @@ static int wgrad_plan(int n, int h, int w, int cin, int cout, int ksize, int str
   const int want = (2 * sm_count() + p->n_items - 1) / p->n_items;
   p->splits = std::max(1, std::min(want, p->m_tiles));
   return Ho * 65536 + Wo;
+}
+
+// the bytes ctl_conv2d_wgrad_workspace_bytes reports and the launch requires: the partial tiles plus 256 bytes of slack
+static size_t wgrad_workspace_need(const WgradParams& p) {
+  return (size_t)p.splits * p.cout_pad * p.n_taps * p.cin * sizeof(float) + 256;
 }
 
 
@@ -1059,11 +1081,11 @@ extern "C" {
 size_t ctl_conv2d_wgrad_workspace_bytes(int32_t n, int32_t h, int32_t w, int32_t cin, int32_t cout, int32_t ksize,
                                         int32_t stride) {
   if (n < 1 || h < 1 || w < 1 || cin % 64 != 0 || cout % 64 != 0 || (ksize != 1 && ksize != 3) ||
-      (stride != 1 && stride != 2))
+      (stride != 1 && stride != 2) || (stride == 2 && (h % 2 != 0 || w % 2 != 0)))
     return 0;
   WgradParams p = {};
   wgrad_plan(n, h, w, cin, cout, ksize, stride, &p);
-  return (size_t)p.splits * p.cout_pad * p.n_taps * cin * sizeof(float) + 256;
+  return wgrad_workspace_need(p);
 }
 
 int ctl_conv2d_wgrad_nhwc_f16(const void* x, int32_t n, int32_t h, int32_t w, int32_t cin, const void* dy, int32_t cout,
@@ -1096,7 +1118,7 @@ int ctl_conv2d_wgrad_nhwc_f16_ex(const void* x, int32_t n, int32_t h, int32_t w,
   WgradParams p = {};
   const int hw = wgrad_plan(n, h, w, cin, cout, ksize, stride, &p);
   const int Ho = hw >> 16, Wo = hw & 65535;
-  const size_t need = (size_t)p.splits * p.cout_pad * p.n_taps * cin * sizeof(float);
+  const size_t need = wgrad_workspace_need(p);
   CTL_CHECK_ARG(workspace_bytes >= need, "workspace too small: %zu < %zu", workspace_bytes, need);
   CTL_CHECK_ARG((reinterpret_cast<uintptr_t>(workspace) & 15u) == 0 && (reinterpret_cast<uintptr_t>(dw) & 15u) == 0,
                 "workspace and dw must be 16-byte aligned");
