@@ -102,12 +102,13 @@ SIGNATURES = {
     "ctl_weights_pack": (C.c_int, [_p, C.POINTER(NamedTensor), _i32, _p]),
     "ctl_embed_workspace_bytes": (_sz, [_p, _i32, _i32, _i32]),
     "ctl_embed_forward": (C.c_int, [_p, _p, _i32, _i32, _i32, _p, _p, _p, _sz, _p]),
-    "ctl_trainer_create": (C.c_int, [C.POINTER(_p), _i32, _i32, C.c_float]),
+    "ctl_trainer_create": (C.c_int, [C.POINTER(_p), _i32, _i32, C.c_float, C.POINTER(_i32)]),
     "ctl_trainer_destroy": (None, [_p]),
     "ctl_trainer_bind": (C.c_int, [_p, C.POINTER(NamedTensor), _i32, C.POINTER(NamedTensor), _i32]),
     "ctl_train_workspace_bytes": (_sz, [_p, _i32, _i32, _i32]),
     "ctl_train_forward": (C.c_int, [_p, _p, _i32, _i32, _i32, _p, _p, _sz, _p]),
     "ctl_train_backward": (C.c_int, [_p, _p, C.c_float, _p, _sz, _p]),
+    "ctl_train_saved": (C.c_int, [_p, _i32, C.POINTER(_p), C.POINTER(_p), C.POINTER(_i32)]),
     "ctl_stem_conv7x7_tc": (C.c_int, [_p, _i32, _i32, _i32, _p, _p, _i32, _p, _p]),
     "ctl_stem_pad_bytes": (C.c_size_t, [_i32, _i32, _i32]),
     "ctl_stem_pool_fused": (C.c_int, [_p, _i32, _i32, _i32, _p, _p, _p, _i32, _p, _p]),

@@ -1,11 +1,14 @@
 // Train-mode trunk behind the C ABI (SURVEY 8b, the "train fwd/bwd variants" of the whole-trunk entry points): what torch
 // autograd does through ResNet.forward / ResNet_IBN.forward in train mode (modelling/backbones/resnet.py:67-87,122-133,
 // resnet_ibn_a.py:18-32,126-141) and Baseline.forward's global average pool (modelling/baseline.py:91-96), as ONE forward
-// call and ONE backward call on an opaque handle.  A host that is not Python runs a training step as
-//   ctl_trainer_bind -> ctl_train_forward -> (its loss on global_feat, ctl_ctl_loss_step) -> ctl_train_backward ->
+// call and ONE backward call on an opaque handle.  A training step is
+//   ctl_trainer_bind -> ctl_train_forward -> (the loss on global_feat, ctl_ctl_loss_step) -> ctl_train_backward ->
 //   ctl_adam_multi_step
-// without re-implementing modelling/backbones/engine_train.py.  The launches are the same C entry points engine_train.py
-// issues, in the same order, on the same shapes -- the two drivers produce the same bits (tests/test_train_gpu.py).
+// This is the only driver of the training trunk: modelling/backbones/engine_train.py::TrunkTrainer is its ctypes form.
+// The forward walks the stem, then every bottleneck (conv1, conv2, downsample, conv3) through the conv / BatchNorm
+// entry points; the backward walks the blocks in reverse: BN backward, weight gradient, data gradient through the
+// transposed convolution (stride-2 layers via zero-insertion upsampling), the shortcut's gradient added through
+// conv1's residual input, and the stem's weight gradient as an im2col GEMM.
 //
 // Memory: everything lives in the caller's workspace of ctl_train_workspace_bytes(...) bytes, carved by a bump allocator
 // that is walked once "dry" (no launches) to size it.  The forward keeps y (raw conv output) and z (normalised output) of
@@ -94,7 +97,7 @@ struct TrainBlock {
 struct ctl_trainer {
   int ibn = 0, last_stride = 1;
   float momentum = 0.1f;
-  bool bound = false, forwarded = false;
+  bool bound = false, forwarded = false, saved = false;  // saved: the last forward completed (ctl_train_saved)
   std::vector<ctl::TrainBlock> blocks;
   // stem
   const float *w0 = nullptr, *g0 = nullptr, *b0 = nullptr;
@@ -168,7 +171,7 @@ static int bind_conv(ConvSpec& c, const RefMap& p, const RefMap& g) {
   return rc;
 }
 
-// conv (raw fp16 output) -> batch statistics -> z = [relu](gamma * xhat + beta [+ residual])   (engine_train.py::_conv_bn)
+// conv (raw fp16 output) -> batch statistics -> z = [relu](gamma * xhat + beta [+ residual]); y and z stay saved
 static int conv_bn_forward(ctl_trainer* t, ConvSpec& c, Bump& ws, void* bn_ws, size_t bn_ws_bytes, size_t* bn_need, const void* a, int n,
                            int h, int w, const void* residual, cudaStream_t st) {
   const int pad = c.k == 3 ? 1 : 0;
@@ -234,7 +237,8 @@ static int bn_backward(ctl_trainer* t, ConvSpec& c, Bump& ws, void* bn_ws, size_
 }
 
 // weight gradient of `c` (parameter layout, un-scaled) and, when `dx_out`, the data gradient w.r.t. its input (+ residual)
-// written to *dx_out (a caller buffer) or fresh scratch (engine_train.py::_conv_bwd)
+// written to *dx_out (a caller buffer) or fresh scratch.  The data gradient is the forward conv kernel on dy with the
+// transposed / flipped weights (wd); stride 2 goes through zero-insertion upsampling
 static int conv_backward(ctl_trainer* t, ConvSpec& c, Bump& ws, void* wg_ws, size_t wg_ws_bytes, size_t* wg_need, const void* dy,
                          float inv_scale, bool need_dx, const void* residual, void* dx_buffer, void** dx_out, cudaStream_t st) {
   const size_t need = ctl_conv2d_wgrad_workspace_bytes(c.n, c.h, c.w_in, c.cin, c.cout, c.k, c.stride);
@@ -409,18 +413,20 @@ using namespace ctl;
 
 extern "C" {
 
-int ctl_trainer_create(ctl_trainer** out, int32_t ibn, int32_t last_stride, float momentum) {
-  CTL_CHECK_ARG(out != nullptr, "null pointer");
+int ctl_trainer_create(ctl_trainer** out, int32_t ibn, int32_t last_stride, float momentum, const int32_t stage_blocks[4]) {
+  CTL_CHECK_ARG(out != nullptr && stage_blocks != nullptr, "null pointer");
   CTL_CHECK_ARG(last_stride == 1 || last_stride == 2, "last_stride must be 1 or 2 (config/defaults.py:24)");
   CTL_CHECK_ARG(momentum > 0.f && momentum <= 1.f, "momentum must be in (0, 1]");
+  for (int li = 0; li < 4; ++li)
+    CTL_CHECK_ARG(stage_blocks[li] >= 1, "stage_blocks[%d] = %d: every stage needs at least one block", li, stage_blocks[li]);
   ctl_trainer* t = new ctl_trainer();
   t->ibn = ibn ? 1 : 0;
   t->last_stride = last_stride;
   t->momentum = momentum;
-  const int planes[4] = {64, 128, 256, 512}, nblk[4] = {3, 4, 6, 3};
+  const int planes[4] = {64, 128, 256, 512};
   int inplanes = 64;
   for (int li = 0; li < 4; ++li)
-    for (int bi = 0; bi < nblk[li]; ++bi) {
+    for (int bi = 0; bi < stage_blocks[li]; ++bi) {
       TrainBlock b;
       const std::string p = "layer" + std::to_string(li + 1) + "." + std::to_string(bi);
       const int stride0 = li == 0 ? 1 : (li == 3 ? last_stride : 2);
@@ -513,7 +519,7 @@ int ctl_trainer_bind(ctl_trainer* t, const ctl_named_tensor* params, int32_t n_p
   size_t off = 0;
   long long chunks = 0;
   for (TrainBlock& b : t->blocks) {
-    // table order == engine_train.py's (state_dict order: conv1, conv2, conv3, downsample.0)
+    // table order: state_dict order (conv1, conv2, conv3, downsample.0)
     ConvSpec* cs[4] = {&b.c1, &b.c2, &b.c3, b.has_down ? &b.down : nullptr};
     for (ConvSpec* c : cs) {
       if (!c) continue;
@@ -564,7 +570,7 @@ int ctl_train_forward(ctl_trainer* t, const float* x_nchw, int32_t n, int32_t he
   ws.cap = l.total - l.bn_bytes - l.wg_bytes;
   ws.dry = false;
   Plan plan;
-  t->forwarded = false;
+  t->forwarded = t->saved = false;
   t->x = x_nchw;
   t->n = n;
   t->H = height;
@@ -576,13 +582,40 @@ int ctl_train_forward(ctl_trainer* t, const float* x_nchw, int32_t n, int32_t he
   t->lay_wg = l.wg_bytes;
   t->lay_total = l.total;
   t->fwd_workspace = workspace;
-  t->forwarded = true;
+  t->forwarded = t->saved = true;
   return 0;
 }
 
+int ctl_train_saved(const ctl_trainer* t, int32_t index, const void** y, const void** z, int32_t nhwc[4]) {
+  CTL_CHECK_ARG(t && y && z && nhwc, "null pointer");
+  CTL_CHECK_ARG(t->saved, "ctl_train_saved needs a completed ctl_train_forward");
+  if (index == 0) {
+    *y = t->y0;
+    *z = t->z0;
+    const int32_t s[4] = {t->n, (t->H + 6 - 7) / 2 + 1, (t->W + 6 - 7) / 2 + 1, 64};
+    memcpy(nhwc, s, sizeof(s));
+    return 0;
+  }
+  int32_t i = 1;
+  for (const TrainBlock& b : t->blocks) {
+    const ConvSpec* cs[4] = {&b.c1, &b.c2, b.has_down ? &b.down : nullptr, &b.c3};  // forward order
+    for (const ConvSpec* c : cs) {
+      if (!c || i++ != index) continue;
+      *y = c->y;
+      *z = c->z;
+      const int32_t s[4] = {c->n, c->ho, c->wo, c->cout};
+      memcpy(nhwc, s, sizeof(s));
+      return 0;
+    }
+  }
+  set_error("ctl_train_saved: index %d is outside [0, %d)", index, i);
+  return CTL_ERR_INVALID_ARGUMENT;
+}
+
 int ctl_train_backward(ctl_trainer* t, const float* dfeat, float grad_scale, void* workspace, size_t workspace_bytes, ctl_stream_t stream) {
-  CTL_CHECK_ARG(t && dfeat && workspace, "null pointer");
+  CTL_CHECK_ARG(t != nullptr, "null pointer");
   CTL_CHECK_ARG(t->forwarded, "ctl_train_backward needs the ctl_train_forward of the same step (same workspace, same input)");
+  CTL_CHECK_ARG(dfeat && workspace, "null pointer");
   CTL_CHECK_ARG(grad_scale > 0.f, "grad_scale must be positive");
   CTL_CHECK_ARG(workspace == t->fwd_workspace && workspace_bytes >= t->lay_total,
                 "ctl_train_backward must get the workspace of the forward (it holds the saved activations)");

@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define CTL_ABI_VERSION 1
+#define CTL_ABI_VERSION 2
 
 #define CTL_OK 0
 #define CTL_ERR_INVALID_ARGUMENT (-1)
@@ -384,8 +384,11 @@ int ctl_stem_im2col_f16(const float* x_nchw, int32_t n, int32_t h, int32_t w, vo
  * replaces: torch autograd through ResNet.forward / ResNet_IBN.forward in train mode (modelling/backbones/resnet.py:67-87,
  * 122-133, resnet_ibn_a.py:18-32,126-141) + Baseline.forward's pooling (modelling/baseline.py:91-96) inside
  * CTLModel.training_step (train_ctl_model.py:38-179): x -> global_feat [n][2048], then d(loss)/d(global_feat) -> every
- * parameter gradient.  Same launches, same order, same bits as modelling/backbones/engine_train.py.
- *   ctl_trainer_create      : ResNet50 or ResNet50-IBN-a (`ibn` != 0), MODEL.LAST_STRIDE 1 or 2, BatchNorm momentum.
+ * parameter gradient.  This is the training trunk's only driver; modelling/backbones/engine_train.py::TrunkTrainer
+ * is its ctypes form.
+ *   ctl_trainer_create      : bottleneck ResNet with `stage_blocks` blocks per stage ({3, 4, 6, 3} = ResNet50,
+ *                             {3, 4, 23, 3} = ResNet101, each >= 1), IBN-a when `ibn` != 0, MODEL.LAST_STRIDE 1 or 2,
+ *                             BatchNorm momentum.
  *   ctl_trainer_bind        : `params` = the `base.*`-stripped fp32 parameters AND BatchNorm running buffers as device
  *                             pointers, by name (running_mean / running_var optional per layer, updated in place like
  *                             torch); `grads` = one fp32 output per PARAMETER, same name, the parameter's own layout
@@ -396,6 +399,10 @@ int ctl_stem_im2col_f16(const float* x_nchw, int32_t n, int32_t h, int32_t w, vo
  *   ctl_train_backward      : dfeat [n][2048] fp32 = dLoss/dglobal_feat.  Activation gradients are computed on
  *                             grad_scale * dfeat in fp16 (loss scaling, the role of PL's GradScaler, utils/misc.py:111);
  *                             the parameter gradients are written UN-scaled.  Same workspace as the forward, once per forward.
+ *   ctl_train_saved         : inspection call for checkers: the fp16 NHWC tensors the last completed forward saved in
+ *                             its workspace, raw conv output `y` and normalised output `z`, with their shape `nhwc`.
+ *                             index 0 = the stem, 1... = every conv + BatchNorm in forward order (conv1, conv2,
+ *                             downsample, conv3 per block).  An error before a forward or out of range.
  * Not thread-safe; all launches go to `stream`; 256-byte aligned workspace. */
 typedef struct ctl_trainer ctl_trainer;
 typedef struct ctl_named_buffer {
@@ -403,7 +410,7 @@ typedef struct ctl_named_buffer {
   float* data; /* device pointer, written */
   int64_t numel;
 } ctl_named_buffer;
-int ctl_trainer_create(ctl_trainer** out, int32_t ibn, int32_t last_stride, float momentum);
+int ctl_trainer_create(ctl_trainer** out, int32_t ibn, int32_t last_stride, float momentum, const int32_t stage_blocks[4]);
 void ctl_trainer_destroy(ctl_trainer* t);
 int ctl_trainer_bind(ctl_trainer* t, const ctl_named_tensor* params, int32_t n_params, const ctl_named_buffer* grads,
                      int32_t n_grads);
@@ -412,6 +419,7 @@ int ctl_train_forward(ctl_trainer* t, const float* x_nchw, int32_t n, int32_t he
                       void* workspace, size_t workspace_bytes, ctl_stream_t stream);
 int ctl_train_backward(ctl_trainer* t, const float* dfeat, float grad_scale, void* workspace, size_t workspace_bytes,
                        ctl_stream_t stream);
+int ctl_train_saved(const ctl_trainer* t, int32_t index, const void** y, const void** z, int32_t nhwc[4]);
 
 /* One table entry per parameter tensor, resident on the device; chunk_begin = running sum of
  * ceil(numel / CTL_OPT_CHUNK) over the preceding entries. */

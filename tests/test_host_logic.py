@@ -23,7 +23,7 @@ def test_abi_exports_every_declared_symbol():
     missing = [n for n in sorted(declared) if not hasattr(lib, n)]
     assert not missing, f"declared in the header but not exported: {missing}"
     assert declared == set(N.SIGNATURES), declared ^ set(N.SIGNATURES)
-    assert N.lib().ctl_abi_version() == 1
+    assert N.lib().ctl_abi_version() == 2
 
 
 def test_no_cpu_fallback():

@@ -209,7 +209,7 @@ def test_trunk_train_step_against_float64_autograd():
     torch.cuda.synchronize()
     assert _rel(feat.cpu(), feat_o) <= 2e-2
     nchw = lambda t: t.cpu().float().permute(0, 3, 1, 2)  # noqa: E731
-    forced = [(nchw(tr._stem[0]), nchw(tr._stem[1]))] + [(nchw(s.y), nchw(s.z)) for s in tr.saved]
+    forced = [(nchw(y), nchw(z)) for y, z in tr.saved_activations()]
     grads = tr.backward(dfeat.cuda())
     torch.cuda.synchronize()
     assert set(grads.keys()) == set(grads_o.keys())
@@ -294,20 +294,19 @@ def test_ctl_training_step_end_to_end():
     np.testing.assert_allclose(float(loss), float(ref["total"]), rtol=5e-3)
 
 
-def test_trunk_train_cuda_graphs_reproduce_eager_bits():
-    """graphs=True replays the captured forward/backward; kernels are deterministic, so features, gradients and
-    running statistics are bit-identical to the eager path, step after step."""
+def _graphs_reproduce_eager_bits(ibn, shape, last_stride):
     from oracle import ctl_oracle as O
     from ctl_b200.modelling.backbones.engine_train import TrunkTrainer
 
-    sd = O.make_trunk_state(seed=3)
+    sd = O.make_trunk_state(seed=3, ibn=ibn)
+    n, H, W = shape
     g = torch.Generator().manual_seed(8)
-    xs = [torch.randn(4, 3, 64, 32, generator=g).cuda() for _ in range(2)]
-    dfs = [(torch.randn(4, 2048, generator=g) * 1e-3).cuda() for _ in range(2)]
+    xs = [torch.randn(n, 3, H, W, generator=g).cuda() for _ in range(2)]
+    dfs = [(torch.randn(n, 2048, generator=g) * 1e-3).cuda() for _ in range(2)]
     outs = []
     for graphs in (False, True):
         params = {k: v.clone().cuda() for k, v in sd.items() if v.is_floating_point()}
-        tr = TrunkTrainer("cuda", graphs=graphs)
+        tr = TrunkTrainer("cuda", last_stride=last_stride, graphs=graphs, ibn=ibn)
         res = []
         for x, df in zip(xs, dfs):
             feat = tr.forward(x, params)
@@ -318,8 +317,23 @@ def test_trunk_train_cuda_graphs_reproduce_eager_bits():
     (eager, run_e), (graph, run_g) = outs
     for (fe, ge), (fg, gg) in zip(eager, graph):
         assert torch.equal(fe, fg)
+        assert set(ge) == set(gg)
         assert all(torch.equal(ge[k], gg[k]) for k in ge)
     assert all(torch.equal(run_e[k], run_g[k]) for k in run_e)
+
+
+def test_trunk_train_cuda_graphs_reproduce_eager_bits():
+    """graphs=True replays the captured forward/backward of the ctl_trainer handle (its host code runs inside the
+    capture); kernels are deterministic, so features, every gradient and the running statistics are bit-identical to
+    the eager path, step after step."""
+    _graphs_reproduce_eager_bits(False, (4, 64, 32), 1)
+
+
+@pytest.mark.parametrize("ibn,shape,last_stride", [(False, (3, 96, 64), 2), (True, (6, 160, 80), 1)])
+def test_trunk_train_cuda_graphs_reproduce_eager_bits_on_variants(ibn, shape, last_stride):
+    """The same two-step bit check for MODEL.LAST_STRIDE 2 (stride-2 layer4) and ResNet50-IBN-a
+    (InstanceNorm halves, ReLU after the stem)."""
+    _graphs_reproduce_eager_bits(ibn, shape, last_stride)
 
 
 def test_full_training_iterations_reduce_the_loss():
@@ -372,7 +386,7 @@ def test_ibn_trunk_train_step_teacher_forced():
     feat = tr.forward(x.cuda(), params)
     torch.cuda.synchronize()
     nchw = lambda t: t.cpu().float().permute(0, 3, 1, 2)  # noqa: E731
-    forced = [(nchw(tr._stem[0]), nchw(tr._stem[1]))] + [(nchw(s.y), nchw(s.z)) for s in tr.saved]
+    forced = [(nchw(y), nchw(z)) for y, z in tr.saved_activations()]
     grads = tr.backward(dfeat.cuda())
     torch.cuda.synchronize()
     feat_o, _, running_o = O.trunk_train_fp16sim(x, sd, ibn=True)
@@ -436,67 +450,79 @@ def test_trunk_train_matches_reference_under_autocast(tag, ibn):
     print(f"{tag}: worst gradient cosine vs reference-under-autocast {worst[0]:.4f} ({worst[1]})")
 
 
-@pytest.mark.parametrize("ibn,shape,last_stride", [(False, (4, 64, 32), 1), (False, (3, 96, 64), 2), (True, (6, 160, 80), 1)])
-def test_native_trainer_handle_matches_trunk_trainer(ibn, shape, last_stride):
-    """ctl_trainer_* (csrc/trunk_train.cu, the train forward / backward behind the C ABI) issues the launches of
-    engine_train.TrunkTrainer in the same order: features, every parameter gradient and the running statistics are
-    bit-identical over two consecutive steps (the InstanceNorm affine gradients, which TrunkTrainer sums over the
-    images with torch.sum and the handle with its own fixed-order kernel: 1e-6 relative)."""
+def test_resnet101_trunk_train_step_against_float64_autograd():
+    """The handle builds the stage depths it is given: a ResNet-101 (3, 4, 23, 3) train step against float64 autograd
+    of the same network with the engine's fp16 rounding points.  Features and running statistics of the independent
+    forward within 2e-2; gradients teacher-forced (through the engine's saved activations) within 2e-2 max-norm
+    relative.  The independent forward's direction check of the ResNet-50 test does not transfer: across 33 blocks the
+    ReLU-mask noise of two correct fp16 forwards leaves BatchNorm gradients at cosine ~0.95 on an H100, while the
+    teacher-forced gradients measured within 3e-3."""
     from oracle import ctl_oracle as O
-    from ctl_b200.modelling.backbones.engine_train import NativeTrainer, TrunkTrainer
+    from ctl_b200.modelling.backbones.engine_train import TrunkTrainer
 
-    sd = O.make_trunk_state(seed=21, ibn=ibn)
-    n, H, W = shape
-    g = torch.Generator().manual_seed(31)
-    xs = [torch.randn(n, 3, H, W, generator=g).cuda() for _ in range(2)]
-    dfs = [(torch.randn(n, 2048, generator=g) * 1e-3).cuda() for _ in range(2)]
-    outs = []
-    for native in (False, True):
-        params = {k: v.clone().cuda().contiguous() for k, v in sd.items() if v.is_floating_point()}
-        tr = (NativeTrainer(params, "cuda:0", last_stride=last_stride, ibn=ibn, grad_scale=2048.0) if native
-              else TrunkTrainer("cuda:0", last_stride=last_stride, ibn=ibn, grad_scale=2048.0))
-        res = []
-        for x, df in zip(xs, dfs):
-            feat = tr.forward(x) if native else tr.forward(x, params)
-            grads = tr.backward(df)
-            res.append((feat.clone(), {k: v.clone() for k, v in grads.items()}))
-        torch.cuda.synchronize()
-        outs.append((res, {k: v.clone() for k, v in params.items() if "running" in k}))
-    (py, run_p), (nat, run_n) = outs
-    for (fp, gp), (fn, gn) in zip(py, nat):
-        assert torch.equal(fp, fn)
-        assert set(gp) == set(gn)
-        for k in gp:
-            assert gp[k].shape == gn[k].shape, k
-            if ".IN." in k:
-                assert _rel(gn[k], gp[k]) < 1e-6, k
-            else:
-                assert torch.equal(gp[k], gn[k]), k
-    assert all(torch.equal(run_p[k], run_n[k]) for k in run_p)
+    layers = (3, 4, 23, 3)
+    sd = O.make_trunk_state(seed=19, layers=layers)
+    g = torch.Generator().manual_seed(3)
+    x = torch.randn(4, 3, 64, 32, generator=g)
+    dfeat = torch.randn(4, 2048, generator=g) * 1e-3
+    params = {k: v.clone().cuda() for k, v in sd.items() if v.is_floating_point()}
+    tr = TrunkTrainer("cuda", layers=layers, grad_scale=4096.0)
+    feat = tr.forward(x.cuda(), params)
+    torch.cuda.synchronize()
+    nchw = lambda t: t.cpu().float().permute(0, 3, 1, 2)  # noqa: E731
+    saved = tr.saved_activations()
+    assert len(saved) == 1 + 3 * sum(layers) + 4
+    forced = [(nchw(y), nchw(z)) for y, z in saved]
+    grads = tr.backward(dfeat.cuda())
+    torch.cuda.synchronize()
+    feat_o, _, running_o = O.trunk_train_fp16sim(x, sd, layers=layers)
+    assert _rel(feat.cpu(), feat_o) <= 2e-2
+    for k, v in running_o.items():
+        assert _rel(params[k].cpu(), v) <= 2e-2, k
+    feat_f, grads_f, _ = O.trunk_train_fp16sim(x, sd, dfeat, layers=layers, forced=forced)
+    assert set(grads.keys()) == set(grads_f.keys())
+    assert _rel(feat.cpu(), feat_f) <= 1e-5
+    gscale = max(float(v.abs().max()) for v in grads_f.values())
+    bad = {}
+    for k, go in grads_f.items():
+        assert torch.isfinite(grads[k]).all(), k
+        if float(go.abs().max()) < 1e-6 * gscale:
+            continue
+        r = _rel(grads[k].cpu(), go)
+        if r > 2e-2:
+            bad[k] = r
+    assert not bad, f"gradient mismatch (max-norm relative): {sorted(bad.items(), key=lambda t: -t[1])[:8]}"
 
 
 def test_native_trainer_argument_errors():
-    """missing tensors, a backward without its forward, and a foreign workspace are reported, not executed."""
+    """wrong tensors, a missing tensor, a backward without its forward and a foreign workspace are reported, not
+    executed."""
     import ctypes as C
 
     from ctl_b200 import _native as N
     from oracle import ctl_oracle as O
-    from ctl_b200.modelling.backbones.engine_train import NativeTrainer
+    from ctl_b200.modelling.backbones.engine_train import TrunkTrainer
 
     sd = O.make_trunk_state(seed=2)
     params = {k: v.clone().cuda().contiguous() for k, v in sd.items() if v.is_floating_point()}
+    x = torch.randn(2, 3, 64, 32, device="cuda")
+    df = torch.zeros(2, 2048, device="cuda")
+    tr = TrunkTrainer("cuda:0")
+    with pytest.raises(TypeError, match="layer1.0.conv1.weight"):
+        tr.forward(x, {**params, "layer1.0.conv1.weight": params["layer1.0.conv1.weight"].half()})
     broken = dict(params)
     del broken["layer2.0.downsample.1.weight"]
     with pytest.raises(ValueError, match="layer2.0.downsample.1.weight"):
-        NativeTrainer(broken, "cuda:0")
-    tr = NativeTrainer(params, "cuda:0")
-    df = torch.zeros(2, 2048, device="cuda")
-    tr._ws = torch.empty(1 << 20, dtype=torch.uint8, device="cuda")
+        tr.forward(x, broken)
     with pytest.raises(ValueError, match="forward"):
         tr.backward(df)
-    tr.forward(torch.randn(2, 3, 64, 32, device="cuda"))
+    with pytest.raises(ValueError, match="forward"):
+        tr.saved_activations()
+    tr.forward(x, params)
     other = torch.empty_like(tr._ws)
     rc = N.lib().ctl_train_backward(tr._h, df.data_ptr(), C.c_float(1024.0), other.data_ptr(), other.numel(), N.stream_ptr())
     assert rc != 0 and b"workspace of the forward" in N.lib().ctl_last_error()
     tr.backward(df)  # the right workspace still works
+    with pytest.raises(ValueError, match="forward"):
+        tr.backward(df)  # one backward per forward
     torch.cuda.synchronize()

@@ -1,8 +1,8 @@
 """GPU: the training step's data-gradient, normalisation and loss-scaling kernels, one C entry point at a time, against
 float64 torch on the CPU computed on the same fp16-rounded operands.
 
-Every entry point is driven in the sequence the training engines use (engine_train.py::TrunkTrainer._conv_bwd /
-_bn_bwd, csrc/trunk_train.cu::conv_backward / bn_backward), and every output buffer starts as NaN so that an element the
+Every entry point is driven in the sequence the training trunk uses (csrc/trunk_train.cu::conv_backward /
+bn_backward), and every output buffer starts as NaN so that an element the
 kernel never writes fails the check.  Channel-slice kernels (pitch > C, the two halves of an IBN layer) must also leave
 every channel outside their slice bit-identical.
 
@@ -50,7 +50,7 @@ def _nan32(*shape):
 # 1. ctl_train_pack_weights: fp16 forward operand [cout][k][k][cin] and flipped data-gradient operand [cin][k][k][cout]
 # ===================================================================================================================
 def _pack_table(entries):
-    """The 48-byte entries of engine_train.TrunkTrainer._pack_weights: {src, fwd, dgrad, cout | cin << 32, k (pad 0),
+    """The 48-byte entries of csrc/trunk_train.cu's pack table (ctl_trainer_bind): {src, fwd, dgrad, cout | cin << 32, k (pad 0),
     chunk_begin}; entries = [(src fp32 [cout][cin][k][k], fwd, dgrad or None)]."""
     rows, chunks = [], 0
     for src, fwd, dgr in entries:
@@ -261,7 +261,7 @@ def _bn_slice_case(rows, c, pitch, relu, res, running, shift=0.0, seed=0):
     assert float(err) <= float(zref.abs().max()) * 2.0 ** -10 + 1e-6  # one fp16 rounding at the output's scale
     assert torch.isnan(o[:, :off]).all(), "forward wrote outside its channel slice"
 
-    # backward: z is the reference's own fp16 output (same ReLU mask), g_out aliases dz (engine_train.py::_bn_bwd)
+    # backward: z is the reference's own fp16 output (same ReLU mask), g_out aliases dz (csrc/trunk_train.cu::bn_backward)
     zfull = torch.randn(rows, pitch, generator=g).half()
     zfull[:, sl] = zref16
     zc = zfull.cuda()

@@ -2,8 +2,8 @@
 (im2col, the arg-max max-pool pair), one C entry point at a time, at the geometries and batch sizes of a training step,
 against float64 references.
 
-Every entry point is called with the arguments the engines pass (engine_train.py::TrunkTrainer._wgrad / backward,
-csrc/trunk_train.cu::conv_backward / the stem), and every output buffer and workspace starts as NaN so that an element
+Every entry point is called with the arguments the training trunk passes (csrc/trunk_train.cu::conv_backward / the
+stem), and every output buffer and workspace starts as NaN so that an element
 the kernel never writes fails the check.
 
 The weight gradient splits the pixel reduction K = n*Ho*Wo into S = `splits` ranges of 128-pixel tiles; each
@@ -343,7 +343,7 @@ def test_stem_weight_gradient_as_the_trainer_chains_it():
     assert torch.equal(_bits(dw[:, 168:]), _bits(torch.zeros(64, 24, device="cuda"))), "k >= 168 not +0"
     pad_s = dw[:, :168].reshape(64, 3, 7, 8)[..., 7]
     assert torch.equal(_bits(pad_s.contiguous()), _bits(torch.zeros_like(pad_s))), "s = 7 not +0"
-    got = dw[:, :168].reshape(64, 3, 7, 8)[..., :7]   # engine_train.py's unpack (before the 1 / loss-scale)
+    got = dw[:, :168].reshape(64, 3, 7, 8)[..., :7]   # stem_train_unpack_kernel's order (before the 1 / loss-scale)
     xd, dyd = x.half().double(), dy.double().permute(0, 3, 1, 2)
     ref = torch.nn.grad.conv2d_weight(xd, (64, 3, 7, 7), dyd, stride=2, padding=3)
     mag = torch.nn.grad.conv2d_weight(xd.abs(), (64, 3, 7, 7), dyd.abs(), stride=2, padding=3)

@@ -25,6 +25,6 @@ for _ in range(it):
     torch.cuda.synchronize()
     fw += ev[0].elapsed_time(ev[1]); bw += ev[1].elapsed_time(ev[2])
 wall = (time.perf_counter() - t0) / it * 1e3
-print(f"train trunk bs={bs}: forward {fw/it:.2f} ms, backward {bw/it:.2f} ms, wall {wall:.2f} ms/step, launches {tr.launches}, "
+print(f"train trunk bs={bs}: forward {fw/it:.2f} ms, backward {bw/it:.2f} ms, wall {wall:.2f} ms/step, "
       f"{bs/((fw+bw)/it)*1e3:.0f} img/s, {3*bs*8.1065/((fw+bw)/it):.1f} TFLOP/s (3x fwd flops)")
 print(f"peak memory {torch.cuda.max_memory_allocated()/2**30:.1f} GiB")
