@@ -97,6 +97,9 @@ SIGNATURES = {
     "ctl_xent_smooth_step": (C.c_int, [_p, _i32, _i32, _p, _f, _p, _p, _p, _sz, _p]),
     "ctl_conv2d_nhwc_f16": (C.c_int, [_p, _i32, _i32, _i32, _i32, _p, _p, _p, _p, _i32, _i32, _i32, _i32, _i32, _p]),
     "ctl_conv1x1_dual_nhwc_f16": (C.c_int, [_p, _i32, _p, _i32, _i32, _i32, _i32, _i32, _p, _p, _p, _i32, _i32, _p]),
+    "ctl_conv1x1_chain_supported": (_i32, [_i32, _i32]),
+    "ctl_conv1x1_chain_nhwc_f16": (C.c_int, [_p, _i32, _p, _i32, _i32, _i32, _i32, _i32, _p, _p, _p, _p, _i32, _p, _p,
+                                             _i32, _i32, _p, _p]),
     "ctl_trunk_create": (C.c_int, [C.POINTER(_p), _i32, _i32]),
     "ctl_trunk_destroy": (None, [_p]),
     "ctl_weights_pack": (C.c_int, [_p, C.POINTER(NamedTensor), _i32, _p]),

@@ -60,6 +60,12 @@ struct ConvKernelParams {
   int has_residual;
   int relu;                 // apply ReLU to channels >= relu_from
   int relu_from;
+  // chained launch (conv_gemm_kernel<BN, N2 > 0>): the next 1x1 convolution of the layer, out2 = act(out W2^T + bias2)
+  // with ReLU on channels >= relu_from2, computed from the staged fp16 output tile
+  CUtensorMap b2_map;    // W2 [N2][Cout] fp16, box {64, N2}
+  CUtensorMap out2_map;  // NHWC [.., N2] output, box {64 ch, TW, TH, 1}
+  const float* bias2;    // [N2]
+  int relu_from2;
 };
 
 template <int BN>
@@ -133,10 +139,17 @@ __device__ __forceinline__ void store_subtile_f16(const float* d, uint8_t* slab,
   }
 }
 
-template <int BN>
+// N2 > 0: chained launch.  Staging slab j of an output tile is exactly the K-major SWIZZLE_128B A operand of
+// k-block (nt * BN / 64 + j) of the next 1x1 convolution (K2 = Cout, N2 outputs), so once a slab is complete each
+// consumer warpgroup issues that k-block (m64 nN2 k16 x 4, the shape and k order of the stand-alone launch: same bits)
+// into a second accumulator that lives across the m-tile's n-tiles; its weight slab W2[:, 64 kb .. 64 kb + 63] rides
+// the operand ring after the sub-tile's residual slab.  After the last n-tile the second accumulator goes through the
+// same epilogue into out2, so the block output is never re-read from HBM.  Each CTA owns whole m-tiles.
+template <int BN, int N2 = 0>
 __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid_constant__ ConvKernelParams p) {
   using Cfg = ConvCfg<BN>;
   constexpr int NSUB = BN / 64;
+  static_assert(N2 == 0 || N2 == 64 || N2 == 128, "chained 1x1 width");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t out_stage = smem_base + Cfg::STAGES * Cfg::STAGE_BYTES;
@@ -149,10 +162,15 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid
   const int warp = threadIdx.x >> 5;
   const int num_tiles = p.m_tiles * p.n_tiles;
   const int conv_kblocks = p.k_blocks;
-  // contiguous, balanced tile range of this CTA
-  const int per = num_tiles / (int)gridDim.x, rem = num_tiles - per * (int)gridDim.x;
-  const int t_begin = (int)blockIdx.x * per + min((int)blockIdx.x, rem);
-  const int t_end = t_begin + per + ((int)blockIdx.x < rem ? 1 : 0);
+  // contiguous, balanced tile range of this CTA (chained: of whole m-tiles)
+  const int units = N2 > 0 ? p.m_tiles : num_tiles;
+  const int per = units / (int)gridDim.x, rem = units - per * (int)gridDim.x;
+  int t_begin = (int)blockIdx.x * per + min((int)blockIdx.x, rem);
+  int t_end = t_begin + per + ((int)blockIdx.x < rem ? 1 : 0);
+  if constexpr (N2 > 0) {
+    t_begin *= p.n_tiles;
+    t_end *= p.n_tiles;
+  }
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < Cfg::STAGES; ++s) {
@@ -164,9 +182,16 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid
     tma_prefetch_desc(&p.b_map);
     tma_prefetch_desc(&p.out_map);
     tma_prefetch_desc(&p.res_map);
+    if constexpr (N2 > 0) {
+      tma_prefetch_desc(&p.b2_map);
+      tma_prefetch_desc(&p.out2_map);
+    }
   }
   for (int i = threadIdx.x; i < p.Cout; i += blockDim.x)
     reinterpret_cast<float*>(gsm + (bias_sm - smem_base))[i] = p.bias[i];
+  if constexpr (N2 > 0)  // bias2 right after bias (Cout + N2 <= 2048)
+    for (int i = threadIdx.x; i < N2; i += blockDim.x)
+      reinterpret_cast<float*>(gsm + (bias_sm - smem_base))[p.Cout + i] = p.bias2[i];
   __syncthreads();
   pdl_launch_dependents();  // the next kernel may begin its prologue
   pdl_wait();               // activations of the previous kernel are complete and visible
@@ -195,17 +220,29 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid
             }
           }
         }
-        if (p.has_residual) {
+        if (p.has_residual || N2 > 0) {
           // the residual rides the same ring: one [128 px][64 ch] slab per 64 output channels, read by
-          // the epilogue of that sub-tile straight from its ring slot
+          // the epilogue of that sub-tile straight from its ring slot; a chained launch follows each with
+          // the W2 slab of that sub-tile's GEMM2 k-block
           for (int j = 0; j < NSUB; ++j) {
-            mbar_wait(empty_bar(stage), phase ^ 1u);
-            mbar_arrive_expect_tx(full_bar(stage), A_TILE_BYTES);
-            tma_load_4d(smem_base + stage * Cfg::STAGE_BYTES, &p.res_map, full_bar(stage), it.nt * BN + j * 64, w0, h0,
-                        it.img);
-            if (++stage == Cfg::STAGES) {
-              stage = 0;
-              phase ^= 1u;
+            if (p.has_residual) {
+              mbar_wait(empty_bar(stage), phase ^ 1u);
+              mbar_arrive_expect_tx(full_bar(stage), A_TILE_BYTES);
+              tma_load_4d(smem_base + stage * Cfg::STAGE_BYTES, &p.res_map, full_bar(stage), it.nt * BN + j * 64, w0, h0,
+                          it.img);
+              if (++stage == Cfg::STAGES) {
+                stage = 0;
+                phase ^= 1u;
+              }
+            }
+            if constexpr (N2 > 0) {
+              mbar_wait(empty_bar(stage), phase ^ 1u);
+              mbar_arrive_expect_tx(full_bar(stage), N2 * CBK * 2);
+              tma_load_2d(smem_base + stage * Cfg::STAGE_BYTES, &p.b2_map, full_bar(stage), it.nt * BN + j * 64, 0);
+              if (++stage == Cfg::STAGES) {
+                stage = 0;
+                phase ^= 1u;
+              }
             }
           }
         }
@@ -224,6 +261,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid
     uint8_t* oslabs = gsm + (out_stage - smem_base);
     const float* bias_s = reinterpret_cast<const float*>(gsm + (bias_sm - smem_base));
     float acc[BN / 2];
+    [[maybe_unused]] float acc2[N2 > 0 ? N2 / 2 : 1];  // GEMM2 (chained launch only)
     int stage = 0;
     uint32_t phase = 0;
     uint32_t g = 0;  // running sub-tile counter -> staging slab
@@ -252,6 +290,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid
       }
       wgmma_wait<0>();
       if (held >= 0 && wg_leader) mbar_arrive(empty_bar(held));
+      [[maybe_unused]] int held2 = -1;  // ring slot of the W2 slab read by the GEMM2 group in flight
 #pragma unroll
       for (int j = 0; j < NSUB; ++j, ++g) {
         const uint32_t b = g & (Cfg::OUT_SLABS - 1);
@@ -277,6 +316,46 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid
         if (leader) {
           tma_store_4d(&p.out_map, out_stage + b * A_TILE_BYTES, it.nt * BN + j * 64, w0, h0, it.img);
           tma_store_commit();
+        }
+        if constexpr (N2 > 0) {
+          // GEMM2 k-block nt * NSUB + j from this warpgroup's 64 rows of slab b.  Each warpgroup reads only the rows it
+          // wrote, and the group reading slab b has completed (wgmma_wait<1> one sub-tile later) before it is rewritten.
+          mbar_wait(full_bar(stage), phase);
+          const uint64_t da = make_sw128_kmajor_desc(out_stage + b * A_TILE_BYTES + wg * A_HALF_BYTES);
+          const uint64_t db = make_sw128_kmajor_desc(smem_base + stage * Cfg::STAGE_BYTES);
+          const bool first = it.nt == 0 && j == 0;
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < CBK / 16; ++k)
+            wgmma_f16<N2>(acc2, desc_advance_k(da, k), desc_advance_k(db, k), (!first || k > 0) ? 1u : 0u);
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (held2 >= 0 && wg_leader) mbar_arrive(empty_bar(held2));  // the previous W2 slab
+          held2 = stage;
+          if (++stage == Cfg::STAGES) {
+            stage = 0;
+            phase ^= 1u;
+          }
+        }
+      }
+      if constexpr (N2 > 0) {
+        wgmma_wait<0>();
+        if (wg_leader) mbar_arrive(empty_bar(held2));
+        if (it.nt == p.n_tiles - 1) {  // the m-tile's GEMM2 is complete: its epilogue, into out2
+#pragma unroll
+          for (int j = 0; j < N2 / 64; ++j, ++g) {
+            const uint32_t b = g & (Cfg::OUT_SLABS - 1);
+            if (leader) tma_store_wait_read<Cfg::OUT_SLABS - 1>();
+            named_bar_sync(1, 256);
+            store_subtile_f16(acc2 + 32 * j, oslabs + b * A_TILE_BYTES, row0, bias_s + p.Cout + j * 64, j * 64, 1,
+                              p.relu_from2);
+            fence_proxy_async();
+            named_bar_sync(1, 256);
+            if (leader) {
+              tma_store_4d(&p.out2_map, out_stage + b * A_TILE_BYTES, j * 64, w0, h0, it.img);
+              tma_store_commit();
+            }
+          }
         }
       }
     }
@@ -962,20 +1041,36 @@ __global__ void __launch_bounds__(256) instnorm_relu_kernel(__half* __restrict__
 // ---------------------------------------------------------------------------------------
 // host
 // ---------------------------------------------------------------------------------------
-template <int BN>
+template <int BN, int N2 = 0>
 static int launch_conv(const ConvKernelParams& p, cudaStream_t st) {
   static bool attr_set = false;
   if (!attr_set) {
-    CTL_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    CTL_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN, N2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   (int)ConvCfg<BN>::SMEM));
     attr_set = true;
   }
-  const long long tiles = (long long)p.m_tiles * p.n_tiles;
-  const int grid = (int)std::min<long long>(tiles, sm_count());
-  CTL_CUDA(launch_k(conv_gemm_kernel<BN>, dim3(grid), dim3(CONV_THREADS), ConvCfg<BN>::SMEM, st, p));
+  const long long units = N2 > 0 ? (long long)p.m_tiles : (long long)p.m_tiles * p.n_tiles;
+  const int grid = (int)std::min<long long>(units, sm_count());
+  CTL_CUDA(launch_k(conv_gemm_kernel<BN, N2>, dim3(grid), dim3(CONV_THREADS), ConvCfg<BN>::SMEM, st, p));
   CTL_LAUNCH_CHECK();
   return 0;
 }
+
+// Whether the 1x1 convolution cout -> cout2 that reads a launch's output can be chained into that launch
+// (conv_gemm_kernel<128, cout2>).  The kernel's 168 registers per thread (384 threads, one CTA per SM) hold GEMM1's
+// 64 accumulators of a 128-wide n-tile plus GEMM2's cout2 / 2 (a 256-wide n-tile's 128 plus 32 already spill); at most
+// four n-tiles per m-tile keep the m-tiles (the unit a CTA owns) numerous enough to balance.
+static bool chain_fits(int cout, int cout2) {
+  return cout % 128 == 0 && cout <= 512 && (cout2 == 64 || cout2 == 128);
+}
+
+// The next 1x1 convolution of a chained launch (ctl_conv1x1_chain_nhwc_f16).
+struct ChainNext {
+  const void* weight;  // [cout2][cout] fp16
+  const float* bias;
+  void* out;
+  int cout2, relu_from;
+};
 
 static int launch_c64(const void* x, int n, int h, int w, const void* weight, const float* bias, void* out, int relu,
                       cudaStream_t st) {
@@ -1009,10 +1104,11 @@ static int launch_c64(const void* x, int n, int h, int w, const void* weight, co
 }
 
 // Fills the tile geometry, the output / residual / weight maps and dispatches.  The caller has filled the A maps,
-// the taps and k_blocks; `ktot` = row length of the weight matrix [Cout][ktot].
+// the taps and k_blocks; `ktot` = row length of the weight matrix [Cout][ktot]; `next` (chain_fits(cout, cout2))
+// chains the following 1x1 convolution into the launch.
 static int finish_and_launch(ConvKernelParams& p, int n, int Ho, int Wo, int cout, int ktot, const void* weight,
                              const float* bias, const void* residual, void* out, int relu, int relu_from,
-                             cudaStream_t st) {
+                             cudaStream_t st, const ChainNext* next = nullptr) {
   int rc;
   p.n_img = n;
   p.Ho = Ho;
@@ -1023,7 +1119,7 @@ static int finish_and_launch(ConvKernelParams& p, int n, int Ho, int Wo, int cou
   p.relu = relu;
   p.relu_from = relu_from;
   p.m_tiles = n * p.tiles_h * p.tiles_w;
-  const int BN = cout % 256 == 0 ? 256 : (cout % 128 == 0 ? 128 : 64);
+  const int BN = next ? 128 : (cout % 256 == 0 ? 256 : (cout % 128 == 0 ? 128 : 64));
   p.n_tiles = cout / BN;
   {
     const uint64_t odims[4] = {(uint64_t)cout, (uint64_t)Wo, (uint64_t)Ho, (uint64_t)n};
@@ -1042,6 +1138,24 @@ static int finish_and_launch(ConvKernelParams& p, int n, int Ho, int Wo, int cou
   if ((rc = encode_tensor_map(&p.b_map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 2, weight, bdims, bstr, bbox,
                               CU_TENSOR_MAP_SWIZZLE_128B)))
     return rc;
+  if (next) {
+    const int c2 = next->cout2;
+    const uint64_t odims[4] = {(uint64_t)c2, (uint64_t)Wo, (uint64_t)Ho, (uint64_t)n};
+    const uint64_t ostr[4] = {2, (uint64_t)c2 * 2, (uint64_t)Wo * c2 * 2, (uint64_t)Ho * Wo * c2 * 2};
+    const uint32_t obox[4] = {64, (uint32_t)p.TW, (uint32_t)p.TH, 1};
+    if ((rc = encode_tensor_map(&p.out2_map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 4, next->out, odims, ostr, obox,
+                                CU_TENSOR_MAP_SWIZZLE_128B)))
+      return rc;
+    const uint64_t wdims[2] = {(uint64_t)cout, (uint64_t)c2};
+    const uint64_t wstr[2] = {2, (uint64_t)cout * 2};
+    const uint32_t wbox[2] = {CBK, (uint32_t)c2};
+    if ((rc = encode_tensor_map(&p.b2_map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 2, next->weight, wdims, wstr, wbox,
+                                CU_TENSOR_MAP_SWIZZLE_128B)))
+      return rc;
+    p.bias2 = next->bias;
+    p.relu_from2 = next->relu_from;
+    return c2 == 64 ? launch_conv<128, 64>(p, st) : launch_conv<128, 128>(p, st);
+  }
   if (BN == 256) return launch_conv<256>(p, st);
   if (BN == 128) return launch_conv<128>(p, st);
   return launch_conv<64>(p, st);
@@ -1071,6 +1185,28 @@ static int encode_source(CUtensorMap* maps, int count, const void* x, int n, int
                                 strd, abox, CU_TENSOR_MAP_SWIZZLE_128B)))
       return rc;
   }
+  return 0;
+}
+
+// Tile geometry, A maps and taps of a 1x1 convolution at the output resolution Ho x Wo = h2 / stride2 x w2 / stride2:
+// x1 [n][Ho][Wo][cin1] alone, or K-concatenated with x2 [n][h2][w2][cin2] read at stride2.
+static int setup_1x1(ConvKernelParams& p, const void* x1, int cin1, const void* x2, int h2, int w2, int cin2, int stride2,
+                     int n) {
+  int rc;
+  const int Ho = h2 / stride2, Wo = w2 / stride2;
+  pick_tile(Ho, Wo, &p.TH, &p.TW);
+  p.tiles_h = (Ho + p.TH - 1) / p.TH;
+  p.tiles_w = (Wo + p.TW - 1) / p.TW;
+  // map 0: x1 at the output resolution; map 1: x2 (its (0, 0) parity view when strided); unused maps repeat map 0
+  if ((rc = encode_source(&p.a_map[0], 1, x1, n, Ho, Wo, cin1, 1, p.TH, p.TW))) return rc;
+  p.a_map[1] = p.a_map[0];
+  if (x2 && (rc = encode_source(&p.a_map[1], 1, x2, n, h2, w2, cin2, stride2, p.TH, p.TW))) return rc;
+  p.a_map[2] = p.a_map[0];
+  p.a_map[3] = p.a_map[0];
+  p.n_taps = x2 ? 2 : 1;
+  p.taps[0] = ConvTap{0, 0, 0, 0, cin1 / 64};
+  if (x2) p.taps[1] = ConvTap{1, 0, 0, cin1, cin2 / 64};
+  p.k_blocks = (cin1 + (x2 ? cin2 : 0)) / 64;
   return 0;
 }
 
@@ -1130,21 +1266,35 @@ int ctl_conv1x1_dual_nhwc_f16(const void* x1, int32_t cin1, const void* x2, int3
   CTL_CHECK_ARG(stride2 == 1 || (stride2 == 2 && h2 % 2 == 0 && w2 % 2 == 0), "stride2 must be 1, or 2 with even H2, W2");
   int rc = ctl_device_check();
   if (rc) return rc;
-  const int Ho = h2 / stride2, Wo = w2 / stride2;
   ConvKernelParams p = {};
-  pick_tile(Ho, Wo, &p.TH, &p.TW);
-  p.tiles_h = (Ho + p.TH - 1) / p.TH;
-  p.tiles_w = (Wo + p.TW - 1) / p.TW;
-  // map 0: x1 at the output resolution; map 1: x2 (its (0, 0) parity view when strided); maps 2, 3 unused
-  if ((rc = encode_source(&p.a_map[0], 1, x1, n, Ho, Wo, cin1, 1, p.TH, p.TW))) return rc;
-  if ((rc = encode_source(&p.a_map[1], 1, x2, n, h2, w2, cin2, stride2, p.TH, p.TW))) return rc;
-  p.a_map[2] = p.a_map[0];
-  p.a_map[3] = p.a_map[0];
-  p.n_taps = 2;
-  p.taps[0] = ConvTap{0, 0, 0, 0, cin1 / 64};
-  p.taps[1] = ConvTap{1, 0, 0, cin1, cin2 / 64};
-  p.k_blocks = (cin1 + cin2) / 64;
-  return finish_and_launch(p, n, Ho, Wo, cout, cin1 + cin2, weight_cat, bias, nullptr, out, relu, 0, (cudaStream_t)stream);
+  if ((rc = setup_1x1(p, x1, cin1, x2, h2, w2, cin2, stride2, n))) return rc;
+  return finish_and_launch(p, n, h2 / stride2, w2 / stride2, cout, cin1 + cin2, weight_cat, bias, nullptr, out, relu, 0,
+                           (cudaStream_t)stream);
+}
+
+int32_t ctl_conv1x1_chain_supported(int32_t cout, int32_t cout2) { return chain_fits(cout, cout2) ? 1 : 0; }
+
+int ctl_conv1x1_chain_nhwc_f16(const void* x1, int32_t cin1, const void* x2, int32_t h2, int32_t w2, int32_t cin2,
+                               int32_t stride2, int32_t n, const void* weight, const float* bias, const void* residual,
+                               void* out, int32_t cout, const void* weight2, const float* bias2, int32_t cout2,
+                               int32_t relu_from2, void* out2, ctl_stream_t stream) {
+  CTL_CHECK_ARG(x1 && weight && bias && out && weight2 && bias2 && out2, "null pointer");
+  CTL_CHECK_ARG(!(x2 && residual), "the K-concatenated form (x2) takes no residual");
+  CTL_CHECK_ARG(n >= 1 && h2 >= 1 && w2 >= 1, "bad activation shape");
+  CTL_CHECK_ARG(cin1 % 64 == 0 && cin1 >= 64 && (!x2 || (cin2 % 64 == 0 && cin2 >= 64)),
+                "Cin1=%d and Cin2=%d must be multiples of 64", cin1, cin2);
+  CTL_CHECK_ARG(chain_fits(cout, cout2), "Cout=%d -> Cout2=%d cannot be chained (see ctl_conv1x1_chain_supported)", cout,
+                cout2);
+  CTL_CHECK_ARG(relu_from2 % 32 == 0, "relu_from2=%d must be a multiple of 32", relu_from2);
+  CTL_CHECK_ARG(x2 ? (stride2 == 1 || (stride2 == 2 && h2 % 2 == 0 && w2 % 2 == 0)) : stride2 == 1,
+                "stride2 must be 1, or 2 with even H2, W2 and a second source");
+  int rc = ctl_device_check();
+  if (rc) return rc;
+  ConvKernelParams p = {};
+  if ((rc = setup_1x1(p, x1, cin1, x2, h2, w2, cin2, stride2, n))) return rc;
+  const ChainNext next = {weight2, bias2, out2, cout2, relu_from2};
+  return finish_and_launch(p, n, h2 / stride2, w2 / stride2, cout, cin1 + (x2 ? cin2 : 0), weight, bias, residual, out, 1,
+                           0, (cudaStream_t)stream, &next);
 }
 
 int ctl_stem_conv7x7_tc(const float* x_nchw, int32_t n, int32_t h, int32_t w, const void* weight_k192_f16,

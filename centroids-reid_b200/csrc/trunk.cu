@@ -366,32 +366,52 @@ int ctl_embed_forward(ctl_trunk* h, const float* x_nchw, int32_t n, int32_t hgt,
   }
   hh = hp;
   ww = wp;
-  int cur = 0;  // index of the buffer holding the block input
-  for (const TrunkBlock& blk : h->blocks) {
-    void* o1 = buf[(cur + 1) % 5];
-    void* o2 = buf[(cur + 2) % 5];
-    void* res = buf[(cur + 3) % 5];
-    void* out = buf[(cur + 4) % 5];
-    if ((rc = run_conv(blk.c1, a, n, hh, ww, nullptr, o1, st))) return rc;
+  int cur = 0;         // index of the buffer holding the block input
+  int o1_ready = -1;   // buffer holding this block's conv1 output when the previous block's launch computed it
+  for (size_t bi = 0; bi < h->blocks.size(); ++bi) {
+    const TrunkBlock& blk = h->blocks[bi];
+    // roles of the four buffers other than the input; a conv1 output computed ahead keeps its buffer (dead again once
+    // conv2 has read it, so the next chained launch writes there too) and the other roles rotate around it
+    int role[4], k = 0;
+    if (o1_ready >= 0) role[k++] = o1_ready;
+    for (int i = 1; i < 5; ++i)
+      if ((cur + i) % 5 != o1_ready && k < 4) role[k++] = (cur + i) % 5;
+    void* o1 = buf[role[0]];
+    void* o2 = buf[role[1]];
+    void* res = buf[role[2]];
+    void* out = buf[role[3]];
+    if (o1_ready < 0 && (rc = run_conv(blk.c1, a, n, hh, ww, nullptr, o1, st))) return rc;
     if (blk.has_in)
       if ((rc = ctl_instnorm_relu_nhwc_f16(o1, n, hh * ww, blk.c1.cout, blk.in_half, blk.in_gamma, blk.in_beta, TRUNK_BN_EPS, st)))
         return rc;
     const int s = blk.c2.stride;
     const int h2 = (hh + 2 - 3) / s + 1, w2 = (ww + 2 - 3) / s + 1;
     if ((rc = run_conv(blk.c2, o1, n, hh, ww, nullptr, o2, st))) return rc;
-    if (blk.has_down && hh % s == 0 && ww % s == 0) {
-      if ((rc = ctl_conv1x1_dual_nhwc_f16(o2, blk.c3.cin, a, hh, ww, blk.down.cin, s, n, blk.dual_w, blk.dual_b, out, blk.c3.cout, 1, st)))
-        return rc;
-    } else {
-      const void* r = a;
-      if (blk.has_down) {
-        if ((rc = run_conv(blk.down, a, n, hh, ww, nullptr, res, st))) return rc;
-        r = res;
-      }
-      if ((rc = run_conv(blk.c3, o2, n, h2, w2, r, out, st))) return rc;
+    const bool dual = blk.has_down && hh % s == 0 && ww % s == 0;
+    const void* r = a;
+    if (blk.has_down && !dual) {
+      if ((rc = run_conv(blk.down, a, n, hh, ww, nullptr, res, st))) return rc;
+      r = res;
     }
+    // the next block's conv1 in this launch's epilogue: its output goes to o1's buffer (a and res are still read)
+    const PackedConv* nx = bi + 1 < h->blocks.size() ? &h->blocks[bi + 1].c1 : nullptr;
+    const bool chain = nx && ctl_conv1x1_chain_supported(blk.c3.cout, nx->cout);
+    if (chain) {
+      if (dual)
+        rc = ctl_conv1x1_chain_nhwc_f16(o2, blk.c3.cin, a, hh, ww, blk.down.cin, s, n, blk.dual_w, blk.dual_b, nullptr, out,
+                                        blk.c3.cout, nx->w, nx->b, nx->cout, nx->relu_from, o1, st);
+      else
+        rc = ctl_conv1x1_chain_nhwc_f16(o2, blk.c3.cin, nullptr, h2, w2, 0, 1, n, blk.c3.w, blk.c3.b, r, out, blk.c3.cout,
+                                        nx->w, nx->b, nx->cout, nx->relu_from, o1, st);
+    } else if (dual) {
+      rc = ctl_conv1x1_dual_nhwc_f16(o2, blk.c3.cin, a, hh, ww, blk.down.cin, s, n, blk.dual_w, blk.dual_b, out, blk.c3.cout, 1, st);
+    } else {
+      rc = run_conv(blk.c3, o2, n, h2, w2, r, out, st);
+    }
+    if (rc) return rc;
     a = out;
-    cur = (cur + 4) % 5;
+    cur = role[3];
+    o1_ready = chain ? role[0] : -1;
     hh = h2;
     ww = w2;
   }

@@ -215,23 +215,60 @@ class TrunkEngine:
                 N.check(L.ctl_maxpool3x3s2_nhwc_f16(s.data_ptr(), n, h, w, 64, a.data_ptr(), N.stream_ptr()))
         return a, n, hp, wp
 
+    def _chain(self, o2, a, res, n, h, w, h2, w2, blk, nxt: _Conv):
+        """The block's last convolution (dual form when `res` is None and the block has a shortcut branch, else conv3 +
+        residual) and the next block's conv1 in one launch (ctl_conv1x1_chain_nhwc_f16) -> (out, next conv1 output)."""
+        c3 = blk["conv3"]
+        dual = res is None and "down" in blk
+        out = torch.empty(n, h2, w2, c3.cout, dtype=torch.float16, device=self.device)
+        o1 = torch.empty(n, h2, w2, nxt.cout, dtype=torch.float16, device=self.device)
+        m = n * h2 * w2
+        k1 = c3.cin + (blk["down"].cin if dual else 0)
+        flops = 2.0 * m * c3.cout * k1 + 2.0 * m * nxt.cout * nxt.cin
+        # the block output is written once and never re-read; the next conv1's output is written once
+        nbytes = 2.0 * (m * k1 + m * c3.cout * (1 if dual else 2) + c3.cout * k1 + m * nxt.cout + nxt.cout * nxt.cin)
+        L = N.lib()
+        with self._timed("conv_chain", flops, nbytes):
+            if dual:
+                cd = blk["down"]
+                rc = L.ctl_conv1x1_chain_nhwc_f16(o2.data_ptr(), c3.cin, a.data_ptr(), h, w, cd.cin, cd.stride, n,
+                                                  blk["dual_w"].data_ptr(), blk["dual_b"].data_ptr(), None, out.data_ptr(),
+                                                  c3.cout, nxt.w.data_ptr(), nxt.b.data_ptr(), nxt.cout, nxt.relu_from,
+                                                  o1.data_ptr(), N.stream_ptr())
+            else:
+                rc = L.ctl_conv1x1_chain_nhwc_f16(o2.data_ptr(), c3.cin, None, h2, w2, 0, 1, n, c3.w.data_ptr(),
+                                                  c3.b.data_ptr(), res.data_ptr(), out.data_ptr(), c3.cout, nxt.w.data_ptr(),
+                                                  nxt.b.data_ptr(), nxt.cout, nxt.relu_from, o1.data_ptr(), N.stream_ptr())
+            N.check(rc)
+        return out, o1
+
     def bottlenecks(self, a, n, h, w):
         L = N.lib()
-        for blk in self.blocks:
-            o1, h1, w1 = self._conv(a, n, h, w, blk["conv1"])
+        o1 = None  # the block's conv1 output when the previous block's last launch computed it
+        for i, blk in enumerate(self.blocks):
+            if o1 is None:
+                o1, h1, w1 = self._conv(a, n, h, w, blk["conv1"])
+            else:
+                h1, w1 = h, w
             if "in" in blk:
                 half, g, b = blk["in"]
                 with self._timed("instnorm_relu", 0.0, 2.0 * 2 * n * h1 * w1 * half):
                     N.check(L.ctl_instnorm_relu_nhwc_f16(o1.data_ptr(), n, h1 * w1, blk["conv1"].cout, half,
                                                          g.data_ptr(), b.data_ptr(), BN_EPS, N.stream_ptr()))
             o2, h2, w2 = self._conv(o1, n, h1, w1, blk["conv2"])
-            if "down" in blk and h % blk["down"].stride == 0 and w % blk["down"].stride == 0:
-                a, h, w = self._dual(o2, a, n, h, w, h2, w2, blk)
-                continue
-            res = a
-            if "down" in blk:
+            dual = "down" in blk and h % blk["down"].stride == 0 and w % blk["down"].stride == 0
+            res = None if dual else a
+            if "down" in blk and not dual:
                 res, _, _ = self._conv(a, n, h, w, blk["down"])
-            a, h, w = self._conv(o2, n, h2, w2, blk["conv3"], residual=res)
+            nxt = self.blocks[i + 1]["conv1"] if i + 1 < len(self.blocks) else None
+            o1 = None
+            if nxt is not None and L.ctl_conv1x1_chain_supported(blk["conv3"].cout, nxt.cout):
+                a, o1 = self._chain(o2, a, res, n, h, w, h2, w2, blk, nxt)
+            elif dual:
+                a, _, _ = self._dual(o2, a, n, h, w, h2, w2, blk)
+            else:
+                a, _, _ = self._conv(o2, n, h2, w2, blk["conv3"], residual=res)
+            h, w = h2, w2
         return a, h, w
 
     def tail(self, a, n, h, w, want_base=False, want_emb=False):

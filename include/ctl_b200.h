@@ -253,6 +253,20 @@ int ctl_conv2d_nhwc_f16(const void* x, int32_t n, int32_t h, int32_t w, int32_t 
 int ctl_conv1x1_dual_nhwc_f16(const void* x1, int32_t cin1, const void* x2, int32_t h2, int32_t w2, int32_t cin2,
                               int32_t stride2, int32_t n, const void* weight_cat, const float* bias, void* out,
                               int32_t cout, int32_t relu, ctl_stream_t stream);
+/* The last 1x1 of a bottleneck and the first 1x1 of the next one in ONE launch (the block output is not re-read):
+ *   out [n][i][j][:] = relu( W[:, :cin1] x1[n][i][j][:] [+ W[:, cin1:] x2[n][i*stride2][j*stride2][:]] + bias
+ *                            [+ residual[n][i][j][:]] )
+ *   out2[n][i][j][c] = act_c( W2[c][:] out[n][i][j][:] + bias2[c] ),  act_c = ReLU for c >= relu_from2, identity below
+ * x2 != NULL is the K-concatenated form of ctl_conv1x1_dual_nhwc_f16 (no residual); x2 == NULL: x1 alone (stride2 = 1,
+ * cin2 ignored) with an optional residual [n][h2][w2][cout].  x1: [n][h2/stride2][w2/stride2][cin1]; weight
+ * [cout][cin1 (+ cin2)], weight2 [cout2][cout] fp16; out2 NHWC [n][h2/stride2][w2/stride2][cout2].  Both outputs are
+ * bit-identical to the two stand-alone launches.  Only shapes with ctl_conv1x1_chain_supported(cout, cout2) != 0 are
+ * accepted. */
+int32_t ctl_conv1x1_chain_supported(int32_t cout, int32_t cout2);
+int ctl_conv1x1_chain_nhwc_f16(const void* x1, int32_t cin1, const void* x2, int32_t h2, int32_t w2, int32_t cin2,
+                               int32_t stride2, int32_t n, const void* weight, const float* bias, const void* residual,
+                               void* out, int32_t cout, const void* weight2, const float* bias2, int32_t cout2,
+                               int32_t relu_from2, void* out2, ctl_stream_t stream);
 /* tensor-core stem: weight_k192_f16 = [64][192] fp16, k = (c*7 + r)*8 + s (s = 7 and k >= 168 zero) */
 int ctl_stem_conv7x7_tc(const float* x_nchw, int32_t n, int32_t h, int32_t w, const void* weight_k192_f16,
                         const float* bias, int32_t relu, void* out_nhwc_f16, ctl_stream_t stream);
