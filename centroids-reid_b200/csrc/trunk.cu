@@ -1,17 +1,19 @@
 // Whole-trunk entry points of the C ABI (SURVEY 8b: ctl_weights_pack + ctl_embed_forward): the layer graph of the eval
 // embedding path -- ResNet.forward / ResNet_IBN.forward (modelling/backbones/resnet.py:122-133, resnet_ibn_a.py:126-141),
 // Baseline.forward's global average pool (modelling/baseline.py:91-96) and the eval BatchNorm1d of
-// ModelBase.validation_step (modelling/bases.py:169-177) -- behind an opaque handle, so that a host that is not Python can
-// run `bn(backbone(x))` without re-implementing modelling/backbones/engine.py.
+// ModelBase.validation_step (modelling/bases.py:169-177) -- behind an opaque handle.  This is the eval trunk's only
+// driver: modelling/backbones/engine.py::TrunkEngine is its ctypes form, and a host that is not Python binds the same calls.
 //
 // The handle owns the PACKED operands: [Cout][kh][kw][Cin] fp16 weights with the eval BatchNorm folded in and fp32
-// biases, produced on the device from the reference's fp32 state_dict tensors (fold_pack_kernel: exactly the arithmetic
-// of engine.py::_fold, operation by operation, so both paths produce the same bits), the K-concatenated [W3 | Wd]
-// matrices of every first block, the two stem layouts, and the zero-bordered staging buffer of the fused stem.
-// Activations live in a caller-provided workspace.  The launches are the same C entry points engine.py calls.
+// biases, produced on the device from the reference's fp32 state_dict tensors (fold_pack_kernel: fp32 divide / sqrt /
+// multiply / subtract, each correctly rounded, then one rounding to fp16), the K-concatenated [W3 | Wd] matrices of every
+// first block, the two stem layouts, and one zero-bordered staging buffer of the fused stem per input shape.
+// Activations live in a caller-provided workspace.
 #include <math.h>
 #include <string.h>
 
+#include <array>
+#include <map>
 #include <string>
 #include <unordered_map>
 #include <vector>
@@ -46,8 +48,8 @@ __global__ void fold_pack_kernel(const float* __restrict__ w, int cout, int cin,
   if (threadIdx.x == 0 && bias != nullptr) bias[co] = accumulate ? __fadd_rn(bias[co], b) : b;
 }
 
-// stem layouts from the folded [64][3][7][7] weights (engine.py: stem_w = [64][192], k = (c*7 + r)*8 + s, s = 7 and
-// k >= 168 zero;  pack_stem_fused = [28][64][8], chunk = r*4 + s/2, element = (s%2)*4 + ch, ch == 3 and s == 7 zero)
+// stem layouts from the folded [64][3][7][7] weights (ctl_stem_conv7x7_tc: [64][192], k = (c*7 + r)*8 + s, s = 7 and
+// k >= 168 zero;  ctl_stem_pool_fused: [28][64][8], chunk = r*4 + s/2, element = (s%2)*4 + ch, ch == 3 and s == 7 zero)
 __global__ void stem_pack_kernel(const float* __restrict__ w, const float* __restrict__ gamma, const float* __restrict__ beta,
                                  const float* __restrict__ mean, const float* __restrict__ var, __half* __restrict__ w192,
                                  __half* __restrict__ w3, float* __restrict__ bias) {
@@ -85,6 +87,7 @@ struct PackedConv {
   int cin = 0, cout = 0, k = 1, stride = 1, relu = 1, relu_from = 0;
 };
 struct TrunkBlock {
+  std::string prefix;  // "layer<stage>.<block>" of the state_dict names
   PackedConv c1, c2, c3, down;
   bool has_down = false, has_in = false;
   int in_half = 0;
@@ -102,9 +105,10 @@ struct ctl_trunk {
   __half *stem_w192 = nullptr, *stem_w3 = nullptr;
   float* stem_b = nullptr;
   float *head_scale = nullptr, *head_shift = nullptr;
-  void* stem_pad = nullptr;
-  size_t stem_pad_bytes = 0;
-  int pad_n = 0, pad_h = 0, pad_w = 0;
+  // (n, h, w) -> zero-bordered staging buffer of the fused stem.  Kept until ctl_trunk_destroy: a CUDA graph captured at
+  // one shape still reads its buffer after calls at other shapes.
+  std::map<std::array<int, 3>, void*> stem_pads;
+  int32_t launches = 0;      // kernels launched by the last ctl_embed_* call
   std::vector<void*> owned;  // every cudaMalloc of this handle
 };
 
@@ -169,17 +173,20 @@ using namespace ctl;
 
 extern "C" {
 
-int ctl_trunk_create(ctl_trunk** out, int32_t ibn, int32_t last_stride) {
-  CTL_CHECK_ARG(out != nullptr, "null pointer");
+int ctl_trunk_create(ctl_trunk** out, int32_t ibn, int32_t last_stride, const int32_t stage_blocks[4]) {
+  CTL_CHECK_ARG(out != nullptr && stage_blocks != nullptr, "null pointer");
   CTL_CHECK_ARG(last_stride == 1 || last_stride == 2, "last_stride must be 1 or 2 (config/defaults.py:24)");
+  for (int li = 0; li < 4; ++li)
+    CTL_CHECK_ARG(stage_blocks[li] >= 1, "stage_blocks[%d] = %d: every stage needs at least one block", li, stage_blocks[li]);
   ctl_trunk* h = new ctl_trunk();
   h->ibn = ibn ? 1 : 0;
   h->last_stride = last_stride;
-  const int planes[4] = {64, 128, 256, 512}, nblk[4] = {3, 4, 6, 3};
+  const int planes[4] = {64, 128, 256, 512};
   int inplanes = 64;
   for (int li = 0; li < 4; ++li)
-    for (int bi = 0; bi < nblk[li]; ++bi) {
+    for (int bi = 0; bi < stage_blocks[li]; ++bi) {
       TrunkBlock blk;
+      blk.prefix = "layer" + std::to_string(li + 1) + "." + std::to_string(bi);
       const int stride0 = li == 0 ? 1 : (li == 3 ? last_stride : 2);
       blk.c1.cin = inplanes;
       blk.c1.cout = planes[li];
@@ -207,7 +214,6 @@ int ctl_trunk_create(ctl_trunk** out, int32_t ibn, int32_t last_stride) {
 void ctl_trunk_destroy(ctl_trunk* h) {
   if (!h) return;
   for (void* p : h->owned) cudaFree(p);
-  if (h->stem_pad) cudaFree(h->stem_pad);
   delete h;
 }
 
@@ -240,63 +246,59 @@ int ctl_weights_pack(ctl_trunk* h, const ctl_named_tensor* tensors, int32_t n_te
     CTL_LAUNCH_CHECK();
   }
   // ---- bottlenecks ----
-  const int nblk[4] = {3, 4, 6, 3};
-  size_t idx = 0;
-  for (int li = 0; li < 4; ++li)
-    for (int bi = 0; bi < nblk[li]; ++bi, ++idx) {
-      TrunkBlock& blk = h->blocks[idx];
-      const std::string p = "layer" + std::to_string(li + 1) + "." + std::to_string(bi);
-      if (blk.has_in) {
-        // IBN: channels [0, half) keep the raw convolution (InstanceNorm + ReLU follow as their own kernel), the
-        // BatchNorm half is folded; ReLU in the conv epilogue only from channel `half` on
-        if ((rc = pack_conv(h, m, p + ".conv1", p + ".bn1.BN", blk.c1.cout, blk.c1.cin, 1, blk.in_half, &blk.c1, st))) return rc;
-        blk.c1.relu_from = blk.in_half;
-        const float *ig = need(m, p + ".bn1.IN.weight", blk.in_half, &rc), *ib = need(m, p + ".bn1.IN.bias", blk.in_half, &rc);
-        if (rc) return rc;
-        if (!blk.in_gamma) {
-          blk.in_gamma = dev_alloc<float>(h, blk.in_half);
-          blk.in_beta = dev_alloc<float>(h, blk.in_half);
-        }
-        CTL_CUDA(cudaMemcpyAsync(blk.in_gamma, ig, blk.in_half * sizeof(float), cudaMemcpyDeviceToDevice, st));
-        CTL_CUDA(cudaMemcpyAsync(blk.in_beta, ib, blk.in_half * sizeof(float), cudaMemcpyDeviceToDevice, st));
-      } else {
-        if ((rc = pack_conv(h, m, p + ".conv1", p + ".bn1", blk.c1.cout, blk.c1.cin, 1, 0, &blk.c1, st))) return rc;
+  for (TrunkBlock& blk : h->blocks) {
+    const std::string& p = blk.prefix;
+    if (blk.has_in) {
+      // IBN: channels [0, half) keep the raw convolution (InstanceNorm + ReLU follow as their own kernel), the
+      // BatchNorm half is folded; ReLU in the conv epilogue only from channel `half` on
+      if ((rc = pack_conv(h, m, p + ".conv1", p + ".bn1.BN", blk.c1.cout, blk.c1.cin, 1, blk.in_half, &blk.c1, st))) return rc;
+      blk.c1.relu_from = blk.in_half;
+      const float *ig = need(m, p + ".bn1.IN.weight", blk.in_half, &rc), *ib = need(m, p + ".bn1.IN.bias", blk.in_half, &rc);
+      if (rc) return rc;
+      if (!blk.in_gamma) {
+        blk.in_gamma = dev_alloc<float>(h, blk.in_half);
+        blk.in_beta = dev_alloc<float>(h, blk.in_half);
       }
-      const int s2 = blk.c2.stride;
-      if ((rc = pack_conv(h, m, p + ".conv2", p + ".bn2", blk.c2.cout, blk.c2.cin, 3, 0, &blk.c2, st))) return rc;
-      blk.c2.stride = s2;
-      if ((rc = pack_conv(h, m, p + ".conv3", p + ".bn3", blk.c3.cout, blk.c3.cin, 1, 0, &blk.c3, st))) return rc;
-      if (blk.has_down) {
-        const int sd = blk.down.stride;
-        if ((rc = pack_conv(h, m, p + ".downsample.0", p + ".downsample.1", blk.down.cout, blk.down.cin, 1, 0, &blk.down, st))) return rc;
-        blk.down.stride = sd;
-        blk.down.relu = 0;
-        // [W3 | Wd] and bias3 + bias_d for the single-GEMM form of conv3 + shortcut (ctl_conv1x1_dual_nhwc_f16)
-        const int kt = blk.c3.cin + blk.down.cin;
-        if (!blk.dual_w) {
-          blk.dual_w = dev_alloc<__half>(h, (size_t)blk.c3.cout * kt);
-          blk.dual_b = dev_alloc<float>(h, blk.c3.cout);
-        }
-        if (!blk.dual_w || !blk.dual_b) {
-          set_error("ctl_weights_pack: out of device memory");
-          return (int)cudaErrorMemoryAllocation;
-        }
-        CTL_CUDA(cudaMemcpy2DAsync(blk.dual_w, (size_t)kt * 2, blk.c3.w, (size_t)blk.c3.cin * 2, (size_t)blk.c3.cin * 2, blk.c3.cout,
-                                   cudaMemcpyDeviceToDevice, st));
-        CTL_CUDA(cudaMemcpy2DAsync(blk.dual_w + blk.c3.cin, (size_t)kt * 2, blk.down.w, (size_t)blk.down.cin * 2,
-                                   (size_t)blk.down.cin * 2, blk.c3.cout, cudaMemcpyDeviceToDevice, st));
-        // bias3 + bias_d in fp32, like engine.py (c3.b + cd.b)
-        CTL_CUDA(cudaMemcpyAsync(blk.dual_b, blk.c3.b, blk.c3.cout * sizeof(float), cudaMemcpyDeviceToDevice, st));
-        const std::string d = p + ".downsample.1";
-        int rc2 = 0;
-        fold_pack_kernel<<<blk.c3.cout, 32, 0, st>>>(need(m, p + ".downsample.0.weight", (long long)blk.down.cout * blk.down.cin, &rc2), blk.down.cout, 0, 1,
-                                                     need(m, d + ".weight", blk.down.cout, &rc2), need(m, d + ".bias", blk.down.cout, &rc2),
-                                                     need(m, d + ".running_mean", blk.down.cout, &rc2),
-                                                     need(m, d + ".running_var", blk.down.cout, &rc2), 0, blk.down.w, 0, 0, blk.dual_b, 1);
-        CTL_LAUNCH_CHECK();
-        if (rc2) return rc2;
-      }
+      CTL_CUDA(cudaMemcpyAsync(blk.in_gamma, ig, blk.in_half * sizeof(float), cudaMemcpyDeviceToDevice, st));
+      CTL_CUDA(cudaMemcpyAsync(blk.in_beta, ib, blk.in_half * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    } else {
+      if ((rc = pack_conv(h, m, p + ".conv1", p + ".bn1", blk.c1.cout, blk.c1.cin, 1, 0, &blk.c1, st))) return rc;
     }
+    const int s2 = blk.c2.stride;
+    if ((rc = pack_conv(h, m, p + ".conv2", p + ".bn2", blk.c2.cout, blk.c2.cin, 3, 0, &blk.c2, st))) return rc;
+    blk.c2.stride = s2;
+    if ((rc = pack_conv(h, m, p + ".conv3", p + ".bn3", blk.c3.cout, blk.c3.cin, 1, 0, &blk.c3, st))) return rc;
+    if (blk.has_down) {
+      const int sd = blk.down.stride;
+      if ((rc = pack_conv(h, m, p + ".downsample.0", p + ".downsample.1", blk.down.cout, blk.down.cin, 1, 0, &blk.down, st))) return rc;
+      blk.down.stride = sd;
+      blk.down.relu = 0;
+      // [W3 | Wd] and bias3 + bias_d for the single-GEMM form of conv3 + shortcut (ctl_conv1x1_dual_nhwc_f16)
+      const int kt = blk.c3.cin + blk.down.cin;
+      if (!blk.dual_w) {
+        blk.dual_w = dev_alloc<__half>(h, (size_t)blk.c3.cout * kt);
+        blk.dual_b = dev_alloc<float>(h, blk.c3.cout);
+      }
+      if (!blk.dual_w || !blk.dual_b) {
+        set_error("ctl_weights_pack: out of device memory");
+        return (int)cudaErrorMemoryAllocation;
+      }
+      CTL_CUDA(cudaMemcpy2DAsync(blk.dual_w, (size_t)kt * 2, blk.c3.w, (size_t)blk.c3.cin * 2, (size_t)blk.c3.cin * 2, blk.c3.cout,
+                                 cudaMemcpyDeviceToDevice, st));
+      CTL_CUDA(cudaMemcpy2DAsync(blk.dual_w + blk.c3.cin, (size_t)kt * 2, blk.down.w, (size_t)blk.down.cin * 2,
+                                 (size_t)blk.down.cin * 2, blk.c3.cout, cudaMemcpyDeviceToDevice, st));
+      // bias3 + bias_d, one fp32 add per channel
+      CTL_CUDA(cudaMemcpyAsync(blk.dual_b, blk.c3.b, blk.c3.cout * sizeof(float), cudaMemcpyDeviceToDevice, st));
+      const std::string d = p + ".downsample.1";
+      int rc2 = 0;
+      fold_pack_kernel<<<blk.c3.cout, 32, 0, st>>>(need(m, p + ".downsample.0.weight", (long long)blk.down.cout * blk.down.cin, &rc2), blk.down.cout, 0, 1,
+                                                   need(m, d + ".weight", blk.down.cout, &rc2), need(m, d + ".bias", blk.down.cout, &rc2),
+                                                   need(m, d + ".running_mean", blk.down.cout, &rc2),
+                                                   need(m, d + ".running_var", blk.down.cout, &rc2), 0, blk.down.w, 0, 0, blk.dual_b, 1);
+      CTL_LAUNCH_CHECK();
+      if (rc2) return rc2;
+    }
+  }
   // ---- optional BatchNorm1d head (ModelBase.bn, modelling/bases.py:83) ----
   h->has_head = m.count("bn_head.weight") != 0;
   if (h->has_head) {
@@ -314,109 +316,217 @@ int ctl_weights_pack(ctl_trunk* h, const ctl_named_tensor* tensors, int32_t n_te
   return 0;
 }
 
-static size_t trunk_act_bytes(int n, int hgt, int wid) {
-  // largest activation of the trunk: the stem's conv output [n, H/2, W/2, 64] == layer1's output [n, H/4, W/4, 256]
-  const size_t h2 = (hgt + 6 - 7) / 2 + 1, w2 = (wid + 6 - 7) / 2 + 1;
-  return ((size_t)n * h2 * w2 * 64 * 2 + 255) & ~(size_t)255;
+}  // extern "C"
+
+namespace ctl {
+
+static size_t round256(size_t b) { return (b + 255) & ~(size_t)255; }
+static int stem_side(int s) { return (s + 6 - 7) / 2 + 1; }  // conv1 7x7 / 2, pad 3
+static int pool_side(int s) { return (s + 2 - 3) / 2 + 1; }  // maxpool 3x3 / 2, pad 1
+static bool fused_stem_fits(int hgt, int wid) { return hgt % 4 == 0 && wid % 2 == 0 && wid <= 128; }
+
+// One of the five activation slots of the bottleneck walk on a [n, hp, wp, 64] stem output: layer1's output
+// [n, hp, wp, 256] is the largest tensor the blocks write (each later stage halves both sides -- stride-2 convolutions
+// take even sides only -- before it doubles the channels).
+static size_t block_slot_bytes(int n, int hp, int wp) { return round256((size_t)n * hp * wp * 256 * 2); }
+// the tensor-core stem's conv output [n, h/2, w/2, 64], which is larger than a slot when h/2 or w/2 is odd
+static size_t stem_tmp_bytes(int n, int hgt, int wid) { return round256((size_t)n * stem_side(hgt) * stem_side(wid) * 64 * 2); }
+
+static int check_workspace(size_t need, size_t have) {
+  if (have < need) {
+    set_error("workspace too small: need %zu bytes, have %zu", need, have);
+    return CTL_ERR_WORKSPACE;
+  }
+  return 0;
 }
+
+// what every ctl_embed_* call checks once its arguments are valid
+static int begin_call(ctl_trunk* h) {
+  CTL_CHECK_ARG(h->packed, "ctl_weights_pack has not been called on this handle");
+  h->launches = 0;
+  return ctl_device_check();
+}
+
+static int stem_pad(ctl_trunk* h, int n, int hgt, int wid, cudaStream_t st, void** pad) {
+  const std::array<int, 3> key = {n, hgt, wid};
+  auto it = h->stem_pads.find(key);
+  if (it != h->stem_pads.end()) {
+    *pad = it->second;
+    return 0;
+  }
+  cudaStreamCaptureStatus capture;
+  CTL_CUDA(cudaStreamIsCapturing(st, &capture));
+  CTL_CHECK_ARG(capture == cudaStreamCaptureStatusNone,
+                "the fused stem's staging buffer for n=%d, %dx%d would be allocated during stream capture: run one call "
+                "at this shape on the handle before capturing",
+                n, hgt, wid);
+  const size_t bytes = ctl_stem_pad_bytes(n, hgt, wid);
+  void* p = dev_alloc<char>(h, bytes);
+  if (!p) {
+    set_error("out of device memory (stem staging buffer of %zu bytes)", bytes);
+    return (int)cudaErrorMemoryAllocation;
+  }
+  CTL_CUDA(cudaMemsetAsync(p, 0, bytes, st));  // the zero border is written once
+  h->stem_pads[key] = p;
+  *pad = p;
+  return 0;
+}
+
+// conv1 + bn1 (+ReLU for IBN-a) + maxpool -> out [n, hp, wp, 64]; x is fp32 NCHW, or uint8 NHWC when mean3 / std3 are
+// given (fused stem only).  The tensor-core stem's conv output goes to `tmp` (stem_tmp_bytes).
+static int run_stem(ctl_trunk* h, const void* x, const float* mean3, const float* std3, int n, int hgt, int wid, void* out,
+                    void* tmp, cudaStream_t st) {
+  int rc;
+  h->launches += 2;  // input packing + conv/pool, or conv + pool
+  if (fused_stem_fits(hgt, wid)) {
+    void* pad = nullptr;
+    if ((rc = stem_pad(h, n, hgt, wid, st, &pad))) return rc;
+    return mean3 ? ctl_stem_pool_fused_u8(x, n, hgt, wid, mean3, std3, pad, h->stem_w3, h->stem_b, h->ibn, out, st)
+                 : ctl_stem_pool_fused(static_cast<const float*>(x), n, hgt, wid, pad, h->stem_w3, h->stem_b, h->ibn, out, st);
+  }
+  if ((rc = ctl_stem_conv7x7_tc(static_cast<const float*>(x), n, hgt, wid, h->stem_w192, h->stem_b, h->ibn, tmp, st))) return rc;
+  return ctl_maxpool3x3s2_nhwc_f16(tmp, n, stem_side(hgt), stem_side(wid), 64, out, st);
+}
+
+static int run_conv(ctl_trunk* h, const PackedConv& c, const void* x, int n, int hh, int ww, const void* residual, void* out,
+                    cudaStream_t st) {
+  ++h->launches;
+  return ctl_conv2d_nhwc_f16(x, n, hh, ww, c.cin, c.w, c.b, residual, out, c.cout, c.k, c.stride, c.relu, c.relu_from, st);
+}
+
+// The bottleneck walk on x [n, hh, ww, 64].  Intermediates rotate through five workspace slots of `slot` bytes; x is
+// slot x_slot (recycled once read) or, with x_slot < 0, a caller tensor that is never written.  The last block writes
+// `out` when it is given, else a slot.  *y = the trunk output [n, *hh, *ww, 2048].
+static int run_blocks(ctl_trunk* h, const void* x, int x_slot, int n, int* hh, int* ww, char* ws, size_t slot, void* out,
+                      const void** y, cudaStream_t st) {
+  int rc;
+  void* const buf[5] = {ws, ws + slot, ws + 2 * slot, ws + 3 * slot, ws + 4 * slot};
+  const void* a = x;
+  int cur = x_slot;   // slot holding the block input; < 0: the caller's tensor
+  int o1_ready = -1;  // slot holding this block's conv1 output when the previous block's launch computed it
+  for (size_t bi = 0; bi < h->blocks.size(); ++bi) {
+    const TrunkBlock& blk = h->blocks[bi];
+    // roles of four slots other than the input's; a conv1 output computed ahead keeps its slot (dead again once conv2
+    // has read it, so the next chained launch writes there too) and the other roles rotate around it
+    int role[4], k = 0;
+    if (o1_ready >= 0) role[k++] = o1_ready;
+    for (int i = 1; i <= 5 && k < 4; ++i)
+      if ((cur + i) % 5 != cur && (cur + i) % 5 != o1_ready) role[k++] = (cur + i) % 5;
+    void* o1 = buf[role[0]];
+    void* o2 = buf[role[1]];
+    void* res = buf[role[2]];
+    void* dst = out && bi + 1 == h->blocks.size() ? out : buf[role[3]];
+    const int h1 = *hh, w1 = *ww;
+    if (o1_ready < 0 && (rc = run_conv(h, blk.c1, a, n, h1, w1, nullptr, o1, st))) return rc;
+    if (blk.has_in) {
+      ++h->launches;
+      if ((rc = ctl_instnorm_relu_nhwc_f16(o1, n, h1 * w1, blk.c1.cout, blk.in_half, blk.in_gamma, blk.in_beta, TRUNK_BN_EPS, st)))
+        return rc;
+    }
+    const int s = blk.c2.stride;
+    const int h2 = (h1 + 2 - 3) / s + 1, w2 = (w1 + 2 - 3) / s + 1;
+    if ((rc = run_conv(h, blk.c2, o1, n, h1, w1, nullptr, o2, st))) return rc;
+    const bool dual = blk.has_down && h1 % s == 0 && w1 % s == 0;
+    const void* r = a;
+    if (blk.has_down && !dual) {
+      if ((rc = run_conv(h, blk.down, a, n, h1, w1, nullptr, res, st))) return rc;
+      r = res;
+    }
+    // the next block's conv1 in this launch's epilogue: its output goes to o1's slot (a and res are still read)
+    const PackedConv* nx = bi + 1 < h->blocks.size() ? &h->blocks[bi + 1].c1 : nullptr;
+    const bool chain = nx && ctl_conv1x1_chain_supported(blk.c3.cout, nx->cout);
+    if (chain || dual) ++h->launches;  // run_conv counts the plain conv3
+    if (chain) {
+      if (dual)
+        rc = ctl_conv1x1_chain_nhwc_f16(o2, blk.c3.cin, a, h1, w1, blk.down.cin, s, n, blk.dual_w, blk.dual_b, nullptr, dst,
+                                        blk.c3.cout, nx->w, nx->b, nx->cout, nx->relu_from, o1, st);
+      else
+        rc = ctl_conv1x1_chain_nhwc_f16(o2, blk.c3.cin, nullptr, h2, w2, 0, 1, n, blk.c3.w, blk.c3.b, r, dst, blk.c3.cout,
+                                        nx->w, nx->b, nx->cout, nx->relu_from, o1, st);
+    } else if (dual) {
+      rc = ctl_conv1x1_dual_nhwc_f16(o2, blk.c3.cin, a, h1, w1, blk.down.cin, s, n, blk.dual_w, blk.dual_b, dst, blk.c3.cout, 1, st);
+    } else {
+      rc = run_conv(h, blk.c3, o2, n, h2, w2, r, dst, st);
+    }
+    if (rc) return rc;
+    a = dst;
+    cur = role[3];
+    o1_ready = chain ? role[0] : -1;
+    *hh = h2;
+    *ww = w2;
+  }
+  *y = a;
+  return 0;
+}
+
+// global average pool (+ the folded BatchNorm1d head when out_emb is given)
+static int run_head(ctl_trunk* h, const void* y, int n, int hw, float* out_feat, float* out_emb, cudaStream_t st) {
+  ++h->launches;
+  return ctl_gap_bn_nhwc_f16(y, n, hw, 2048, out_emb ? h->head_scale : nullptr, out_emb ? h->head_shift : nullptr, out_feat,
+                             out_emb, st);
+}
+
+}  // namespace ctl
+
+extern "C" {
 
 size_t ctl_embed_workspace_bytes(const ctl_trunk* h, int32_t n, int32_t hgt, int32_t wid) {
   if (!h || n < 1 || hgt < 8 || wid < 8) return 0;
-  return 5 * trunk_act_bytes(n, hgt, wid);
+  return 5 * std::max(block_slot_bytes(n, pool_side(stem_side(hgt)), pool_side(stem_side(wid))), stem_tmp_bytes(n, hgt, wid));
 }
 
-static int run_conv(const PackedConv& c, const void* x, int n, int hh, int ww, const void* residual, void* out, cudaStream_t st) {
-  return ctl_conv2d_nhwc_f16(x, n, hh, ww, c.cin, c.w, c.b, residual, out, c.cout, c.k, c.stride, c.relu, c.relu_from, st);
+int ctl_embed_stem(ctl_trunk* h, const void* x, int32_t n, int32_t hgt, int32_t wid, const float* mean3_host,
+                   const float* std3_host, void* out_nhwc, void* workspace, size_t workspace_bytes, ctl_stream_t stream) {
+  CTL_CHECK_ARG(h && x && out_nhwc && workspace, "null pointer");
+  CTL_CHECK_ARG(n >= 1 && hgt >= 8 && wid >= 8, "bad input shape");
+  CTL_CHECK_ARG((mean3_host == nullptr) == (std3_host == nullptr), "uint8 input needs both mean3_host and std3_host");
+  CTL_CHECK_ARG(!mean3_host || fused_stem_fits(hgt, wid), "uint8 input needs h %% 4 == 0 and an even w <= 128 (got %dx%d)", hgt,
+                wid);
+  int rc = check_workspace(ctl_embed_workspace_bytes(h, n, hgt, wid), workspace_bytes);
+  if (rc || (rc = begin_call(h))) return rc;
+  return run_stem(h, x, mean3_host, std3_host, n, hgt, wid, out_nhwc, workspace, (cudaStream_t)stream);
+}
+
+int ctl_embed_blocks(ctl_trunk* h, const void* x_nhwc, int32_t n, int32_t hgt, int32_t wid, void* out_nhwc, void* workspace,
+                     size_t workspace_bytes, ctl_stream_t stream) {
+  CTL_CHECK_ARG(h && x_nhwc && out_nhwc && workspace, "null pointer");
+  CTL_CHECK_ARG(n >= 1 && hgt >= 2 && wid >= 2, "bad activation shape");
+  const size_t slot = block_slot_bytes(n, hgt, wid);
+  int rc = check_workspace(5 * slot, workspace_bytes);
+  if (rc || (rc = begin_call(h))) return rc;
+  int hh = hgt, ww = wid;
+  const void* y = nullptr;
+  return run_blocks(h, x_nhwc, -1, n, &hh, &ww, static_cast<char*>(workspace), slot, out_nhwc, &y, (cudaStream_t)stream);
+}
+
+int ctl_embed_head(ctl_trunk* h, const void* x_nhwc, int32_t n, int32_t hw, float* out_feat, float* out_emb,
+                   ctl_stream_t stream) {
+  CTL_CHECK_ARG(h && x_nhwc && (out_feat || out_emb), "null pointer");
+  CTL_CHECK_ARG(n >= 1 && hw >= 1, "bad activation shape");
+  CTL_CHECK_ARG(out_emb == nullptr || h->has_head, "out_emb needs the bn_head.* tensors in ctl_weights_pack");
+  int rc = begin_call(h);
+  if (rc) return rc;
+  return run_head(h, x_nhwc, n, hw, out_feat, out_emb, (cudaStream_t)stream);
 }
 
 int ctl_embed_forward(ctl_trunk* h, const float* x_nchw, int32_t n, int32_t hgt, int32_t wid, float* out_feat, float* out_emb,
                       void* workspace, size_t workspace_bytes, ctl_stream_t stream) {
   CTL_CHECK_ARG(h && x_nchw && workspace && (out_feat || out_emb), "null pointer");
-  CTL_CHECK_ARG(h->packed, "ctl_weights_pack has not been called on this handle");
   CTL_CHECK_ARG(n >= 1 && hgt >= 8 && wid >= 8, "bad input shape");
   CTL_CHECK_ARG(out_emb == nullptr || h->has_head, "out_emb needs the bn_head.* tensors in ctl_weights_pack");
-  const size_t act = trunk_act_bytes(n, hgt, wid);
-  if (workspace_bytes < 5 * act) {
-    set_error("workspace too small: need %zu bytes, have %zu", 5 * act, workspace_bytes);
-    return CTL_ERR_WORKSPACE;
-  }
-  int rc = ctl_device_check();
-  if (rc) return rc;
+  int rc = check_workspace(ctl_embed_workspace_bytes(h, n, hgt, wid), workspace_bytes);
+  if (rc || (rc = begin_call(h))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
+  int hh = pool_side(stem_side(hgt)), ww = pool_side(stem_side(wid));
+  const size_t slot = block_slot_bytes(n, hh, ww);
   char* ws = static_cast<char*>(workspace);
-  void* buf[5] = {ws, ws + act, ws + 2 * act, ws + 3 * act, ws + 4 * act};
-  int hh = (hgt + 6 - 7) / 2 + 1, ww = (wid + 6 - 7) / 2 + 1;
-  const int hp = (hh + 2 - 3) / 2 + 1, wp = (ww + 2 - 3) / 2 + 1;
-  void* a = buf[0];
-  if (hgt % 4 == 0 && wid % 2 == 0 && wid <= 128) {
-    if (h->pad_n != n || h->pad_h != hgt || h->pad_w != wid) {
-      if (h->stem_pad) CTL_CUDA(cudaFree(h->stem_pad));
-      h->stem_pad = nullptr;
-      h->stem_pad_bytes = ctl_stem_pad_bytes(n, hgt, wid);
-      CTL_CUDA(cudaMalloc(&h->stem_pad, h->stem_pad_bytes));
-      CTL_CUDA(cudaMemsetAsync(h->stem_pad, 0, h->stem_pad_bytes, st));  // the zero border is written once
-      h->pad_n = n;
-      h->pad_h = hgt;
-      h->pad_w = wid;
-    }
-    if ((rc = ctl_stem_pool_fused(x_nchw, n, hgt, wid, h->stem_pad, h->stem_w3, h->stem_b, h->ibn, a, st))) return rc;
-  } else {
-    if ((rc = ctl_stem_conv7x7_tc(x_nchw, n, hgt, wid, h->stem_w192, h->stem_b, h->ibn, buf[1], st))) return rc;
-    if ((rc = ctl_maxpool3x3s2_nhwc_f16(buf[1], n, hh, ww, 64, a, st))) return rc;
-  }
-  hh = hp;
-  ww = wp;
-  int cur = 0;         // index of the buffer holding the block input
-  int o1_ready = -1;   // buffer holding this block's conv1 output when the previous block's launch computed it
-  for (size_t bi = 0; bi < h->blocks.size(); ++bi) {
-    const TrunkBlock& blk = h->blocks[bi];
-    // roles of the four buffers other than the input; a conv1 output computed ahead keeps its buffer (dead again once
-    // conv2 has read it, so the next chained launch writes there too) and the other roles rotate around it
-    int role[4], k = 0;
-    if (o1_ready >= 0) role[k++] = o1_ready;
-    for (int i = 1; i < 5; ++i)
-      if ((cur + i) % 5 != o1_ready && k < 4) role[k++] = (cur + i) % 5;
-    void* o1 = buf[role[0]];
-    void* o2 = buf[role[1]];
-    void* res = buf[role[2]];
-    void* out = buf[role[3]];
-    if (o1_ready < 0 && (rc = run_conv(blk.c1, a, n, hh, ww, nullptr, o1, st))) return rc;
-    if (blk.has_in)
-      if ((rc = ctl_instnorm_relu_nhwc_f16(o1, n, hh * ww, blk.c1.cout, blk.in_half, blk.in_gamma, blk.in_beta, TRUNK_BN_EPS, st)))
-        return rc;
-    const int s = blk.c2.stride;
-    const int h2 = (hh + 2 - 3) / s + 1, w2 = (ww + 2 - 3) / s + 1;
-    if ((rc = run_conv(blk.c2, o1, n, hh, ww, nullptr, o2, st))) return rc;
-    const bool dual = blk.has_down && hh % s == 0 && ww % s == 0;
-    const void* r = a;
-    if (blk.has_down && !dual) {
-      if ((rc = run_conv(blk.down, a, n, hh, ww, nullptr, res, st))) return rc;
-      r = res;
-    }
-    // the next block's conv1 in this launch's epilogue: its output goes to o1's buffer (a and res are still read)
-    const PackedConv* nx = bi + 1 < h->blocks.size() ? &h->blocks[bi + 1].c1 : nullptr;
-    const bool chain = nx && ctl_conv1x1_chain_supported(blk.c3.cout, nx->cout);
-    if (chain) {
-      if (dual)
-        rc = ctl_conv1x1_chain_nhwc_f16(o2, blk.c3.cin, a, hh, ww, blk.down.cin, s, n, blk.dual_w, blk.dual_b, nullptr, out,
-                                        blk.c3.cout, nx->w, nx->b, nx->cout, nx->relu_from, o1, st);
-      else
-        rc = ctl_conv1x1_chain_nhwc_f16(o2, blk.c3.cin, nullptr, h2, w2, 0, 1, n, blk.c3.w, blk.c3.b, r, out, blk.c3.cout,
-                                        nx->w, nx->b, nx->cout, nx->relu_from, o1, st);
-    } else if (dual) {
-      rc = ctl_conv1x1_dual_nhwc_f16(o2, blk.c3.cin, a, hh, ww, blk.down.cin, s, n, blk.dual_w, blk.dual_b, out, blk.c3.cout, 1, st);
-    } else {
-      rc = run_conv(blk.c3, o2, n, h2, w2, r, out, st);
-    }
-    if (rc) return rc;
-    a = out;
-    cur = role[3];
-    o1_ready = chain ? role[0] : -1;
-    hh = h2;
-    ww = w2;
-  }
-  return ctl_gap_bn_nhwc_f16(a, n, hh * ww, 2048, out_emb ? h->head_scale : nullptr, out_emb ? h->head_shift : nullptr, out_feat,
-                             out_emb, st);
+  // the stem writes slot 0; the tensor-core stem's temporary (at most one activation) starts at slot 1
+  if ((rc = run_stem(h, x_nchw, nullptr, nullptr, n, hgt, wid, ws, ws + slot, st))) return rc;
+  const void* y = nullptr;
+  if ((rc = run_blocks(h, ws, 0, n, &hh, &ww, ws, slot, nullptr, &y, st))) return rc;
+  return run_head(h, y, n, hh * ww, out_feat, out_emb, st);
 }
+
+int32_t ctl_embed_launches(const ctl_trunk* h) { return h ? h->launches : 0; }
 
 }  // extern "C"

@@ -3,7 +3,8 @@
 These modules exist so that `state_dict()` keys, shapes and the optimizer's named_parameters
 are IDENTICAL to modelling/backbones/resnet.py:90-120 and resnet_ibn_a.py:77-124 of the
 reference (checkpoints load unchanged).  They carry no arithmetic: the forward pass is the
-H100 engine (engine.py); the layer graph is described there, not here.
+H100 engine (engine.py, engine_train.py); the layer graph is described by the C handles they
+drive (csrc/trunk.cu, csrc/trunk_train.cu), not here.
 """
 from __future__ import annotations
 

@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define CTL_ABI_VERSION 2
+#define CTL_ABI_VERSION 3
 
 #define CTL_OK 0
 #define CTL_ERR_INVALID_ARGUMENT (-1)
@@ -296,8 +296,10 @@ int ctl_instnorm_relu_nhwc_f16(void* x, int32_t n, int32_t hw, int32_t c, int32_
 /* ---- whole-trunk entry points (SURVEY 8b): the eval embedding path bn(backbone(x)) behind an opaque handle ----
  * replaces: ResNet.forward / ResNet_IBN.forward (modelling/backbones/resnet.py:122-133, resnet_ibn_a.py:126-141),
  * Baseline.forward's pooling (modelling/baseline.py:91-96), ModelBase.validation_step / inference_utils._inference
- * (modelling/bases.py:169-177, inference/inference_utils.py:104-113).
- *   ctl_trunk_create   : ResNet50 (3,4,6,3 bottlenecks) or ResNet50-IBN-a (`ibn` != 0), MODEL.LAST_STRIDE 1 or 2.
+ * (modelling/bases.py:169-177, inference/inference_utils.py:104-113).  This is the eval trunk's only driver;
+ * modelling/backbones/engine.py::TrunkEngine is its ctypes form.
+ *   ctl_trunk_create   : bottleneck ResNet with `stage_blocks` blocks per stage ({3, 4, 6, 3} = ResNet50, {3, 4, 23, 3} =
+ *                        ResNet101, {3, 8, 36, 3} = ResNet152, each >= 1), IBN-a when `ibn` != 0, MODEL.LAST_STRIDE 1 or 2.
  *   ctl_weights_pack   : `tensors` = the reference's `base.*`-stripped state_dict as DEVICE fp32 pointers, by name
  *                        ("conv1.weight", "bn1.running_var", "layer3.0.downsample.1.bias", "layer1.0.bn1.IN.weight", ...),
  *                        plus optionally "bn_head.weight|bias|running_mean|running_var" (ModelBase.bn, [2048]).  Folds every
@@ -305,20 +307,42 @@ int ctl_instnorm_relu_nhwc_f16(void* x, int32_t n, int32_t hw, int32_t c, int32_
  *                        handle.  Call again whenever the parameters change (after opt.step(), load_state_dict).
  *   ctl_embed_forward  : x NCHW fp32 [n][3][h][w] on the device -> out_feat [n][2048] (global_feat) and / or out_emb
  *                        [n][2048] (= eval BatchNorm1d(global_feat); needs the bn_head.* tensors).  Activations live in the
- *                        caller's workspace of ctl_embed_workspace_bytes(...) bytes.  All launches go to `stream`.
- * The handle is per device and not thread-safe; a missing / mis-sized tensor is CTL_ERR_INVALID_ARGUMENT naming it. */
+ *                        caller's workspace of ctl_embed_workspace_bytes(h, n, h, w) bytes.  The entry point for C hosts:
+ *                        stem -> blocks -> head below in one call.
+ * The same forward in three stages, for hosts that capture or time them separately; NHWC fp16 tensors between them are
+ * the caller's:
+ *   ctl_embed_stem     : conv1 7x7/2 + bn1 (+ReLU for IBN-a) + maxpool 3x3/2 -> out [n][hp][wp][64], hp = (h/2 - 1)/2 + 1
+ *                        with h/2 = (h - 1)/2 + 1 (wp alike).  x is fp32 NCHW [n][3][h][w], or with mean3_host and std3_host
+ *                        uint8 NHWC [n][h][w][3] crops normalised as ctl_stem_pool_fused_u8 does (h % 4 == 0, even w <= 128).
+ *                        Workspace: ctl_embed_workspace_bytes(h, n, h, w) bytes (the tensor-core stem's temporary).
+ *   ctl_embed_blocks   : x [n][hp][wp][64] -> out [n][ho][wo][2048] (ho = hp / 4, / 8 with last_stride 2).  Never writes x.
+ *                        Workspace: ctl_embed_workspace_bytes(h, n, 4 * hp, 4 * wp) bytes, no more than the image size needs.
+ *   ctl_embed_head     : x [n][hw][2048] -> out_feat and / or out_emb as ctl_embed_forward.
+ *   ctl_embed_launches : kernels launched by the handle's last ctl_embed_* call.
+ * The fused stem (h % 4 == 0, even w <= 128) stages its input in a zero-bordered buffer that the handle allocates at the
+ * first call with each (n, h, w) and keeps until ctl_trunk_destroy; a call that would allocate one while `stream` is
+ * capturing a graph is CTL_ERR_INVALID_ARGUMENT, so capture after one eager call at the same shape.
+ * The handle is per device and not thread-safe; all launches go to `stream`; a missing / mis-sized tensor is
+ * CTL_ERR_INVALID_ARGUMENT naming it. */
 typedef struct ctl_trunk ctl_trunk;
 typedef struct ctl_named_tensor {
   const char* name;
   const float* data; /* device pointer */
   int64_t numel;
 } ctl_named_tensor;
-int ctl_trunk_create(ctl_trunk** out, int32_t ibn, int32_t last_stride);
+int ctl_trunk_create(ctl_trunk** out, int32_t ibn, int32_t last_stride, const int32_t stage_blocks[4]);
 void ctl_trunk_destroy(ctl_trunk* h);
 int ctl_weights_pack(ctl_trunk* h, const ctl_named_tensor* tensors, int32_t n_tensors, ctl_stream_t stream);
 size_t ctl_embed_workspace_bytes(const ctl_trunk* h, int32_t n, int32_t height, int32_t width);
 int ctl_embed_forward(ctl_trunk* h, const float* x_nchw, int32_t n, int32_t height, int32_t width, float* out_feat,
                       float* out_emb, void* workspace, size_t workspace_bytes, ctl_stream_t stream);
+int ctl_embed_stem(ctl_trunk* h, const void* x, int32_t n, int32_t height, int32_t width, const float* mean3_host,
+                   const float* std3_host, void* out_nhwc, void* workspace, size_t workspace_bytes, ctl_stream_t stream);
+int ctl_embed_blocks(ctl_trunk* h, const void* x_nhwc, int32_t n, int32_t height, int32_t width, void* out_nhwc,
+                     void* workspace, size_t workspace_bytes, ctl_stream_t stream);
+int ctl_embed_head(ctl_trunk* h, const void* x_nhwc, int32_t n, int32_t hw, float* out_feat, float* out_emb,
+                   ctl_stream_t stream);
+int32_t ctl_embed_launches(const ctl_trunk* h);
 
 /* ---- training-side trunk kernels (autograd through modelling/backbones/resnet.py:67-87 in train mode) ---- */
 

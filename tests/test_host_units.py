@@ -111,6 +111,10 @@ def test_c_abi_argument_errors_are_reported_without_a_gpu():
         lambda: L.ctl_trainer_create(C.byref(C.c_void_p()), 0, 3, 0.1, r50),                                 # LAST_STRIDE 3
         lambda: L.ctl_trainer_create(C.byref(C.c_void_p()), 0, 1, 0.0, r50),                                 # momentum 0
         lambda: L.ctl_trainer_create(C.byref(C.c_void_p()), 0, 1, 0.1, (C.c_int32 * 4)(3, 0, 6, 3)),         # empty stage
+        lambda: L.ctl_trunk_create(None, 0, 1, r50),                                                          # null handle
+        lambda: L.ctl_trunk_create(C.byref(C.c_void_p()), 0, 1, None),                                       # null stages
+        lambda: L.ctl_trunk_create(C.byref(C.c_void_p()), 0, 3, r50),                                        # LAST_STRIDE 3
+        lambda: L.ctl_trunk_create(C.byref(C.c_void_p()), 0, 1, (C.c_int32 * 4)(3, 4, 0, 3)),                # empty stage
     ]
     for i, call in enumerate(cases):
         rc = call()
@@ -145,6 +149,53 @@ def test_trainer_handle_plans_its_workspace_without_a_gpu():
         assert b"forward" in L.ctl_last_error()
         L.ctl_trainer_destroy(h)
         L.ctl_trainer_destroy(h101)
+
+
+def test_trunk_handle_stage_calls_check_arguments_without_a_gpu():
+    """The eval trunk's entry points reject null pointers (CTL_ERR_INVALID_ARGUMENT) and a short workspace
+    (CTL_ERR_WORKSPACE) before any device work.  One workspace size covers every entry point: five of the largest
+    activation, which is layer1's output when the stem's conv output has odd sides."""
+    import ctypes as C
+
+    from ctl_b200 import _native as N
+
+    L = N.lib()
+    one = C.c_void_p(256)
+    h = C.c_void_p()
+    assert L.ctl_trunk_create(C.byref(h), 0, 1, (C.c_int32 * 4)(3, 4, 6, 3)) == 0
+    try:
+        n, H, W, hp, wp = 2, 256, 128, 64, 32
+        need = L.ctl_embed_workspace_bytes(h, n, H, W)
+        assert need == 5 * n * 128 * 64 * 64 * 2  # the stem's conv output == layer1's output
+        assert L.ctl_embed_workspace_bytes(h, n, 4 * hp, 4 * wp) == need
+        # 110 x 62: conv output 55 x 31, pooled 28 x 16; layer1's output [28, 16, 256] is the largest activation
+        assert L.ctl_embed_workspace_bytes(h, n, 110, 62) >= 5 * n * 28 * 16 * 256 * 2
+        assert L.ctl_embed_workspace_bytes(h, 0, H, W) == 0 and L.ctl_embed_workspace_bytes(None, n, H, W) == 0
+        mean = (C.c_float * 3)(0.5, 0.5, 0.5)
+        cases = [
+            (-1, lambda: L.ctl_embed_stem(h, None, n, H, W, None, None, one, one, need, None)),
+            (-1, lambda: L.ctl_embed_stem(h, one, n, H, W, None, None, None, one, need, None)),
+            (-1, lambda: L.ctl_embed_stem(h, one, n, H, W, mean, None, one, one, need, None)),     # mean without std
+            (-1, lambda: L.ctl_embed_stem(h, one, n, 96, 160, mean, mean, one, one, need, None)),  # uint8, W > 128
+            (-1, lambda: L.ctl_embed_blocks(h, None, n, hp, wp, one, one, need, None)),
+            (-1, lambda: L.ctl_embed_blocks(h, one, n, hp, wp, None, one, need, None)),
+            (-1, lambda: L.ctl_embed_blocks(h, one, n, hp, wp, one, None, need, None)),
+            (-1, lambda: L.ctl_embed_head(h, None, n, 128, one, None, None)),
+            (-1, lambda: L.ctl_embed_head(h, one, n, 128, None, None, None)),
+            (-1, lambda: L.ctl_embed_forward(h, None, n, H, W, one, None, one, need, None)),
+            (-2, lambda: L.ctl_embed_stem(h, one, n, H, W, None, None, one, one, need - 1, None)),
+            (-2, lambda: L.ctl_embed_blocks(h, one, n, hp, wp, one, one, need - 1, None)),
+            (-2, lambda: L.ctl_embed_forward(h, one, n, H, W, one, None, one, need - 1, None)),
+            # a handle without packed weights: after the argument checks, before the device
+            (-1, lambda: L.ctl_embed_head(h, one, n, 128, one, None, None)),
+        ]
+        for i, (want, call) in enumerate(cases):
+            assert call() == want, (i, L.ctl_last_error())
+            assert len(L.ctl_last_error()) > 0
+        assert b"ctl_weights_pack" in L.ctl_last_error()
+        assert L.ctl_embed_launches(h) == 0
+    finally:
+        L.ctl_trunk_destroy(h)
 
 
 def test_identity_orders_and_encoded_ids_on_the_host():

@@ -285,31 +285,104 @@ def test_trunk_matches_reference_under_autocast(tag, ibn, hw):
 
 
 @pytest.mark.parametrize("ibn,hw,n", [(False, (256, 128), 6), (True, (320, 320), 3), (True, (128, 64), 5), (False, (96, 48), 2)])
-def test_native_trunk_handle_matches_engine(ibn, hw, n):
-    """SURVEY 8b: ctl_trunk_create + ctl_weights_pack + ctl_embed_forward -- the layer graph behind the C ABI, packing
-    done on the device from the fp32 state_dict -- must reproduce the Python-hosted engine BIT FOR BIT (same kernels,
-    same folded operands), with and without the BatchNorm1d head, across re-packs."""
+def test_trunk_stage_calls_match_embed_forward(ibn, hw, n):
+    """SURVEY 8b: TrunkEngine's three stage calls (ctl_embed_stem -> ctl_embed_blocks -> ctl_embed_head) must reproduce
+    ctl_embed_forward, the one-call entry point for C hosts, on the same handle BIT FOR BIT and with the same launch
+    count, with and without the BatchNorm1d head, across re-packs."""
     from ctl_b200 import _native as N
-    from ctl_b200.modelling.backbones.engine import NativeTrunk, TrunkEngine
+    from ctl_b200.modelling.backbones.engine import TrunkEngine
 
+    L = N.lib()
     sd = O.make_trunk_state(seed=5, ibn=ibn)
     head = dict(weight=torch.rand(2048) + 0.5, bias=torch.randn(2048) * 0.1, running_mean=torch.randn(2048) * 0.1,
                 running_var=torch.rand(2048) + 0.5)
     x = torch.randn(n, 3, *hw, generator=torch.Generator().manual_seed(8)).cuda()
-    ref = TrunkEngine(sd, "cuda", ibn=ibn, bn_head=head).forward(x, want_emb=True)
-    nat = NativeTrunk(sd, "cuda", ibn=ibn, bn_head=head)
-    out = nat.forward(x, want_emb=True)
-    assert torch.equal(out["global_feat"], ref["global_feat"]) and torch.equal(out["emb"], ref["emb"])
-    sd2 = O.make_trunk_state(seed=6, ibn=ibn)
-    nat.pack(sd2)  # re-pack (parameters changed), this time without a head
-    out2 = nat.forward(x)
-    assert torch.equal(out2["global_feat"], TrunkEngine(sd2, "cuda", ibn=ibn).forward(x)["global_feat"])
+    eng = TrunkEngine(sd, "cuda", ibn=ibn, bn_head=head)
+    ws = torch.empty(L.ctl_embed_workspace_bytes(eng._h, n, *hw), dtype=torch.uint8, device="cuda")
+
+    def embed_forward(want_emb):
+        feat = torch.empty(n, 2048, device="cuda")
+        emb = torch.empty(n, 2048, device="cuda") if want_emb else None
+        N.check(L.ctl_embed_forward(eng._h, x.data_ptr(), n, hw[0], hw[1], feat.data_ptr(), N.ptr(emb), ws.data_ptr(),
+                                    ws.numel(), N.stream_ptr()))
+        return feat, emb
+
+    out = eng.forward(x, want_emb=True)
+    feat, emb = embed_forward(True)
+    assert torch.equal(out["global_feat"], feat) and torch.equal(out["emb"], emb)
+    assert L.ctl_embed_launches(eng._h) == eng.launches_per_forward
+    eng.pack(O.make_trunk_state(seed=6, ibn=ibn))  # re-pack (parameters changed), this time without a head
+    out2 = eng.forward(x, want_emb=True)
+    assert "emb" not in out2
+    feat2, _ = embed_forward(False)
+    assert torch.equal(out2["global_feat"], feat2) and not torch.equal(feat2, feat)
     with pytest.raises(ValueError, match="bn_head"):
-        N.check(N.lib().ctl_embed_forward(nat._h, x.data_ptr(), n, hw[0], hw[1], out["global_feat"].data_ptr(),
-                                          out["emb"].data_ptr(), nat._ws.data_ptr(), nat._ws.numel(), N.stream_ptr()))
+        N.check(L.ctl_embed_forward(eng._h, x.data_ptr(), n, hw[0], hw[1], feat.data_ptr(), emb.data_ptr(), ws.data_ptr(),
+                                    ws.numel(), N.stream_ptr()))
     bad = {k: v for k, v in sd.items() if k != "layer2.1.bn2.running_var"}
     with pytest.raises(ValueError, match="layer2.1.bn2.running_var"):
-        nat.pack(bad)
+        eng.pack(bad)
+
+
+@pytest.mark.parametrize("tag,layers,ibn,hw", [
+    ("r101", (3, 4, 23, 3), False, (128, 64)),
+    ("r101_ibn", (3, 4, 23, 3), True, (128, 64)),
+    # 110 x 62 takes the tensor-core stem, whose conv output (55 x 31) has odd sides: layer1's output is then larger
+    # than the stem's, and the workspace must be sized for it
+    ("r50_odd_stem", (3, 4, 6, 3), False, (110, 62)),
+])
+def test_trunk_variants_match_checker(tag, layers, ibn, hw):
+    """The deeper trunks Baseline evaluates (MODEL.NAME resnet101 / resnet101_ibn_a) through the same handle, against
+    the fp16-rounding checker at the tolerance of test_full_trunk_matches_checker_and_reference_golden."""
+    from ctl_b200.modelling.backbones.engine import TrunkEngine
+
+    sd = O.make_trunk_state(seed=7, ibn=ibn, layers=layers)
+    x = torch.randn(2, 3, *hw, generator=torch.Generator().manual_seed(21))
+    feat = TrunkEngine(sd, "cuda", ibn=ibn, layers=layers).forward(x.cuda())["global_feat"].cpu()
+    with torch.no_grad():
+        _, sim = O.trunk_forward_fp16sim(x, sd, ibn=ibn, layers=layers)
+    scale = float(sim.abs().max())
+    err = float((feat - sim).abs().max())
+    print(f"{tag}: |feat|max {scale:.4f}  err vs fp16-sim {err:.3e}")
+    assert err <= 3e-3 * scale
+
+
+def test_bottlenecks_never_write_their_input():
+    """bench.py replays the bottleneck segment many times on one stem output: the segment must leave it untouched and
+    compute the same bits every time."""
+    from ctl_b200.modelling.backbones.engine import TrunkEngine
+
+    eng = TrunkEngine(O.make_trunk_state(seed=3), "cuda")
+    x = torch.randn(4, 3, 256, 128, generator=torch.Generator().manual_seed(2)).cuda()
+    a, n, h, w = eng.stem(x)
+    before = a.clone()
+    y1, h1, w1 = eng.bottlenecks(a, n, h, w)
+    y1 = y1.clone()
+    y2, h2, w2 = eng.bottlenecks(a, n, h, w)
+    assert torch.equal(a, before)
+    assert (h1, w1) == (h2, w2) and torch.equal(y1, y2)
+
+
+def test_graph_outlives_calls_at_other_shapes():
+    """A CUDA graph captured at one input shape reads the handle's stem staging buffer and its own workspace: both must
+    stay valid after eager forwards and captures at other shapes (fused and tensor-core stems)."""
+    from ctl_b200.modelling.backbones.engine import GraphedForward, TrunkEngine
+
+    head = dict(weight=torch.rand(2048) + 0.5, bias=torch.randn(2048) * 0.1, running_mean=torch.randn(2048) * 0.1,
+                running_var=torch.rand(2048) + 0.5)
+    eng = TrunkEngine(O.make_trunk_state(seed=4), "cuda", bn_head=head)
+    gen = torch.Generator().manual_seed(6)
+    xa = torch.randn(4, 3, 128, 64, generator=gen).cuda()
+    ga = GraphedForward(eng, xa, want_emb=True)
+    for shape in ((2, 3, 96, 48), (3, 3, 64, 160)):
+        xb = torch.randn(*shape, generator=gen).cuda()
+        eng.forward(xb, want_emb=True)
+        gb = GraphedForward(eng, xb, want_emb=True)
+        assert torch.equal(gb()["emb"], eng.forward(xb, want_emb=True)["emb"])
+    torch.cuda.synchronize()
+    out = ga()
+    ref = eng.forward(xa, want_emb=True)
+    assert torch.equal(out["emb"], ref["emb"]) and torch.equal(out["global_feat"], ref["global_feat"])
 
 
 @pytest.mark.parametrize("ibn,shape", [(False, (6, 256, 128)), (True, (3, 64, 32)), (False, (2, 96, 160))])
