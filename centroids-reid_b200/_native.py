@@ -19,6 +19,8 @@ CTL_DIST_COSINE = 1
 CTL_FLAG_NORMALIZE = 2
 CTL_DIST_SQRT = 4
 CTL_FLAG_EXACT_PASS = 8
+CTL_BLOCK_BOTTLENECK = 0
+CTL_BLOCK_BASIC = 1
 
 _ERRORS = {
     -1: ValueError,   # CTL_ERR_INVALID_ARGUMENT
@@ -97,10 +99,13 @@ SIGNATURES = {
     "ctl_xent_smooth_step": (C.c_int, [_p, _i32, _i32, _p, _f, _p, _p, _p, _sz, _p]),
     "ctl_conv2d_nhwc_f16": (C.c_int, [_p, _i32, _i32, _i32, _i32, _p, _p, _p, _p, _i32, _i32, _i32, _i32, _i32, _p]),
     "ctl_conv1x1_dual_nhwc_f16": (C.c_int, [_p, _i32, _p, _i32, _i32, _i32, _i32, _i32, _p, _p, _p, _i32, _i32, _p]),
+    "ctl_conv3x3_dual_nhwc_f16": (C.c_int, [_p, _i32, _p, _i32, _i32, _i32, _i32, _i32, _p, _p, _p, _i32, _i32, _p]),
     "ctl_conv1x1_chain_supported": (_i32, [_i32, _i32]),
     "ctl_conv1x1_chain_nhwc_f16": (C.c_int, [_p, _i32, _p, _i32, _i32, _i32, _i32, _i32, _p, _p, _p, _p, _i32, _p, _p,
                                              _i32, _i32, _p, _p]),
     "ctl_trunk_create": (C.c_int, [C.POINTER(_p), _i32, _i32, C.POINTER(_i32)]),
+    "ctl_trunk_create_ex": (C.c_int, [C.POINTER(_p), _i32, _i32, _i32, C.POINTER(_i32)]),
+    "ctl_trunk_feature_dim": (_i32, [_p]),
     "ctl_trunk_destroy": (None, [_p]),
     "ctl_weights_pack": (C.c_int, [_p, C.POINTER(NamedTensor), _i32, _p]),
     "ctl_embed_workspace_bytes": (_sz, [_p, _i32, _i32, _i32]),
@@ -110,6 +115,8 @@ SIGNATURES = {
     "ctl_embed_head": (C.c_int, [_p, _p, _i32, _i32, _p, _p, _p]),
     "ctl_embed_launches": (_i32, [_p]),
     "ctl_trainer_create": (C.c_int, [C.POINTER(_p), _i32, _i32, C.c_float, C.POINTER(_i32)]),
+    "ctl_trainer_create_ex": (C.c_int, [C.POINTER(_p), _i32, _i32, _i32, C.c_float, C.POINTER(_i32)]),
+    "ctl_trainer_feature_dim": (_i32, [_p]),
     "ctl_trainer_destroy": (None, [_p]),
     "ctl_trainer_bind": (C.c_int, [_p, C.POINTER(NamedTensor), _i32, C.POINTER(NamedTensor), _i32]),
     "ctl_train_workspace_bytes": (_sz, [_p, _i32, _i32, _i32]),

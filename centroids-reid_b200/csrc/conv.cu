@@ -66,6 +66,9 @@ struct ConvKernelParams {
   CUtensorMap out2_map;  // NHWC [.., N2] output, box {64 ch, TW, TH, 1}
   const float* bias2;    // [N2]
   int relu_from2;
+  // tap 9: the shortcut of the K-concatenated 3x3 + 1x1 form (ctl_conv3x3_dual_nhwc_f16).  It sits outside taps[]
+  // because a ten-entry array changes the register allocation of conv_gemm_kernel<256> (more spill traffic).
+  ConvTap tap9;
 };
 
 template <int BN>
@@ -207,7 +210,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid
       for (int tile = t_begin; tile < t_end; ++tile, it.next(p)) {
         const int h0 = it.th * p.TH, w0 = it.tw * p.TW;
         for (int t = 0; t < p.n_taps; ++t) {
-          const ConvTap tap = p.taps[t];
+          const ConvTap tap = t < 9 ? p.taps[t] : p.tap9;
           for (int cb = 0; cb < tap.cblocks; ++cb) {
             mbar_wait(empty_bar(stage), phase ^ 1u);
             const uint32_t dst = smem_base + stage * Cfg::STAGE_BYTES;
@@ -375,12 +378,25 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid
 // 128-byte lines needs NO descriptor base_offset (tests/test_trunk_gpu.py::test_conv_shapes[case3]
 // pins this).  36 KiB of fill per tile instead of 216 KiB.  Consumer warpgroup wg computes output
 // rows [8 wg, 8 wg + 8) of the tile (M = 64, N = 64).
+//
+// RES (a BasicBlock's layer1 conv2, identity shortcut): the tile's [128 px][64 ch] residual is one more TMA box of the
+// output's geometry, landed in its own 16 KiB slab in the swizzled layout store_subtile_f16 reads.  Shared memory:
+// 72 KiB weights + 2 x 36 KiB halos + 4 x 16 KiB output slabs + 16 KiB residual + 512 B bias + barriers and the
+// 1 KiB alignment slack = 225.75 KiB of the 227 KiB an SM grants one CTA.  A second producer thread (warp 1) owns the
+// residual slab: it loads tile t + 1's residual as soon as the epilogue of tile t has read the slab, while the
+// consumers run tile t + 1's MMAs, so the halo ring never waits on it.
 // ---------------------------------------------------------------------------------------
 static constexpr int C64_HALO_BYTES = 18 * 16 * 128;  // 36 KiB
 static constexpr int C64_W_BYTES = 9 * 64 * 128;      // 72 KiB
 static constexpr int C64_HALOS = 2;
 static constexpr int C64_OUT_SLABS = 4;
-static constexpr size_t C64_SMEM = C64_W_BYTES + C64_HALOS * C64_HALO_BYTES + C64_OUT_SLABS * A_TILE_BYTES + 512 + 1024 + 256;
+template <bool RES>
+struct C64Cfg {
+  static constexpr int RES_BYTES = RES ? A_TILE_BYTES : 0;
+  static constexpr size_t SMEM =
+      C64_W_BYTES + C64_HALOS * C64_HALO_BYTES + C64_OUT_SLABS * A_TILE_BYTES + RES_BYTES + 512 + 1024 + 256;
+  static_assert(SMEM <= 227 * 1024, "conv3x3_c64_kernel shared memory");
+};
 
 struct C64Params {
   CUtensorMap x_map;    // NHWC input, box {64, 16, 18, 1}
@@ -388,19 +404,23 @@ struct C64Params {
   CUtensorMap out_map;  // NHWC output, box {64, 8, 16, 1}
   const float* bias;
   int n_img, H, W, tiles_h, tiles_w, relu;
+  CUtensorMap res_map;  // NHWC residual (RES), box {64, 8, 16, 1}
 };
 
+template <bool RES>
 __global__ void __launch_bounds__(CONV_THREADS, 1) conv3x3_c64_kernel(const __grid_constant__ C64Params p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t w_sm = smem_base;
   const uint32_t halo_sm = w_sm + C64_W_BYTES;
   const uint32_t out_stage = halo_sm + C64_HALOS * C64_HALO_BYTES;
-  const uint32_t bias_sm = out_stage + C64_OUT_SLABS * A_TILE_BYTES;
+  const uint32_t res_sm = out_stage + C64_OUT_SLABS * A_TILE_BYTES;  // 1024-aligned, like every slab
+  const uint32_t bias_sm = res_sm + C64Cfg<RES>::RES_BYTES;
   const uint32_t bar_base = bias_sm + 512;
   const uint32_t w_bar = bar_base;
   auto full_bar = [&](int s) { return bar_base + 8u * (1 + s); };
   auto empty_bar = [&](int s) { return bar_base + 8u * (1 + C64_HALOS + s); };
+  const uint32_t res_full = bar_base + 8u * (1 + 2 * C64_HALOS), res_empty = res_full + 8u;
   uint8_t* gsm = smem_raw + (smem_base - smem_u32(smem_raw));
   const int warp = threadIdx.x >> 5;
   const int tiles_per_img = p.tiles_h * p.tiles_w;
@@ -420,10 +440,15 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv3x3_c64_kernel(const __gr
       mbar_init(full_bar(s), 1);
       mbar_init(empty_bar(s), 2);
     }
+    if constexpr (RES) {
+      mbar_init(res_full, 1);
+      mbar_init(res_empty, 1);
+    }
     fence_barrier_init();
     tma_prefetch_desc(&p.x_map);
     tma_prefetch_desc(&p.w_map);
     tma_prefetch_desc(&p.out_map);
+    if constexpr (RES) tma_prefetch_desc(&p.res_map);
   }
   if (threadIdx.x >= 128 && threadIdx.x < 192) reinterpret_cast<float*>(gsm + (bias_sm - smem_base))[threadIdx.x - 128] = p.bias[threadIdx.x - 128];
   __syncthreads();
@@ -445,6 +470,19 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv3x3_c64_kernel(const __gr
         tma_load_4d(halo_sm + stage * C64_HALO_BYTES, &p.x_map, full_bar(stage), 0, w0 - 1, h0 - 1, img);
         if (++stage == C64_HALOS) {
           stage = 0;
+          phase ^= 1u;
+        }
+      }
+    }
+    if constexpr (RES) {
+      if (threadIdx.x == 32) {  // the residual slab: one load per tile, once the previous tile's epilogue has read it
+        uint32_t phase = 0;
+        for (int tile = t_begin; tile < t_end; ++tile) {
+          int w0, h0, img;
+          coords(tile, w0, h0, img);
+          mbar_wait(res_empty, phase ^ 1u);
+          mbar_arrive_expect_tx(res_full, A_TILE_BYTES);
+          tma_load_4d(res_sm, &p.res_map, res_full, 0, w0, h0, img);
           phase ^= 1u;
         }
       }
@@ -485,10 +523,16 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv3x3_c64_kernel(const __gr
       const uint32_t b = g & (C64_OUT_SLABS - 1);
       if (leader) tma_store_wait_read<C64_OUT_SLABS - 1>();
       named_bar_sync(1, 256);
-      store_subtile_f16(acc, oslabs + b * A_TILE_BYTES, row0, bias_s, 0, p.relu, 0);
+      if constexpr (RES) {
+        mbar_wait(res_full, g & 1u);
+        store_subtile_f16(acc, oslabs + b * A_TILE_BYTES, row0, bias_s, 0, p.relu, 0, gsm + (res_sm - smem_base));
+      } else {
+        store_subtile_f16(acc, oslabs + b * A_TILE_BYTES, row0, bias_s, 0, p.relu, 0);
+      }
       fence_proxy_async();
       named_bar_sync(1, 256);
       if (leader) {
+        if constexpr (RES) mbar_arrive(res_empty);  // both warpgroups have read the residual slab
         tma_store_4d(&p.out_map, out_stage + b * A_TILE_BYTES, 0, w0, h0, img);
         tma_store_commit();
       }
@@ -1072,8 +1116,24 @@ struct ChainNext {
   int cout2, relu_from;
 };
 
-static int launch_c64(const void* x, int n, int h, int w, const void* weight, const float* bias, void* out, int relu,
-                      cudaStream_t st) {
+template <bool RES>
+static int launch_c64_kernel(const C64Params& p, cudaStream_t st) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    CTL_CUDA(cudaFuncSetAttribute(conv3x3_c64_kernel<RES>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)C64Cfg<RES>::SMEM));
+    attr_set = true;
+  }
+  const long long tiles = (long long)p.n_img * p.tiles_h * p.tiles_w;
+  const int grid = (int)std::min<long long>(tiles, sm_count());
+  CTL_CUDA(launch_k(conv3x3_c64_kernel<RES>, dim3(grid), dim3(CONV_THREADS), C64Cfg<RES>::SMEM, st, p));
+  CTL_LAUNCH_CHECK();
+  return 0;
+}
+
+// residual (may be null): [n][h][w][64], added before the bias
+static int launch_c64(const void* x, int n, int h, int w, const void* weight, const float* bias, const void* residual,
+                      void* out, int relu, cudaStream_t st) {
   C64Params p = {};
   p.bias = bias;
   p.n_img = n;
@@ -1088,19 +1148,13 @@ static int launch_c64(const void* x, int n, int h, int w, const void* weight, co
   const uint32_t xbox[4] = {64, 16, 18, 1}, obox[4] = {64, 8, 16, 1};
   if ((rc = encode_tensor_map(&p.x_map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 4, x, dims, strd, xbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
   if ((rc = encode_tensor_map(&p.out_map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 4, out, dims, strd, obox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+  if (residual && (rc = encode_tensor_map(&p.res_map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 4, residual, dims, strd, obox,
+                                          CU_TENSOR_MAP_SWIZZLE_128B)))
+    return rc;
   const uint64_t wd[2] = {576, 64}, ws[2] = {2, 576 * 2};
   const uint32_t wbox[2] = {64, 64};
   if ((rc = encode_tensor_map(&p.w_map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 2, weight, wd, ws, wbox, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  static bool attr_set = false;
-  if (!attr_set) {
-    CTL_CUDA(cudaFuncSetAttribute(conv3x3_c64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C64_SMEM));
-    attr_set = true;
-  }
-  const long long tiles = (long long)n * p.tiles_h * p.tiles_w;
-  const int grid = (int)std::min<long long>(tiles, sm_count());
-  CTL_CUDA(launch_k(conv3x3_c64_kernel, dim3(grid), dim3(CONV_THREADS), C64_SMEM, st, p));
-  CTL_LAUNCH_CHECK();
-  return 0;
+  return residual ? launch_c64_kernel<true>(p, st) : launch_c64_kernel<false>(p, st);
 }
 
 // Fills the tile geometry, the output / residual / weight maps and dispatches.  The caller has filled the A maps,
@@ -1188,10 +1242,11 @@ static int encode_source(CUtensorMap* maps, int count, const void* x, int n, int
   return 0;
 }
 
-// Tile geometry, A maps and taps of a 1x1 convolution at the output resolution Ho x Wo = h2 / stride2 x w2 / stride2:
-// x1 [n][Ho][Wo][cin1] alone, or K-concatenated with x2 [n][h2][w2][cin2] read at stride2.
-static int setup_1x1(ConvKernelParams& p, const void* x1, int cin1, const void* x2, int h2, int w2, int cin2, int stride2,
-                     int n) {
+// Tile geometry, A maps and taps of a k1 x k1 (1 or 3, pad k1 / 2, stride 1) convolution at the output resolution
+// Ho x Wo = h2 / stride2 x w2 / stride2: x1 [n][Ho][Wo][cin1] alone, or K-concatenated with the 1x1 of
+// x2 [n][h2][w2][cin2] read at stride2 (weight columns k1 * k1 * cin1 ..).
+static int setup_dual(ConvKernelParams& p, int k1, const void* x1, int cin1, const void* x2, int h2, int w2, int cin2,
+                      int stride2, int n) {
   int rc;
   const int Ho = h2 / stride2, Wo = w2 / stride2;
   pick_tile(Ho, Wo, &p.TH, &p.TW);
@@ -1203,10 +1258,19 @@ static int setup_1x1(ConvKernelParams& p, const void* x1, int cin1, const void* 
   if (x2 && (rc = encode_source(&p.a_map[1], 1, x2, n, h2, w2, cin2, stride2, p.TH, p.TW))) return rc;
   p.a_map[2] = p.a_map[0];
   p.a_map[3] = p.a_map[0];
-  p.n_taps = x2 ? 2 : 1;
-  p.taps[0] = ConvTap{0, 0, 0, 0, cin1 / 64};
-  if (x2) p.taps[1] = ConvTap{1, 0, 0, cin1, cin2 / 64};
-  p.k_blocks = (cin1 + (x2 ? cin2 : 0)) / 64;
+  const int pad = k1 / 2;
+  p.n_taps = 0;
+  for (int r = 0; r < k1; ++r)
+    for (int s = 0; s < k1; ++s) p.taps[p.n_taps++] = ConvTap{0, r - pad, s - pad, (r * k1 + s) * cin1, cin1 / 64};
+  if (x2) {
+    const ConvTap shortcut = {1, 0, 0, k1 * k1 * cin1, cin2 / 64};
+    if (p.n_taps < 9)
+      p.taps[p.n_taps] = shortcut;
+    else
+      p.tap9 = shortcut;
+    ++p.n_taps;
+  }
+  p.k_blocks = (k1 * k1 * cin1 + (x2 ? cin2 : 0)) / 64;
   return 0;
 }
 
@@ -1230,8 +1294,8 @@ int ctl_conv2d_nhwc_f16(const void* x, int32_t n, int32_t h, int32_t w, int32_t 
   if (rc) return rc;
   const int pad = ksize == 3 ? 1 : 0;
   const int Ho = (h + 2 * pad - ksize) / stride + 1, Wo = (w + 2 * pad - ksize) / stride + 1;
-  if (ksize == 3 && stride == 1 && cin == 64 && cout == 64 && !residual && relu_from == 0)
-    return launch_c64(x, n, h, w, weight, bias, out, relu, (cudaStream_t)stream);
+  if (ksize == 3 && stride == 1 && cin == 64 && cout == 64 && relu_from == 0)
+    return launch_c64(x, n, h, w, weight, bias, residual, out, relu, (cudaStream_t)stream);
   ConvKernelParams p = {};
   pick_tile(Ho, Wo, &p.TH, &p.TW);
   p.tiles_h = (Ho + p.TH - 1) / p.TH;
@@ -1267,8 +1331,25 @@ int ctl_conv1x1_dual_nhwc_f16(const void* x1, int32_t cin1, const void* x2, int3
   int rc = ctl_device_check();
   if (rc) return rc;
   ConvKernelParams p = {};
-  if ((rc = setup_1x1(p, x1, cin1, x2, h2, w2, cin2, stride2, n))) return rc;
+  if ((rc = setup_dual(p, 1, x1, cin1, x2, h2, w2, cin2, stride2, n))) return rc;
   return finish_and_launch(p, n, h2 / stride2, w2 / stride2, cout, cin1 + cin2, weight_cat, bias, nullptr, out, relu, 0,
+                           (cudaStream_t)stream);
+}
+
+int ctl_conv3x3_dual_nhwc_f16(const void* x1, int32_t cin1, const void* x2, int32_t h2, int32_t w2, int32_t cin2,
+                              int32_t stride2, int32_t n, const void* weight_cat, const float* bias, void* out,
+                              int32_t cout, int32_t relu, ctl_stream_t stream) {
+  CTL_CHECK_ARG(x1 && x2 && weight_cat && bias && out, "null pointer");
+  CTL_CHECK_ARG(n >= 1 && h2 >= 1 && w2 >= 1, "bad activation shape");
+  CTL_CHECK_ARG(cin1 % 64 == 0 && cin2 % 64 == 0 && cout % 64 == 0 && cin1 >= 64 && cin2 >= 64,
+                "Cin1=%d, Cin2=%d and Cout=%d must be multiples of 64", cin1, cin2, cout);
+  CTL_CHECK_ARG(cout <= 2048, "Cout=%d exceeds 2048 (bias staging)", cout);
+  CTL_CHECK_ARG(stride2 == 1 || (stride2 == 2 && h2 % 2 == 0 && w2 % 2 == 0), "stride2 must be 1, or 2 with even H2, W2");
+  int rc = ctl_device_check();
+  if (rc) return rc;
+  ConvKernelParams p = {};
+  if ((rc = setup_dual(p, 3, x1, cin1, x2, h2, w2, cin2, stride2, n))) return rc;
+  return finish_and_launch(p, n, h2 / stride2, w2 / stride2, cout, 9 * cin1 + cin2, weight_cat, bias, nullptr, out, relu, 0,
                            (cudaStream_t)stream);
 }
 
@@ -1291,7 +1372,7 @@ int ctl_conv1x1_chain_nhwc_f16(const void* x1, int32_t cin1, const void* x2, int
   int rc = ctl_device_check();
   if (rc) return rc;
   ConvKernelParams p = {};
-  if ((rc = setup_1x1(p, x1, cin1, x2, h2, w2, cin2, stride2, n))) return rc;
+  if ((rc = setup_dual(p, 1, x1, cin1, x2, h2, w2, cin2, stride2, n))) return rc;
   const ChainNext next = {weight2, bias2, out2, cout2, relu_from2};
   return finish_and_launch(p, n, h2 / stride2, w2 / stride2, cout, cin1 + (x2 ? cin2 : 0), weight, bias, residual, out, 1,
                            0, (cudaStream_t)stream, &next);

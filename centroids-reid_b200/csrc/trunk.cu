@@ -1,13 +1,14 @@
 // Whole-trunk entry points of the C ABI (SURVEY 8b: ctl_weights_pack + ctl_embed_forward): the layer graph of the eval
-// embedding path -- ResNet.forward / ResNet_IBN.forward (modelling/backbones/resnet.py:122-133, resnet_ibn_a.py:126-141),
+// embedding path -- ResNet.forward / ResNet_IBN.forward (modelling/backbones/resnet.py:122-133, resnet_ibn_a.py:126-141)
+// over Bottleneck (ResNet50/101/152, -IBN-a) or BasicBlock (ResNet18/34) blocks,
 // Baseline.forward's global average pool (modelling/baseline.py:91-96) and the eval BatchNorm1d of
 // ModelBase.validation_step (modelling/bases.py:169-177) -- behind an opaque handle.  This is the eval trunk's only
 // driver: modelling/backbones/engine.py::TrunkEngine is its ctypes form, and a host that is not Python binds the same calls.
 //
 // The handle owns the PACKED operands: [Cout][kh][kw][Cin] fp16 weights with the eval BatchNorm folded in and fp32
 // biases, produced on the device from the reference's fp32 state_dict tensors (fold_pack_kernel: fp32 divide / sqrt /
-// multiply / subtract, each correctly rounded, then one rounding to fp16), the K-concatenated [W3 | Wd] matrices of every
-// first block, the two stem layouts, and one zero-bordered staging buffer of the fused stem per input shape.
+// multiply / subtract, each correctly rounded, then one rounding to fp16), the K-concatenated [W3 | Wd] (bottleneck) or
+// [W2 | Wd] (BasicBlock) matrices of every block with a downsample, the two stem layouts, and one zero-bordered staging buffer of the fused stem per input shape.
 // Activations live in a caller-provided workspace.
 #include <math.h>
 #include <string.h>
@@ -88,7 +89,7 @@ struct PackedConv {
 };
 struct TrunkBlock {
   std::string prefix;  // "layer<stage>.<block>" of the state_dict names
-  PackedConv c1, c2, c3, down;
+  PackedConv c1, c2, c3, down;  // a BasicBlock has no c3: c1 and c2 are its two 3x3 convolutions
   bool has_down = false, has_in = false;
   int in_half = 0;
   float *in_gamma = nullptr, *in_beta = nullptr;
@@ -99,6 +100,7 @@ struct TrunkBlock {
 }  // namespace ctl
 
 struct ctl_trunk {
+  int block = CTL_BLOCK_BOTTLENECK, feature_dim = 2048;
   int ibn = 0, last_stride = 1;
   bool packed = false, has_head = false;
   std::vector<ctl::TrunkBlock> blocks;
@@ -167,6 +169,42 @@ static int pack_conv(ctl_trunk* h, const TensorMap& m, const std::string& conv, 
   return 0;
 }
 
+
+// The downsample of `blk` and the single-GEMM form of its block's last convolution `last` (conv3 of a bottleneck,
+// conv2 of a BasicBlock) + shortcut: [W_last | Wd] with bias_last + bias_d (ctl_conv1x1_dual_nhwc_f16 /
+// ctl_conv3x3_dual_nhwc_f16).  `last` must be packed already.
+static int pack_down_dual(ctl_trunk* h, const TensorMap& m, TrunkBlock& blk, const PackedConv& last, cudaStream_t st) {
+  int rc = 0;
+  const std::string& p = blk.prefix;
+  const int sd = blk.down.stride;
+  if ((rc = pack_conv(h, m, p + ".downsample.0", p + ".downsample.1", blk.down.cout, blk.down.cin, 1, 0, &blk.down, st))) return rc;
+  blk.down.stride = sd;
+  blk.down.relu = 0;
+  const int km = last.k * last.k * last.cin;  // row length of the packed [cout][k][k][cin] weights
+  const int kt = km + blk.down.cin;
+  if (!blk.dual_w) {
+    blk.dual_w = dev_alloc<__half>(h, (size_t)last.cout * kt);
+    blk.dual_b = dev_alloc<float>(h, last.cout);
+  }
+  if (!blk.dual_w || !blk.dual_b) {
+    set_error("ctl_weights_pack: out of device memory");
+    return (int)cudaErrorMemoryAllocation;
+  }
+  CTL_CUDA(cudaMemcpy2DAsync(blk.dual_w, (size_t)kt * 2, last.w, (size_t)km * 2, (size_t)km * 2, last.cout,
+                             cudaMemcpyDeviceToDevice, st));
+  CTL_CUDA(cudaMemcpy2DAsync(blk.dual_w + km, (size_t)kt * 2, blk.down.w, (size_t)blk.down.cin * 2,
+                             (size_t)blk.down.cin * 2, last.cout, cudaMemcpyDeviceToDevice, st));
+  // bias_last + bias_d, one fp32 add per channel
+  CTL_CUDA(cudaMemcpyAsync(blk.dual_b, last.b, last.cout * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  const std::string d = p + ".downsample.1";
+  fold_pack_kernel<<<last.cout, 32, 0, st>>>(need(m, p + ".downsample.0.weight", (long long)blk.down.cout * blk.down.cin, &rc), blk.down.cout, 0, 1,
+                                             need(m, d + ".weight", blk.down.cout, &rc), need(m, d + ".bias", blk.down.cout, &rc),
+                                             need(m, d + ".running_mean", blk.down.cout, &rc),
+                                             need(m, d + ".running_var", blk.down.cout, &rc), 0, blk.down.w, 0, 0, blk.dual_b, 1);
+  CTL_LAUNCH_CHECK();
+  return rc;
+}
+
 }  // namespace ctl
 
 using namespace ctl;
@@ -174,15 +212,49 @@ using namespace ctl;
 extern "C" {
 
 int ctl_trunk_create(ctl_trunk** out, int32_t ibn, int32_t last_stride, const int32_t stage_blocks[4]) {
+  return ctl_trunk_create_ex(out, CTL_BLOCK_BOTTLENECK, ibn, last_stride, stage_blocks);
+}
+
+int ctl_trunk_create_ex(ctl_trunk** out, int32_t block, int32_t ibn, int32_t last_stride, const int32_t stage_blocks[4]) {
   CTL_CHECK_ARG(out != nullptr && stage_blocks != nullptr, "null pointer");
+  CTL_CHECK_ARG(block == CTL_BLOCK_BOTTLENECK || block == CTL_BLOCK_BASIC,
+                "block = %d: expected CTL_BLOCK_BOTTLENECK (0) or CTL_BLOCK_BASIC (1)", block);
+  CTL_CHECK_ARG(block == CTL_BLOCK_BOTTLENECK || !ibn, "IBN-a is defined for bottleneck blocks only (resnet_ibn_a.py)");
   CTL_CHECK_ARG(last_stride == 1 || last_stride == 2, "last_stride must be 1 or 2 (config/defaults.py:24)");
   for (int li = 0; li < 4; ++li)
     CTL_CHECK_ARG(stage_blocks[li] >= 1, "stage_blocks[%d] = %d: every stage needs at least one block", li, stage_blocks[li]);
   ctl_trunk* h = new ctl_trunk();
+  h->block = block;
   h->ibn = ibn ? 1 : 0;
   h->last_stride = last_stride;
   const int planes[4] = {64, 128, 256, 512};
   int inplanes = 64;
+  if (block == CTL_BLOCK_BASIC) {
+    h->feature_dim = 512;
+    // resnet.py:19-48,105-112: conv1 3x3 / stride, conv2 3x3; a downsample where stride != 1 or inplanes != planes,
+    // i.e. on the first block of layers 2-4
+    for (int li = 0; li < 4; ++li)
+      for (int bi = 0; bi < stage_blocks[li]; ++bi) {
+        TrunkBlock blk;
+        blk.prefix = "layer" + std::to_string(li + 1) + "." + std::to_string(bi);
+        const int stride = bi == 0 ? (li == 0 ? 1 : (li == 3 ? last_stride : 2)) : 1;
+        blk.c1.cin = inplanes;
+        blk.c1.cout = blk.c2.cin = blk.c2.cout = planes[li];
+        blk.c1.k = blk.c2.k = 3;
+        blk.c1.stride = stride;
+        blk.has_down = stride != 1 || inplanes != planes[li];
+        if (blk.has_down) {
+          blk.down.cin = inplanes;
+          blk.down.cout = planes[li];
+          blk.down.stride = stride;
+          blk.down.relu = 0;
+        }
+        inplanes = planes[li];
+        h->blocks.push_back(blk);
+      }
+    *out = h;
+    return 0;
+  }
   for (int li = 0; li < 4; ++li)
     for (int bi = 0; bi < stage_blocks[li]; ++bi) {
       TrunkBlock blk;
@@ -210,6 +282,8 @@ int ctl_trunk_create(ctl_trunk** out, int32_t ibn, int32_t last_stride, const in
   *out = h;
   return 0;
 }
+
+int32_t ctl_trunk_feature_dim(const ctl_trunk* h) { return h ? h->feature_dim : 0; }
 
 void ctl_trunk_destroy(ctl_trunk* h) {
   if (!h) return;
@@ -248,6 +322,12 @@ int ctl_weights_pack(ctl_trunk* h, const ctl_named_tensor* tensors, int32_t n_te
   // ---- bottlenecks ----
   for (TrunkBlock& blk : h->blocks) {
     const std::string& p = blk.prefix;
+    if (h->block == CTL_BLOCK_BASIC) {
+      if ((rc = pack_conv(h, m, p + ".conv1", p + ".bn1", blk.c1.cout, blk.c1.cin, 3, 0, &blk.c1, st))) return rc;
+      if ((rc = pack_conv(h, m, p + ".conv2", p + ".bn2", blk.c2.cout, blk.c2.cin, 3, 0, &blk.c2, st))) return rc;
+      if (blk.has_down && (rc = pack_down_dual(h, m, blk, blk.c2, st))) return rc;
+      continue;
+    }
     if (blk.has_in) {
       // IBN: channels [0, half) keep the raw convolution (InstanceNorm + ReLU follow as their own kernel), the
       // BatchNorm half is folded; ReLU in the conv epilogue only from channel `half` on
@@ -268,48 +348,20 @@ int ctl_weights_pack(ctl_trunk* h, const ctl_named_tensor* tensors, int32_t n_te
     if ((rc = pack_conv(h, m, p + ".conv2", p + ".bn2", blk.c2.cout, blk.c2.cin, 3, 0, &blk.c2, st))) return rc;
     blk.c2.stride = s2;
     if ((rc = pack_conv(h, m, p + ".conv3", p + ".bn3", blk.c3.cout, blk.c3.cin, 1, 0, &blk.c3, st))) return rc;
-    if (blk.has_down) {
-      const int sd = blk.down.stride;
-      if ((rc = pack_conv(h, m, p + ".downsample.0", p + ".downsample.1", blk.down.cout, blk.down.cin, 1, 0, &blk.down, st))) return rc;
-      blk.down.stride = sd;
-      blk.down.relu = 0;
-      // [W3 | Wd] and bias3 + bias_d for the single-GEMM form of conv3 + shortcut (ctl_conv1x1_dual_nhwc_f16)
-      const int kt = blk.c3.cin + blk.down.cin;
-      if (!blk.dual_w) {
-        blk.dual_w = dev_alloc<__half>(h, (size_t)blk.c3.cout * kt);
-        blk.dual_b = dev_alloc<float>(h, blk.c3.cout);
-      }
-      if (!blk.dual_w || !blk.dual_b) {
-        set_error("ctl_weights_pack: out of device memory");
-        return (int)cudaErrorMemoryAllocation;
-      }
-      CTL_CUDA(cudaMemcpy2DAsync(blk.dual_w, (size_t)kt * 2, blk.c3.w, (size_t)blk.c3.cin * 2, (size_t)blk.c3.cin * 2, blk.c3.cout,
-                                 cudaMemcpyDeviceToDevice, st));
-      CTL_CUDA(cudaMemcpy2DAsync(blk.dual_w + blk.c3.cin, (size_t)kt * 2, blk.down.w, (size_t)blk.down.cin * 2,
-                                 (size_t)blk.down.cin * 2, blk.c3.cout, cudaMemcpyDeviceToDevice, st));
-      // bias3 + bias_d, one fp32 add per channel
-      CTL_CUDA(cudaMemcpyAsync(blk.dual_b, blk.c3.b, blk.c3.cout * sizeof(float), cudaMemcpyDeviceToDevice, st));
-      const std::string d = p + ".downsample.1";
-      int rc2 = 0;
-      fold_pack_kernel<<<blk.c3.cout, 32, 0, st>>>(need(m, p + ".downsample.0.weight", (long long)blk.down.cout * blk.down.cin, &rc2), blk.down.cout, 0, 1,
-                                                   need(m, d + ".weight", blk.down.cout, &rc2), need(m, d + ".bias", blk.down.cout, &rc2),
-                                                   need(m, d + ".running_mean", blk.down.cout, &rc2),
-                                                   need(m, d + ".running_var", blk.down.cout, &rc2), 0, blk.down.w, 0, 0, blk.dual_b, 1);
-      CTL_LAUNCH_CHECK();
-      if (rc2) return rc2;
-    }
+    if (blk.has_down && (rc = pack_down_dual(h, m, blk, blk.c3, st))) return rc;
   }
   // ---- optional BatchNorm1d head (ModelBase.bn, modelling/bases.py:83) ----
   h->has_head = m.count("bn_head.weight") != 0;
   if (h->has_head) {
-    const float *g = need(m, "bn_head.weight", 2048, &rc), *b = need(m, "bn_head.bias", 2048, &rc),
-                *mu = need(m, "bn_head.running_mean", 2048, &rc), *va = need(m, "bn_head.running_var", 2048, &rc);
+    const int fd = h->feature_dim;
+    const float *g = need(m, "bn_head.weight", fd, &rc), *b = need(m, "bn_head.bias", fd, &rc),
+                *mu = need(m, "bn_head.running_mean", fd, &rc), *va = need(m, "bn_head.running_var", fd, &rc);
     if (rc) return rc;
     if (!h->head_scale) {
-      h->head_scale = dev_alloc<float>(h, 2048);
-      h->head_shift = dev_alloc<float>(h, 2048);
+      h->head_scale = dev_alloc<float>(h, fd);
+      h->head_shift = dev_alloc<float>(h, fd);
     }
-    head_pack_kernel<<<8, 256, 0, st>>>(g, b, mu, va, 2048, h->head_scale, h->head_shift);
+    head_pack_kernel<<<(fd + 255) / 256, 256, 0, st>>>(g, b, mu, va, fd, h->head_scale, h->head_shift);
     CTL_LAUNCH_CHECK();
   }
   h->packed = true;
@@ -325,10 +377,14 @@ static int stem_side(int s) { return (s + 6 - 7) / 2 + 1; }  // conv1 7x7 / 2, p
 static int pool_side(int s) { return (s + 2 - 3) / 2 + 1; }  // maxpool 3x3 / 2, pad 1
 static bool fused_stem_fits(int hgt, int wid) { return hgt % 4 == 0 && wid % 2 == 0 && wid <= 128; }
 
-// One of the five activation slots of the bottleneck walk on a [n, hp, wp, 64] stem output: layer1's output
-// [n, hp, wp, 256] is the largest tensor the blocks write (each later stage halves both sides -- stride-2 convolutions
-// take even sides only -- before it doubles the channels).
-static size_t block_slot_bytes(int n, int hp, int wp) { return round256((size_t)n * hp * wp * 256 * 2); }
+// One of the activation slots of the block walk on a [n, hp, wp, 64] stem output: layer1's output is the largest tensor
+// the blocks write (each later stage halves both sides -- stride-2 convolutions take even sides only -- before it
+// doubles the channels), [n, hp, wp, 256] for bottlenecks and [n, hp, wp, 64] for BasicBlocks.
+static size_t block_slot_bytes(const ctl_trunk* h, int n, int hp, int wp) {
+  return round256((size_t)n * hp * wp * (h->block == CTL_BLOCK_BASIC ? 64 : 256) * 2);
+}
+// the bottleneck walk rotates five slots, the BasicBlock walk three (block input, conv1 output, block output)
+static int block_slots(const ctl_trunk* h) { return h->block == CTL_BLOCK_BASIC ? 3 : 5; }
 // the tensor-core stem's conv output [n, h/2, w/2, 64], which is larger than a slot when h/2 or w/2 is odd
 static size_t stem_tmp_bytes(int n, int hgt, int wid) { return round256((size_t)n * stem_side(hgt) * stem_side(wid) * 64 * 2); }
 
@@ -459,10 +515,51 @@ static int run_blocks(ctl_trunk* h, const void* x, int x_slot, int n, int* hh, i
   return 0;
 }
 
+// The BasicBlock walk (resnet.py:19-48) on x [n, hh, ww, 64]: conv1 (3x3 / stride, ReLU), then conv2 (3x3) + shortcut
+// + ReLU in one launch -- the identity as the epilogue's residual, a downsample as the K-concatenated 1x1 of
+// ctl_conv3x3_dual_nhwc_f16 (its stride-2 parity view needs even sides, which the stride-2 conv1 already requires).
+// Three workspace slots of `slot` bytes: the block input (x_slot; < 0: a caller tensor that is never written), conv1's
+// output and the block output.  The last block writes `out` when it is given.  *y = the trunk output [n, *hh, *ww, 512].
+static int run_basic_blocks(ctl_trunk* h, const void* x, int x_slot, int n, int* hh, int* ww, char* ws, size_t slot,
+                            void* out, const void** y, cudaStream_t st) {
+  int rc;
+  const void* a = x;
+  int cur = x_slot;
+  for (size_t bi = 0; bi < h->blocks.size(); ++bi) {
+    const TrunkBlock& blk = h->blocks[bi];
+    const int o1_slot = (cur + 1) % 3, dst_slot = (cur + 2) % 3;
+    void* o1 = ws + o1_slot * slot;
+    void* dst = out && bi + 1 == h->blocks.size() ? out : ws + dst_slot * slot;
+    const int h1 = *hh, w1 = *ww, s = blk.c1.stride;
+    const int h2 = (h1 + 2 - 3) / s + 1, w2 = (w1 + 2 - 3) / s + 1;
+    if ((rc = run_conv(h, blk.c1, a, n, h1, w1, nullptr, o1, st))) return rc;
+    if (blk.has_down) {
+      ++h->launches;
+      rc = ctl_conv3x3_dual_nhwc_f16(o1, blk.c2.cin, a, h1, w1, blk.down.cin, s, n, blk.dual_w, blk.dual_b, dst, blk.c2.cout,
+                                     1, st);
+    } else {
+      rc = run_conv(h, blk.c2, o1, n, h2, w2, a, dst, st);
+    }
+    if (rc) return rc;
+    a = dst;
+    cur = dst_slot;
+    *hh = h2;
+    *ww = w2;
+  }
+  *y = a;
+  return 0;
+}
+
+static int run_walk(ctl_trunk* h, const void* x, int x_slot, int n, int* hh, int* ww, char* ws, size_t slot, void* out,
+                    const void** y, cudaStream_t st) {
+  return h->block == CTL_BLOCK_BASIC ? run_basic_blocks(h, x, x_slot, n, hh, ww, ws, slot, out, y, st)
+                                     : run_blocks(h, x, x_slot, n, hh, ww, ws, slot, out, y, st);
+}
+
 // global average pool (+ the folded BatchNorm1d head when out_emb is given)
 static int run_head(ctl_trunk* h, const void* y, int n, int hw, float* out_feat, float* out_emb, cudaStream_t st) {
   ++h->launches;
-  return ctl_gap_bn_nhwc_f16(y, n, hw, 2048, out_emb ? h->head_scale : nullptr, out_emb ? h->head_shift : nullptr, out_feat,
+  return ctl_gap_bn_nhwc_f16(y, n, hw, h->feature_dim, out_emb ? h->head_scale : nullptr, out_emb ? h->head_shift : nullptr, out_feat,
                              out_emb, st);
 }
 
@@ -472,7 +569,10 @@ extern "C" {
 
 size_t ctl_embed_workspace_bytes(const ctl_trunk* h, int32_t n, int32_t hgt, int32_t wid) {
   if (!h || n < 1 || hgt < 8 || wid < 8) return 0;
-  return 5 * std::max(block_slot_bytes(n, pool_side(stem_side(hgt)), pool_side(stem_side(wid))), stem_tmp_bytes(n, hgt, wid));
+  const size_t slot = block_slot_bytes(h, n, pool_side(stem_side(hgt)), pool_side(stem_side(wid)));
+  if (h->block == CTL_BLOCK_BASIC)  // the stem's temporary starts at slot 1 (ctl_embed_forward) and may span several
+    return std::max(3 * slot, slot + stem_tmp_bytes(n, hgt, wid));
+  return 5 * std::max(slot, stem_tmp_bytes(n, hgt, wid));
 }
 
 int ctl_embed_stem(ctl_trunk* h, const void* x, int32_t n, int32_t hgt, int32_t wid, const float* mean3_host,
@@ -491,12 +591,12 @@ int ctl_embed_blocks(ctl_trunk* h, const void* x_nhwc, int32_t n, int32_t hgt, i
                      size_t workspace_bytes, ctl_stream_t stream) {
   CTL_CHECK_ARG(h && x_nhwc && out_nhwc && workspace, "null pointer");
   CTL_CHECK_ARG(n >= 1 && hgt >= 2 && wid >= 2, "bad activation shape");
-  const size_t slot = block_slot_bytes(n, hgt, wid);
-  int rc = check_workspace(5 * slot, workspace_bytes);
+  const size_t slot = block_slot_bytes(h, n, hgt, wid);
+  int rc = check_workspace(block_slots(h) * slot, workspace_bytes);
   if (rc || (rc = begin_call(h))) return rc;
   int hh = hgt, ww = wid;
   const void* y = nullptr;
-  return run_blocks(h, x_nhwc, -1, n, &hh, &ww, static_cast<char*>(workspace), slot, out_nhwc, &y, (cudaStream_t)stream);
+  return run_walk(h, x_nhwc, -1, n, &hh, &ww, static_cast<char*>(workspace), slot, out_nhwc, &y, (cudaStream_t)stream);
 }
 
 int ctl_embed_head(ctl_trunk* h, const void* x_nhwc, int32_t n, int32_t hw, float* out_feat, float* out_emb,
@@ -518,12 +618,12 @@ int ctl_embed_forward(ctl_trunk* h, const float* x_nchw, int32_t n, int32_t hgt,
   if (rc || (rc = begin_call(h))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   int hh = pool_side(stem_side(hgt)), ww = pool_side(stem_side(wid));
-  const size_t slot = block_slot_bytes(n, hh, ww);
+  const size_t slot = block_slot_bytes(h, n, hh, ww);
   char* ws = static_cast<char*>(workspace);
   // the stem writes slot 0; the tensor-core stem's temporary (at most one activation) starts at slot 1
   if ((rc = run_stem(h, x_nchw, nullptr, nullptr, n, hgt, wid, ws, ws + slot, st))) return rc;
   const void* y = nullptr;
-  if ((rc = run_blocks(h, ws, 0, n, &hh, &ww, ws, slot, nullptr, &y, st))) return rc;
+  if ((rc = run_walk(h, ws, 0, n, &hh, &ww, ws, slot, nullptr, &y, st))) return rc;
   return run_head(h, y, n, hh * ww, out_feat, out_emb, st);
 }
 

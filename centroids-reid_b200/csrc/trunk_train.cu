@@ -5,9 +5,9 @@
 //   ctl_trainer_bind -> ctl_train_forward -> (the loss on global_feat, ctl_ctl_loss_step) -> ctl_train_backward ->
 //   ctl_adam_multi_step
 // This is the only driver of the training trunk: modelling/backbones/engine_train.py::TrunkTrainer is its ctypes form.
-// The forward walks the stem, then every bottleneck (conv1, conv2, downsample, conv3) through the conv / BatchNorm
-// entry points; the backward walks the blocks in reverse: BN backward, weight gradient, data gradient through the
-// transposed convolution (stride-2 layers via zero-insertion upsampling), the shortcut's gradient added through
+// The forward walks the stem, then every bottleneck (conv1, conv2, downsample, conv3) or BasicBlock (conv1, downsample,
+// conv2) through the conv / BatchNorm entry points; the backward walks the blocks in reverse: BN backward, weight
+// gradient, data gradient through the transposed convolution (stride-2 layers via zero-insertion upsampling), the shortcut's gradient added through
 // conv1's residual input, and the stem's weight gradient as an im2col GEMM.
 //
 // Memory: everything lives in the caller's workspace of ctl_train_workspace_bytes(...) bytes, carved by a bump allocator
@@ -88,13 +88,14 @@ struct ConvSpec {
 };
 
 struct TrainBlock {
-  ConvSpec c1, c2, c3, down;
+  ConvSpec c1, c2, c3, down;  // a BasicBlock has no c3: c1 and c2 are its two 3x3 convolutions
   bool has_down = false;
 };
 
 }  // namespace ctl
 
 struct ctl_trainer {
+  int block = CTL_BLOCK_BOTTLENECK, feature_dim = 2048;
   int ibn = 0, last_stride = 1;
   float momentum = 0.1f;
   bool bound = false, forwarded = false, saved = false;  // saved: the last forward completed (ctl_train_saved)
@@ -301,23 +302,30 @@ static int forward_walk(ctl_trainer* t, Bump& ws, Plan& plan, void* bn_ws, size_
   }
   const void* a = t->pool0;
   int hh = hp, ww = wp;
+  const bool basic = t->block == CTL_BLOCK_BASIC;
   for (TrainBlock& b : t->blocks) {
+    // bottleneck: conv1, conv2, [downsample], conv3 + shortcut; BasicBlock: conv1, [downsample], conv2 + shortcut
+    ConvSpec& last = basic ? b.c2 : b.c3;
     if ((rc = conv_bn_forward(t, b.c1, ws, bn_ws, bn_ws_bytes, &plan.bn_need, a, n, hh, ww, nullptr, st))) return rc;
-    if ((rc = conv_bn_forward(t, b.c2, ws, bn_ws, bn_ws_bytes, &plan.bn_need, b.c1.z, n, b.c1.ho, b.c1.wo, nullptr, st))) return rc;
+    const ConvSpec* prev = &b.c1;
+    if (!basic) {
+      if ((rc = conv_bn_forward(t, b.c2, ws, bn_ws, bn_ws_bytes, &plan.bn_need, b.c1.z, n, b.c1.ho, b.c1.wo, nullptr, st))) return rc;
+      prev = &b.c2;
+    }
     const void* res = a;
     if (b.has_down) {
       if ((rc = conv_bn_forward(t, b.down, ws, bn_ws, bn_ws_bytes, &plan.bn_need, a, n, hh, ww, nullptr, st))) return rc;
       res = b.down.z;
     }
-    if ((rc = conv_bn_forward(t, b.c3, ws, bn_ws, bn_ws_bytes, &plan.bn_need, b.c2.z, n, b.c2.ho, b.c2.wo, res, st))) return rc;
-    a = b.c3.z;
-    hh = b.c3.ho;
-    ww = b.c3.wo;
+    if ((rc = conv_bn_forward(t, last, ws, bn_ws, bn_ws_bytes, &plan.bn_need, prev->z, n, prev->ho, prev->wo, res, st))) return rc;
+    a = last.z;
+    hh = last.ho;
+    ww = last.wo;
   }
   t->last = const_cast<void*>(a);
   t->last_h = hh;
   t->last_w = ww;
-  if (!ws.dry) rc = ctl_gap_bn_nhwc_f16(a, n, hh * ww, 2048, nullptr, nullptr, out_feat, nullptr, st);
+  if (!ws.dry) rc = ctl_gap_bn_nhwc_f16(a, n, hh * ww, t->feature_dim, nullptr, nullptr, out_feat, nullptr, st);
   return rc;
 }
 
@@ -329,21 +337,26 @@ static int backward_walk(ctl_trainer* t, Bump& ws, Plan& plan, void* bn_ws, size
   // the block-boundary gradient ping-pongs between two buffers of the largest block input
   size_t edge = 0;
   for (const TrainBlock& b : t->blocks) edge = std::max(edge, (size_t)n * b.c1.h * b.c1.w_in * b.c1.cin * 2);
-  edge = std::max(edge, (size_t)n * t->last_h * t->last_w * 2048 * 2);
+  edge = std::max(edge, (size_t)n * t->last_h * t->last_w * t->feature_dim * 2);
   void* pp[2] = {ws.take(edge), ws.take(edge)};
   int cur = 0;
   if (!ws.dry)
-    if ((rc = ctl_gap_backward_nhwc_f16(dfeat, n, t->last_h * t->last_w, 2048, (float)((double)grad_scale / (double)(t->last_h * t->last_w)), pp[0], st)))
+    if ((rc = ctl_gap_backward_nhwc_f16(dfeat, n, t->last_h * t->last_w, t->feature_dim, (float)((double)grad_scale / (double)(t->last_h * t->last_w)), pp[0], st)))
       return rc;
   const size_t mark = ws.off;
+  const bool basic = t->block == CTL_BLOCK_BASIC;
   for (size_t bi = t->blocks.size(); bi-- > 0;) {
     TrainBlock& b = t->blocks[bi];
     ws.off = mark;
     void* dz = pp[cur];
     void *dy3, *d2, *dy2, *d1, *dy1, *dyd, *shortcut = dz, *unused;
-    if ((rc = bn_backward(t, b.c3, ws, bn_ws, bn_ws_bytes, dz, true, inv_scale, &dy3, st))) return rc;  // dz becomes g3
-    if ((rc = conv_backward(t, b.c3, ws, wg_ws, wg_ws_bytes, &plan.wg_need, dy3, inv_scale, true, nullptr, nullptr, &d2, st))) return rc;
-    if ((rc = bn_backward(t, b.c2, ws, bn_ws, bn_ws_bytes, d2, true, inv_scale, &dy2, st))) return rc;
+    if (basic) {  // conv2 carries the shortcut: dz becomes its ReLU-masked gradient, which the shortcut also receives
+      if ((rc = bn_backward(t, b.c2, ws, bn_ws, bn_ws_bytes, dz, true, inv_scale, &dy2, st))) return rc;
+    } else {
+      if ((rc = bn_backward(t, b.c3, ws, bn_ws, bn_ws_bytes, dz, true, inv_scale, &dy3, st))) return rc;  // dz becomes g3
+      if ((rc = conv_backward(t, b.c3, ws, wg_ws, wg_ws_bytes, &plan.wg_need, dy3, inv_scale, true, nullptr, nullptr, &d2, st))) return rc;
+      if ((rc = bn_backward(t, b.c2, ws, bn_ws, bn_ws_bytes, d2, true, inv_scale, &dy2, st))) return rc;
+    }
     if ((rc = conv_backward(t, b.c2, ws, wg_ws, wg_ws_bytes, &plan.wg_need, dy2, inv_scale, true, nullptr, nullptr, &d1, st))) return rc;
     if ((rc = bn_backward(t, b.c1, ws, bn_ws, bn_ws_bytes, d1, true, inv_scale, &dy1, st))) return rc;
     if (b.has_down) {
@@ -414,17 +427,59 @@ using namespace ctl;
 extern "C" {
 
 int ctl_trainer_create(ctl_trainer** out, int32_t ibn, int32_t last_stride, float momentum, const int32_t stage_blocks[4]) {
+  return ctl_trainer_create_ex(out, CTL_BLOCK_BOTTLENECK, ibn, last_stride, momentum, stage_blocks);
+}
+
+int ctl_trainer_create_ex(ctl_trainer** out, int32_t block, int32_t ibn, int32_t last_stride, float momentum,
+                          const int32_t stage_blocks[4]) {
   CTL_CHECK_ARG(out != nullptr && stage_blocks != nullptr, "null pointer");
+  CTL_CHECK_ARG(block == CTL_BLOCK_BOTTLENECK || block == CTL_BLOCK_BASIC,
+                "block = %d: expected CTL_BLOCK_BOTTLENECK (0) or CTL_BLOCK_BASIC (1)", block);
+  CTL_CHECK_ARG(block == CTL_BLOCK_BOTTLENECK || !ibn, "IBN-a is defined for bottleneck blocks only (resnet_ibn_a.py)");
   CTL_CHECK_ARG(last_stride == 1 || last_stride == 2, "last_stride must be 1 or 2 (config/defaults.py:24)");
   CTL_CHECK_ARG(momentum > 0.f && momentum <= 1.f, "momentum must be in (0, 1]");
   for (int li = 0; li < 4; ++li)
     CTL_CHECK_ARG(stage_blocks[li] >= 1, "stage_blocks[%d] = %d: every stage needs at least one block", li, stage_blocks[li]);
   ctl_trainer* t = new ctl_trainer();
+  t->block = block;
   t->ibn = ibn ? 1 : 0;
   t->last_stride = last_stride;
   t->momentum = momentum;
   const int planes[4] = {64, 128, 256, 512};
   int inplanes = 64;
+  if (block == CTL_BLOCK_BASIC) {
+    t->feature_dim = 512;
+    // resnet.py:19-48,105-112: conv1 3x3 / stride, conv2 3x3; a downsample on the first block of layers 2-4
+    for (int li = 0; li < 4; ++li)
+      for (int bi = 0; bi < stage_blocks[li]; ++bi) {
+        TrainBlock b;
+        const std::string p = "layer" + std::to_string(li + 1) + "." + std::to_string(bi);
+        const int stride = bi == 0 ? (li == 0 ? 1 : (li == 3 ? last_stride : 2)) : 1;
+        b.c1.conv = p + ".conv1";
+        b.c1.bn = p + ".bn1";
+        b.c1.cin = inplanes;
+        b.c1.cout = planes[li];
+        b.c1.k = 3;
+        b.c1.stride = stride;
+        b.c2.conv = p + ".conv2";
+        b.c2.bn = p + ".bn2";
+        b.c2.cin = b.c2.cout = planes[li];
+        b.c2.k = 3;
+        b.has_down = stride != 1 || inplanes != planes[li];
+        if (b.has_down) {
+          b.down.conv = p + ".downsample.0";
+          b.down.bn = p + ".downsample.1";
+          b.down.cin = inplanes;
+          b.down.cout = planes[li];
+          b.down.stride = stride;
+          b.down.relu = 0;
+        }
+        inplanes = planes[li];
+        t->blocks.push_back(b);
+      }
+    *out = t;
+    return 0;
+  }
   for (int li = 0; li < 4; ++li)
     for (int bi = 0; bi < stage_blocks[li]; ++bi) {
       TrainBlock b;
@@ -460,6 +515,8 @@ int ctl_trainer_create(ctl_trainer** out, int32_t ibn, int32_t last_stride, floa
   return 0;
 }
 
+int32_t ctl_trainer_feature_dim(const ctl_trainer* t) { return t ? t->feature_dim : 0; }
+
 void ctl_trainer_destroy(ctl_trainer* t) {
   if (!t) return;
   for (void* p : t->owned) cudaFree(p);
@@ -493,8 +550,9 @@ int ctl_trainer_bind(ctl_trainer* t, const ctl_named_tensor* params, int32_t n_p
   CTL_CHECK_ARG((t->rm0 == nullptr) == (t->rv0 == nullptr), "bn1 needs running_mean and running_var together (or neither)");
   size_t total = 0;
   int n_convs = 0;
+  const bool basic = t->block == CTL_BLOCK_BASIC;
   for (TrainBlock& b : t->blocks) {
-    ConvSpec* cs[4] = {&b.c1, &b.c2, &b.c3, b.has_down ? &b.down : nullptr};
+    ConvSpec* cs[4] = {&b.c1, &b.c2, basic ? nullptr : &b.c3, b.has_down ? &b.down : nullptr};
     for (ConvSpec* c : cs) {
       if (!c) continue;
       if ((rc = bind_conv(*c, p, g))) return rc;
@@ -519,8 +577,8 @@ int ctl_trainer_bind(ctl_trainer* t, const ctl_named_tensor* params, int32_t n_p
   size_t off = 0;
   long long chunks = 0;
   for (TrainBlock& b : t->blocks) {
-    // table order: state_dict order (conv1, conv2, conv3, downsample.0)
-    ConvSpec* cs[4] = {&b.c1, &b.c2, &b.c3, b.has_down ? &b.down : nullptr};
+    // table order: state_dict order (conv1, conv2, [conv3], downsample.0)
+    ConvSpec* cs[4] = {&b.c1, &b.c2, basic ? nullptr : &b.c3, b.has_down ? &b.down : nullptr};
     for (ConvSpec* c : cs) {
       if (!c) continue;
       const size_t numel = (size_t)c->cout * c->cin * c->k * c->k;
@@ -597,8 +655,10 @@ int ctl_train_saved(const ctl_trainer* t, int32_t index, const void** y, const v
     return 0;
   }
   int32_t i = 1;
+  const bool basic = t->block == CTL_BLOCK_BASIC;
   for (const TrainBlock& b : t->blocks) {
-    const ConvSpec* cs[4] = {&b.c1, &b.c2, b.has_down ? &b.down : nullptr, &b.c3};  // forward order
+    // forward order
+    const ConvSpec* cs[4] = {&b.c1, basic ? nullptr : &b.c2, b.has_down ? &b.down : nullptr, basic ? &b.c2 : &b.c3};
     for (const ConvSpec* c : cs) {
       if (!c || i++ != index) continue;
       *y = c->y;

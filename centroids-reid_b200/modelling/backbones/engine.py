@@ -1,4 +1,4 @@
-"""H100 inference engine of the bottleneck ResNet trunks (ResNet50/101/152, -IBN-A).
+"""H100 inference engine of the ResNet trunks: bottleneck (ResNet50/101/152, -IBN-A) and BasicBlock (ResNet18/34).
 
 TrunkEngine is the ctypes form of the ctl_trunk handle (csrc/trunk.cu, the C ABI a non-Python host binds): the handle
 packs a reference-layout state_dict (keys of modelling/backbones/resnet.py:90-120 / resnet_ibn_a.py:77-124) into kernel
@@ -20,6 +20,7 @@ import torch
 from ... import _native as N
 
 R50_LAYERS = (3, 4, 6, 3)
+BLOCKS = {"bottleneck": N.CTL_BLOCK_BOTTLENECK, "basic": N.CTL_BLOCK_BASIC}
 
 
 def pack_stem_fused(w_folded: torch.Tensor) -> torch.Tensor:
@@ -32,15 +33,20 @@ def pack_stem_fused(w_folded: torch.Tensor) -> torch.Tensor:
 
 class TrunkEngine:
     """Packed weights + forward.  `state` is the `base.*`-stripped trunk state_dict on any
-    device; `bn_head` optionally the BatchNorm1d(2048) of ModelBase (bases.py:83) for `embed`."""
+    device; `bn_head` optionally the BatchNorm1d(feature_dim) of ModelBase (bases.py:83) for `embed`.  `block` is
+    "bottleneck" (feature_dim 2048) or "basic" (ResNet18/34, feature_dim 512)."""
 
     def __init__(self, state: Dict[str, torch.Tensor], device, ibn: bool = False, last_stride: int = 1,
-                 layers=R50_LAYERS, bn_head: Optional[Dict[str, torch.Tensor]] = None):
+                 layers=R50_LAYERS, bn_head: Optional[Dict[str, torch.Tensor]] = None, block: str = "bottleneck"):
+        if block not in BLOCKS:
+            raise ValueError(f"block={block!r}: expected one of {sorted(BLOCKS)}")
         self.device = torch.device(device)
-        self.ibn, self.last_stride = ibn, last_stride
+        self.ibn, self.last_stride, self.block = ibn, last_stride, block
         self.launches_per_forward = 0  # kernels launched by the last forward / forward_u8
         self._h = C.c_void_p()
-        N.check(N.lib().ctl_trunk_create(C.byref(self._h), int(ibn), int(last_stride), (C.c_int32 * 4)(*layers)))
+        N.check(N.lib().ctl_trunk_create_ex(C.byref(self._h), BLOCKS[block], int(ibn), int(last_stride),
+                                            (C.c_int32 * 4)(*layers)))
+        self.feature_dim = N.lib().ctl_trunk_feature_dim(self._h)
         self.pack(state, bn_head)
 
     def pack(self, state: Dict[str, torch.Tensor], bn_head: Optional[Dict[str, torch.Tensor]] = None):
@@ -123,11 +129,11 @@ class TrunkEngine:
         return a, n, hp, wp
 
     def bottlenecks(self, a, n, h, w):
-        """[n, h, w, 64] stem output -> [n, h', w', 2048] trunk output; `a` is only read."""
+        """[n, h, w, 64] stem output -> [n, h', w', feature_dim] trunk output; `a` is only read."""
         ho, wo = h, w
         for s in (2, 2, self.last_stride):  # first blocks of layer2, layer3, layer4: 3x3 / s, pad 1
             ho, wo = (ho + 2 - 3) // s + 1, (wo + 2 - 3) // s + 1
-        out = torch.empty(n, ho, wo, 2048, dtype=torch.float16, device=self.device)
+        out = torch.empty(n, ho, wo, self.feature_dim, dtype=torch.float16, device=self.device)
         ws = self._workspace(n, 4 * h, 4 * w)  # a 4h x 4w image has this stem output and no larger stem temporary
         N.check(N.lib().ctl_embed_blocks(self._h, a.data_ptr(), n, h, w, out.data_ptr(), ws.data_ptr(), ws.numel(),
                                          N.stream_ptr()))
@@ -135,8 +141,8 @@ class TrunkEngine:
 
     def tail(self, a, n, h, w, want_base=False, want_emb=False):
         """global average pool (+ the folded eval BatchNorm1d head)."""
-        feat = torch.empty(n, 2048, dtype=torch.float32, device=self.device)
-        emb = torch.empty(n, 2048, dtype=torch.float32, device=self.device) if (want_emb and self.has_head) else None
+        feat = torch.empty(n, self.feature_dim, dtype=torch.float32, device=self.device)
+        emb = torch.empty(n, self.feature_dim, dtype=torch.float32, device=self.device) if (want_emb and self.has_head) else None
         N.check(N.lib().ctl_embed_head(self._h, a.data_ptr(), n, h * w, feat.data_ptr(), N.ptr(emb), N.stream_ptr()))
         out = {"global_feat": feat}
         if want_base:

@@ -1,4 +1,4 @@
-"""Train-mode bottleneck ResNet trunk on the H100 kernels: forward with batch-statistics BatchNorm and the full backward
+"""Train-mode ResNet trunk (bottleneck or BasicBlock) on the H100 kernels: forward with batch-statistics BatchNorm and the full backward
 (what autograd does through modelling/backbones/resnet.py:67-87,122-133 + baseline.py:91-96 in the reference).
 
 The layer walk is the ctl_trainer handle's (csrc/trunk_train.cu, the C ABI a non-Python host binds): per conv+BN of
@@ -21,6 +21,7 @@ from typing import Dict, List, Tuple
 import torch
 
 from ... import _native as N
+from .engine import BLOCKS
 
 R50_LAYERS = (3, 4, 6, 3)
 
@@ -34,16 +35,21 @@ def _named(tensors: Dict[str, torch.Tensor]):
 
 class TrunkTrainer:
     """`params`: name -> tensor with the reference's `base.*`-stripped names (conv weights [Cout, Cin, k, k], BN
-    weight / bias fp32 on the device; BN running_mean / running_var are updated in place)."""
+    weight / bias fp32 on the device; BN running_mean / running_var are updated in place).  `block` is "bottleneck"
+    (feature_dim 2048) or "basic" (ResNet18/34, feature_dim 512)."""
 
     def __init__(self, device, last_stride: int = 1, layers=R50_LAYERS, grad_scale: float = 1024.0,
-                 momentum: float = 0.1, graphs: bool = False, ibn: bool = False):
+                 momentum: float = 0.1, graphs: bool = False, ibn: bool = False, block: str = "bottleneck"):
+        if block not in BLOCKS:
+            raise ValueError(f"block={block!r}: expected one of {sorted(BLOCKS)}")
         self.device = torch.device(device)
         self.ibn = ibn  # resnet_ibn_a.py: ReLU after the stem, IBN (InstanceNorm half + BatchNorm half) as bn1 of layer1-3
+        self.block = block
         self.last_stride, self.layers, self.grad_scale, self.momentum = last_stride, tuple(layers), float(grad_scale), momentum
         self._h = C.c_void_p()
-        N.check(N.lib().ctl_trainer_create(C.byref(self._h), int(ibn), int(last_stride), float(momentum),
-                                           (C.c_int32 * 4)(*self.layers)))
+        N.check(N.lib().ctl_trainer_create_ex(C.byref(self._h), BLOCKS[block], int(ibn), int(last_stride), float(momentum),
+                                              (C.c_int32 * 4)(*self.layers)))
+        self.feature_dim = N.lib().ctl_trainer_feature_dim(self._h)
         self._bound = None  # (name, data_ptr) of the bound parameters
         self._ws = None
         self._x = None  # the backward's stem im2col reads the input again
@@ -81,7 +87,7 @@ class TrunkTrainer:
         self._x = x.float().contiguous()
         n, _, H, W = self._x.shape
         self._workspace(n, H, W)
-        feat = torch.empty(n, 2048, device=self.device)
+        feat = torch.empty(n, self.feature_dim, device=self.device)
         with torch.cuda.device(self.device):
             N.check(N.lib().ctl_train_forward(self._h, self._x.data_ptr(), n, H, W, feat.data_ptr(), self._ws.data_ptr(),
                                               self._ws.numel(), N.stream_ptr()))
@@ -95,7 +101,7 @@ class TrunkTrainer:
         return self.grads
 
     def forward(self, x: torch.Tensor, params: Dict[str, torch.Tensor]) -> torch.Tensor:
-        """x: [B, 3, H, W] fp32 NCHW on the device -> global_feat [B, 2048] fp32; keeps what backward needs."""
+        """x: [B, 3, H, W] fp32 NCHW on the device -> global_feat [B, feature_dim] fp32; keeps what backward needs."""
         N.require_cuda(x)
         if not self.graphs:
             self._bind(params)
@@ -110,7 +116,7 @@ class TrunkTrainer:
         return g["feat"].clone()
 
     def backward(self, dfeat: torch.Tensor) -> Dict[str, torch.Tensor]:
-        """dfeat: [B, 2048] fp32 = dLoss/dglobal_feat -> {param name: fp32 gradient in the reference's layout}.
+        """dfeat: [B, feature_dim] fp32 = dLoss/dglobal_feat -> {param name: fp32 gradient in the reference's layout}.
         Copies: the next backward overwrites the bound gradient buffers, and autograd may keep these as `.grad`."""
         g = self._graph
         if g is None:
@@ -127,7 +133,7 @@ class TrunkTrainer:
         n, _, H, W = sx.shape
         self._workspace(n, H, W)  # outside the capture: the graphs keep its address
         running = {k: v.clone() for k, v in self._params.items() if "running" in k}
-        sdf = torch.zeros(n, 2048, device=self.device)
+        sdf = torch.zeros(n, self.feature_dim, device=self.device)
         side = torch.cuda.Stream(device=self.device)
         side.wait_stream(torch.cuda.current_stream(self.device))
         with torch.cuda.stream(side):  # eager warm-up: function attributes, allocator pools
@@ -147,8 +153,8 @@ class TrunkTrainer:
 
     def saved_activations(self) -> List[Tuple[torch.Tensor, torch.Tensor]]:
         """(y, z) of the last forward as NHWC fp16 views into the workspace: the stem's raw conv output and its
-        normalised output first, then every conv + BatchNorm in forward order (conv1, conv2, downsample, conv3 per
-        block) -- the order oracle.trunk_train_fp16sim(forced=...) takes."""
+        normalised output first, then every conv + BatchNorm in forward order (conv1, conv2, [downsample], conv3 per
+        bottleneck; conv1, [downsample], conv2 per BasicBlock) -- the order the oracles' `forced=` takes."""
         y, z, shape = C.c_void_p(), C.c_void_p(), (C.c_int32 * 4)()
         base = N.ptr(self._ws)
 
@@ -158,7 +164,11 @@ class TrunkTrainer:
             return self._ws[off:off + 2 * numel].view(torch.float16).view(*shape)
 
         out = []
-        for i in range(1 + 3 * sum(self.layers) + 4):  # stem + three convs per block + one downsample per stage
+        if self.block == "basic":  # stem + two convs per block + the downsamples of layer2-4
+            count = 1 + 2 * sum(self.layers) + 3
+        else:  # stem + three convs per block + one downsample per stage
+            count = 1 + 3 * sum(self.layers) + 4
+        for i in range(count):
             N.check(N.lib().ctl_train_saved(self._h, i, C.byref(y), C.byref(z), shape))
             out.append((view(y.value), view(z.value)))
         return out

@@ -1,8 +1,8 @@
 """Reference-layout parameter containers for the ResNet / ResNet-IBN-A trunks.
 
 These modules exist so that `state_dict()` keys, shapes and the optimizer's named_parameters
-are IDENTICAL to modelling/backbones/resnet.py:90-120 and resnet_ibn_a.py:77-124 of the
-reference (checkpoints load unchanged).  They carry no arithmetic: the forward pass is the
+are IDENTICAL to modelling/backbones/resnet.py:90-120 (Bottleneck or BasicBlock) and
+resnet_ibn_a.py:77-124 of the reference (checkpoints load unchanged).  They carry no arithmetic: the forward pass is the
 H100 engine (engine.py, engine_train.py); the layer graph is described by the C handles they
 drive (csrc/trunk.cu, csrc/trunk_train.cu), not here.
 """
@@ -43,12 +43,33 @@ class Bottleneck(nn.Module):
         self.stride = stride
 
 
-class ResNetParams(nn.Module):
-    """Parameter tree of ResNet(last_stride, Bottleneck, layers) / ResNet_IBN(...)."""
+class BasicBlock(nn.Module):
+    """resnet.py:19-48: two 3x3 convolutions (the first one strided)."""
 
-    def __init__(self, last_stride=1, layers=(3, 4, 6, 3), ibn=False):
+    expansion = 1
+
+    def __init__(self, inplanes, planes, stride=1, downsample=None):
         super().__init__()
+        self.conv1 = _conv(inplanes, planes, 3, stride)
+        self.bn1 = nn.BatchNorm2d(planes)
+        self.conv2 = _conv(planes, planes, 3)
+        self.bn2 = nn.BatchNorm2d(planes)
+        self.downsample = downsample
+        self.stride = stride
+
+
+class ResNetParams(nn.Module):
+    """Parameter tree of ResNet(last_stride, Bottleneck | BasicBlock, layers) / ResNet_IBN(...).
+    `block` is "bottleneck" or "basic"; IBN-a exists for bottlenecks only."""
+
+    def __init__(self, last_stride=1, layers=(3, 4, 6, 3), ibn=False, block="bottleneck"):
+        super().__init__()
+        if block not in ("bottleneck", "basic"):
+            raise ValueError(f"block={block!r}: expected 'bottleneck' or 'basic'")
+        if ibn and block != "bottleneck":
+            raise ValueError("IBN-a is defined for bottleneck blocks only (resnet_ibn_a.py)")
         self.ibn = ibn
+        self.block = block
         self.layers_cfg = tuple(layers)
         self.last_stride = last_stride
         self.inplanes = 64
@@ -63,6 +84,14 @@ class ResNetParams(nn.Module):
         self.random_init()
 
     def _make_layer(self, planes, blocks, stride):
+        if self.block == "basic":  # resnet.py:103-120 with expansion 1
+            down = None
+            if stride != 1 or self.inplanes != planes:
+                down = nn.Sequential(_conv(self.inplanes, planes, 1, stride), nn.BatchNorm2d(planes))
+            mods = [BasicBlock(self.inplanes, planes, stride, down)]
+            self.inplanes = planes
+            mods += [BasicBlock(planes, planes) for _ in range(1, blocks)]
+            return nn.Sequential(*mods)
         down = None
         if stride != 1 or self.inplanes != planes * 4:
             down = nn.Sequential(_conv(self.inplanes, planes * 4, 1, stride), nn.BatchNorm2d(planes * 4))

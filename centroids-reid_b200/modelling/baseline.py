@@ -2,7 +2,7 @@
 
 Parameters live in reference-layout modules (`self.base.*`); eval-mode forward runs the H100
 engine, whose packed operands are rebuilt lazily whenever the parameters change
-(`invalidate()`; call it after `opt.step()` / `load_state_dict`).  Train-mode forward (ResNet-50) runs the
+(`invalidate()`; call it after `opt.step()` / `load_state_dict`).  Train-mode forward runs the
 training engine (batch-statistics BatchNorm, running statistics updated in place) and is differentiable:
 `global_feat.backward()` fills `.grad` of every trunk parameter through the H100 backward kernels.
 """
@@ -17,8 +17,11 @@ from .backbones.engine import TrunkEngine
 from .backbones.engine_train import TrunkTrainer
 from .backbones.resnet import ResNetParams
 
-_LAYERS = {"resnet50": ((3, 4, 6, 3), False), "resnet101": ((3, 4, 23, 3), False), "resnet152": ((3, 8, 36, 3), False),
-           "resnet50_ibn_a": ((3, 4, 6, 3), True), "resnet101_ibn_a": ((3, 4, 23, 3), True)}
+# MODEL.NAME -> (blocks per stage, IBN-a, block kind); modelling/baseline.py:56-100
+_LAYERS = {"resnet18": ((2, 2, 2, 2), False, "basic"), "resnet34": ((3, 4, 6, 3), False, "basic"),
+           "resnet50": ((3, 4, 6, 3), False, "bottleneck"), "resnet101": ((3, 4, 23, 3), False, "bottleneck"),
+           "resnet152": ((3, 8, 36, 3), False, "bottleneck"), "resnet50_ibn_a": ((3, 4, 6, 3), True, "bottleneck"),
+           "resnet101_ibn_a": ((3, 4, 23, 3), True, "bottleneck")}
 
 
 class _TrunkTrainFn(torch.autograd.Function):
@@ -52,11 +55,12 @@ class Baseline(nn.Module):
         super().__init__()
         name = cfg.MODEL.NAME
         if name not in _LAYERS:
-            raise NotImplementedError(f"MODEL.NAME={name!r}: the H100 trunk covers the bottleneck ResNets {sorted(_LAYERS)}")
-        layers, ibn = _LAYERS[name]
+            raise NotImplementedError(f"MODEL.NAME={name!r}: the H100 trunk covers the ResNets {sorted(_LAYERS)}")
+        layers, ibn, block = _LAYERS[name]
+        self.in_planes = 512 if block == "basic" else 2048  # baseline.py:58-69
         self.model_name = name
         self.use_mixed_precision = cfg.USE_MIXED_PRECISION
-        self.base = ResNetParams(cfg.MODEL.LAST_STRIDE, layers, ibn)
+        self.base = ResNetParams(cfg.MODEL.LAST_STRIDE, layers, ibn, block)
         if cfg.MODEL.PRETRAINED and not cfg.MODEL.RESUME_TRAINING and not cfg.TEST.ONLY_TEST:
             self.base.load_param(cfg.MODEL.PRETRAIN_PATH)  # modelling/baseline.py:84-87
             print("Loading pretrained ImageNet model......")
@@ -92,7 +96,7 @@ class Baseline(nn.Module):
                 head = dict(weight=bn_head.weight, bias=bn_head.bias, running_mean=bn_head.running_mean,
                             running_var=bn_head.running_var)
             self._engine = TrunkEngine(sd, dev, ibn=self.base.ibn, last_stride=self.base.last_stride,
-                                       layers=self.base.layers_cfg, bn_head=head)
+                                       layers=self.base.layers_cfg, bn_head=head, block=self.base.block)
             self._engine_key = key
         return self._engine
 
@@ -104,7 +108,8 @@ class Baseline(nn.Module):
                 from ..solver.build import DynamicLossScaler
 
                 self._trainer = TrunkTrainer(dev, last_stride=self.base.last_stride, layers=self.base.layers_cfg,
-                                             graphs=os.environ.get("CTL_TRAIN_GRAPHS", "1") == "1", ibn=self.base.ibn)
+                                             graphs=os.environ.get("CTL_TRAIN_GRAPHS", "1") == "1", ibn=self.base.ibn,
+                                             block=self.base.block)
                 self.loss_scaler = DynamicLossScaler(dev, base_scale=self._trainer.grad_scale,
                                                      enabled=os.environ.get("CTL_DYNAMIC_LOSS_SCALE", "1") == "1")
             names = [k for k, _ in self.base.named_parameters()]

@@ -144,6 +144,10 @@ class CTLModel(_Base):
         self.backbone = Baseline(self.hparams)
         self.contrastive_loss = TripletLoss(self.hparams.SOLVER.MARGIN, self.hparams.SOLVER.DISTANCE_FUNC)
         d_model = self.hparams.MODEL.BACKBONE_EMB_SIZE
+        if d_model != self.backbone.in_planes:
+            # the loss kernels index bn / fc_query / centers by the feature width: a mismatch would be silently wrong
+            raise ValueError(f"MODEL.BACKBONE_EMB_SIZE={d_model} but MODEL.NAME={self.hparams.MODEL.NAME!r} produces "
+                             f"{self.backbone.in_planes}-wide features")
         self.xent = CrossEntropyLabelSmooth(num_classes=self.hparams.num_classes)
         self.center_loss = CenterLoss(num_classes=self.hparams.num_classes, feat_dim=d_model,
                                       use_gpu=torch.cuda.is_available())

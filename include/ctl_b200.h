@@ -253,6 +253,16 @@ int ctl_conv2d_nhwc_f16(const void* x, int32_t n, int32_t h, int32_t w, int32_t 
 int ctl_conv1x1_dual_nhwc_f16(const void* x1, int32_t cin1, const void* x2, int32_t h2, int32_t w2, int32_t cin2,
                               int32_t stride2, int32_t n, const void* weight_cat, const float* bias, void* out,
                               int32_t cout, int32_t relu, ctl_stream_t stream);
+/* The 3x3 counterpart: a 3x3 / 1 convolution (pad 1) and a 1x1 convolution summed in ONE GEMM -- the last layer of a
+ * BasicBlock's first block, out = act(bn2(conv2(x1)) + bn_d(downsample(x2))) (resnet.py:31-47 with a downsample branch):
+ *   out[n][i][j][:] = act( sum_{r,s} W[:, (3r + s) cin1 ..][:cin1] x1[n][i + r - 1][j + s - 1][:]
+ *                          + W[:, 9 cin1:] x2[n][i*stride2][j*stride2][:] + bias )
+ * x1: NHWC fp16 [n][h2/stride2][w2/stride2][cin1] (zero outside); x2: NHWC fp16 [n][h2][w2][cin2]; weight_cat:
+ * [cout][9 cin1 + cin2] fp16 (the folded [cout][3][3][cin1] weights, then the folded shortcut), bias = sum of the two
+ * folded biases.  The shortcut tensor is never written to or re-read from HBM. */
+int ctl_conv3x3_dual_nhwc_f16(const void* x1, int32_t cin1, const void* x2, int32_t h2, int32_t w2, int32_t cin2,
+                              int32_t stride2, int32_t n, const void* weight_cat, const float* bias, void* out,
+                              int32_t cout, int32_t relu, ctl_stream_t stream);
 /* The last 1x1 of a bottleneck and the first 1x1 of the next one in ONE launch (the block output is not re-read):
  *   out [n][i][j][:] = relu( W[:, :cin1] x1[n][i][j][:] [+ W[:, cin1:] x2[n][i*stride2][j*stride2][:]] + bias
  *                            [+ residual[n][i][j][:]] )
@@ -298,15 +308,21 @@ int ctl_instnorm_relu_nhwc_f16(void* x, int32_t n, int32_t hw, int32_t c, int32_
  * Baseline.forward's pooling (modelling/baseline.py:91-96), ModelBase.validation_step / inference_utils._inference
  * (modelling/bases.py:169-177, inference/inference_utils.py:104-113).  This is the eval trunk's only driver;
  * modelling/backbones/engine.py::TrunkEngine is its ctypes form.
- *   ctl_trunk_create   : bottleneck ResNet with `stage_blocks` blocks per stage ({3, 4, 6, 3} = ResNet50, {3, 4, 23, 3} =
- *                        ResNet101, {3, 8, 36, 3} = ResNet152, each >= 1), IBN-a when `ibn` != 0, MODEL.LAST_STRIDE 1 or 2.
+ *   ctl_trunk_create_ex: ResNet of `block` = CTL_BLOCK_BOTTLENECK (resnet.py:51-87) or CTL_BLOCK_BASIC (resnet.py:19-48)
+ *                        blocks with `stage_blocks` blocks per stage (bottleneck: {3, 4, 6, 3} = ResNet50, {3, 4, 23, 3} =
+ *                        ResNet101, {3, 8, 36, 3} = ResNet152; basic: {2, 2, 2, 2} = ResNet18, {3, 4, 6, 3} = ResNet34;
+ *                        each >= 1), IBN-a when `ibn` != 0 (bottleneck only), MODEL.LAST_STRIDE 1 or 2.  An unknown
+ *                        `block`, or a basic block with `ibn` != 0, is CTL_ERR_INVALID_ARGUMENT before any device work.
+ *   ctl_trunk_create   : ctl_trunk_create_ex with block = CTL_BLOCK_BOTTLENECK.
+ *   ctl_trunk_feature_dim: width of the trunk output and of the features below: 2048 (bottleneck) or 512 (basic).
+ *                        Host only.
  *   ctl_weights_pack   : `tensors` = the reference's `base.*`-stripped state_dict as DEVICE fp32 pointers, by name
  *                        ("conv1.weight", "bn1.running_var", "layer3.0.downsample.1.bias", "layer1.0.bn1.IN.weight", ...),
- *                        plus optionally "bn_head.weight|bias|running_mean|running_var" (ModelBase.bn, [2048]).  Folds every
- *                        eval BatchNorm into fp16 weights + fp32 biases on the device and keeps the packed operands in the
- *                        handle.  Call again whenever the parameters change (after opt.step(), load_state_dict).
- *   ctl_embed_forward  : x NCHW fp32 [n][3][h][w] on the device -> out_feat [n][2048] (global_feat) and / or out_emb
- *                        [n][2048] (= eval BatchNorm1d(global_feat); needs the bn_head.* tensors).  Activations live in the
+ *                        plus optionally "bn_head.weight|bias|running_mean|running_var" (ModelBase.bn, [feature_dim]).
+ *                        Folds every eval BatchNorm into fp16 weights + fp32 biases on the device and keeps the packed
+ *                        operands in the handle.  Call again whenever the parameters change (after opt.step(), load_state_dict).
+ *   ctl_embed_forward  : x NCHW fp32 [n][3][h][w] on the device -> out_feat [n][feature_dim] (global_feat) and / or out_emb
+ *                        [n][feature_dim] (= eval BatchNorm1d(global_feat); needs the bn_head.* tensors).  Activations live in the
  *                        caller's workspace of ctl_embed_workspace_bytes(h, n, h, w) bytes.  The entry point for C hosts:
  *                        stem -> blocks -> head below in one call.
  * The same forward in three stages, for hosts that capture or time them separately; NHWC fp16 tensors between them are
@@ -315,9 +331,10 @@ int ctl_instnorm_relu_nhwc_f16(void* x, int32_t n, int32_t hw, int32_t c, int32_
  *                        with h/2 = (h - 1)/2 + 1 (wp alike).  x is fp32 NCHW [n][3][h][w], or with mean3_host and std3_host
  *                        uint8 NHWC [n][h][w][3] crops normalised as ctl_stem_pool_fused_u8 does (h % 4 == 0, even w <= 128).
  *                        Workspace: ctl_embed_workspace_bytes(h, n, h, w) bytes (the tensor-core stem's temporary).
- *   ctl_embed_blocks   : x [n][hp][wp][64] -> out [n][ho][wo][2048] (ho = hp / 4, / 8 with last_stride 2).  Never writes x.
- *                        Workspace: ctl_embed_workspace_bytes(h, n, 4 * hp, 4 * wp) bytes, no more than the image size needs.
- *   ctl_embed_head     : x [n][hw][2048] -> out_feat and / or out_emb as ctl_embed_forward.
+ *   ctl_embed_blocks   : x [n][hp][wp][64] -> out [n][ho][wo][feature_dim] (ho = hp / 4, / 8 with last_stride 2).  Never
+ *                        writes x.  Workspace: ctl_embed_workspace_bytes(h, n, 4 * hp, 4 * wp) bytes, no more than the image
+ *                        size needs.
+ *   ctl_embed_head     : x [n][hw][feature_dim] -> out_feat and / or out_emb as ctl_embed_forward.
  *   ctl_embed_launches : kernels launched by the handle's last ctl_embed_* call.
  * The fused stem (h % 4 == 0, even w <= 128) stages its input in a zero-bordered buffer that the handle allocates at the
  * first call with each (n, h, w) and keeps until ctl_trunk_destroy; a call that would allocate one while `stream` is
@@ -330,7 +347,11 @@ typedef struct ctl_named_tensor {
   const float* data; /* device pointer */
   int64_t numel;
 } ctl_named_tensor;
+#define CTL_BLOCK_BOTTLENECK 0
+#define CTL_BLOCK_BASIC 1
 int ctl_trunk_create(ctl_trunk** out, int32_t ibn, int32_t last_stride, const int32_t stage_blocks[4]);
+int ctl_trunk_create_ex(ctl_trunk** out, int32_t block, int32_t ibn, int32_t last_stride, const int32_t stage_blocks[4]);
+int32_t ctl_trunk_feature_dim(const ctl_trunk* h);
 void ctl_trunk_destroy(ctl_trunk* h);
 int ctl_weights_pack(ctl_trunk* h, const ctl_named_tensor* tensors, int32_t n_tensors, ctl_stream_t stream);
 size_t ctl_embed_workspace_bytes(const ctl_trunk* h, int32_t n, int32_t height, int32_t width);
@@ -421,26 +442,32 @@ int ctl_stem_im2col_f16(const float* x_nchw, int32_t n, int32_t h, int32_t w, vo
 /* ---- train-mode trunk behind an opaque handle (SURVEY 8b: the train forward / backward variants) ----
  * replaces: torch autograd through ResNet.forward / ResNet_IBN.forward in train mode (modelling/backbones/resnet.py:67-87,
  * 122-133, resnet_ibn_a.py:18-32,126-141) + Baseline.forward's pooling (modelling/baseline.py:91-96) inside
- * CTLModel.training_step (train_ctl_model.py:38-179): x -> global_feat [n][2048], then d(loss)/d(global_feat) -> every
- * parameter gradient.  This is the training trunk's only driver; modelling/backbones/engine_train.py::TrunkTrainer
+ * CTLModel.training_step (train_ctl_model.py:38-179): x -> global_feat [n][feature_dim], then d(loss)/d(global_feat) ->
+ * every parameter gradient.  This is the training trunk's only driver; modelling/backbones/engine_train.py::TrunkTrainer
  * is its ctypes form.
- *   ctl_trainer_create      : bottleneck ResNet with `stage_blocks` blocks per stage ({3, 4, 6, 3} = ResNet50,
- *                             {3, 4, 23, 3} = ResNet101, each >= 1), IBN-a when `ibn` != 0, MODEL.LAST_STRIDE 1 or 2,
- *                             BatchNorm momentum.
+ *   ctl_trainer_create_ex   : ResNet of `block` (CTL_BLOCK_BOTTLENECK or CTL_BLOCK_BASIC) blocks with `stage_blocks`
+ *                             blocks per stage ({3, 4, 6, 3} = ResNet50 / ResNet34, {3, 4, 23, 3} = ResNet101,
+ *                             {2, 2, 2, 2} = ResNet18, each >= 1), IBN-a when `ibn` != 0 (bottleneck only),
+ *                             MODEL.LAST_STRIDE 1 or 2, BatchNorm momentum.  Argument errors as ctl_trunk_create_ex.
+ *   ctl_trainer_create      : ctl_trainer_create_ex with block = CTL_BLOCK_BOTTLENECK.
+ *   ctl_trainer_feature_dim : 2048 (bottleneck) or 512 (basic).  Host only.
  *   ctl_trainer_bind        : `params` = the `base.*`-stripped fp32 parameters AND BatchNorm running buffers as device
  *                             pointers, by name (running_mean / running_var optional per layer, updated in place like
  *                             torch); `grads` = one fp32 output per PARAMETER, same name, the parameter's own layout
  *                             (conv [Cout][Cin][k][k]).  The handle keeps the pointers: re-bind when storage moves.
  *   ctl_train_workspace_bytes: bytes of the caller's workspace for one (n, h, w) step: the saved activations of the
  *                             forward + the scratch of the backward (≈ 60 MB per 256x128 image).
- *   ctl_train_forward       : x NCHW fp32 -> out_feat [n][2048] fp32 (global_feat); saved tensors stay in `workspace`.
- *   ctl_train_backward      : dfeat [n][2048] fp32 = dLoss/dglobal_feat.  Activation gradients are computed on
+ *   ctl_train_forward       : x NCHW fp32 -> out_feat [n][feature_dim] fp32 (global_feat); saved tensors stay in
+ *                             `workspace`.
+ *   ctl_train_backward      : dfeat [n][feature_dim] fp32 = dLoss/dglobal_feat.  Activation gradients are computed on
  *                             grad_scale * dfeat in fp16 (loss scaling, the role of PL's GradScaler, utils/misc.py:111);
  *                             the parameter gradients are written UN-scaled.  Same workspace as the forward, once per forward.
  *   ctl_train_saved         : inspection call for checkers: the fp16 NHWC tensors the last completed forward saved in
  *                             its workspace, raw conv output `y` and normalised output `z`, with their shape `nhwc`.
- *                             index 0 = the stem, 1... = every conv + BatchNorm in forward order (conv1, conv2,
- *                             downsample, conv3 per block).  An error before a forward or out of range.
+ *                             index 0 = the stem, 1... = every conv + BatchNorm in forward order: per bottleneck conv1,
+ *                             conv2, [downsample], conv3; per basic block conv1, [downsample], conv2 (conv2's BatchNorm
+ *                             adds the shortcut, so the downsample runs before it).  An error before a forward or out of
+ *                             range.
  * Not thread-safe; all launches go to `stream`; 256-byte aligned workspace. */
 typedef struct ctl_trainer ctl_trainer;
 typedef struct ctl_named_buffer {
@@ -449,6 +476,9 @@ typedef struct ctl_named_buffer {
   int64_t numel;
 } ctl_named_buffer;
 int ctl_trainer_create(ctl_trainer** out, int32_t ibn, int32_t last_stride, float momentum, const int32_t stage_blocks[4]);
+int ctl_trainer_create_ex(ctl_trainer** out, int32_t block, int32_t ibn, int32_t last_stride, float momentum,
+                          const int32_t stage_blocks[4]);
+int32_t ctl_trainer_feature_dim(const ctl_trainer* t);
 void ctl_trainer_destroy(ctl_trainer* t);
 int ctl_trainer_bind(ctl_trainer* t, const ctl_named_tensor* params, int32_t n_params, const ctl_named_buffer* grads,
                      int32_t n_grads);
