@@ -7,7 +7,7 @@ mikwieczorek/centroids-reid, behind the reference's own module surface:
     losses.center_loss    CenterLoss                       (losses/center_loss.py)
     utils.reid_metric     get_euclidean, get_cosine, get_dist_func, R1_mAP
     utils.eval_reid       eval_func
-    modelling.*           Baseline, CTL step               (modelling/, train_ctl_model.py)
+    modelling.*           Baseline, CTL step, base-model step (modelling/, train_ctl_model.py, train_base_model.py)
     inference.*           run_inference, calculate_centroids, get_similar
 
 The directory name carries a hyphen (it is mandated by the build contract), so import it as

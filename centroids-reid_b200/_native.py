@@ -49,6 +49,17 @@ class LossConfig(C.Structure):
 _cfgp = C.POINTER(LossConfig)
 
 
+class BaseLossConfig(C.Structure):
+    """struct ctl_base_loss_config (include/ctl_b200.h)."""
+
+    _fields_ = [("B", _i32), ("D", _i32), ("C", _i32), ("margin", _f), ("soft_margin", _i32), ("cosine", _i32),
+                ("center_weight", _f), ("xent_weight", _f), ("triplet_weight", _f), ("bn_eps", _f),
+                ("bn_momentum", _f), ("label_smooth", _f)]
+
+
+_bcfgp = C.POINTER(BaseLossConfig)
+
+
 class PassDesc(C.Structure):
     """struct ctl_pass_desc (include/ctl_b200.h)."""
 
@@ -97,6 +108,8 @@ SIGNATURES = {
     "ctl_triplet_step_ex": (C.c_int, [_p, _i32, _i32, _p, _p, _f, _i32, _i32, _p, _p, _p, _p, _p, _sz, _p]),
     "ctl_center_loss_step": (C.c_int, [_p, _i32, _i32, _p, _p, _i32, _p, _p, _p, _p, _sz, _p]),
     "ctl_xent_smooth_step": (C.c_int, [_p, _i32, _i32, _p, _f, _p, _p, _p, _sz, _p]),
+    "ctl_base_loss_workspace_bytes": (_sz, [_bcfgp]),
+    "ctl_base_loss_step": (C.c_int, [_bcfgp] + [_p] * 14 + [_p, _sz, _p]),
     "ctl_conv2d_nhwc_f16": (C.c_int, [_p, _i32, _i32, _i32, _i32, _p, _p, _p, _p, _i32, _i32, _i32, _i32, _i32, _p]),
     "ctl_conv1x1_dual_nhwc_f16": (C.c_int, [_p, _i32, _p, _i32, _i32, _i32, _i32, _i32, _p, _p, _p, _i32, _i32, _p]),
     "ctl_conv3x3_dual_nhwc_f16": (C.c_int, [_p, _i32, _p, _i32, _i32, _i32, _i32, _i32, _p, _p, _p, _i32, _i32, _p]),

@@ -1071,3 +1071,190 @@ int ctl_xent_smooth_step(const float* logits, int32_t b, int32_t c, const int32_
 
 }  // extern "C"
 
+// ---------------------------------------------------------------------------------------
+// base-model step (train_base_model.py:38-96): query triplet over all B rows with the anchors
+// masked to is_real, center loss and BN1d -> fc -> label-smoothed CE over ALL B rows (mock rows
+// included).  The kernels above do the work; only the scalar assembly and the final row-wise
+// combine of the three feature-gradient terms are specific to this step.
+// ---------------------------------------------------------------------------------------
+namespace ctl {
+
+// out[0..5] = total, xent, triplet (already written by single_reduce_kernel), center, dist_ap, dist_an
+__global__ void base_scalars_kernel(int B, int C, MineOut o, const float* __restrict__ center_rows,
+                                    const float* __restrict__ xent_rows, float w_center, float w_xent,
+                                    const int* __restrict__ bad, float* __restrict__ out) {
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  float cs = 0.f, xs = 0.f, sap = 0.f, san = 0.f;
+  int n_anchor = 0;
+  for (int b = 0; b < B; ++b) {
+    cs += center_rows[b];
+    xs += xent_rows[b];
+    if (o.a_row[b] >= 0) { sap += o.d_ap[b]; san += o.d_an[b]; ++n_anchor; }
+  }
+  // every one of the B(C-1) masked zeros is clamped to 1e-12 (center_loss.py:43-44)
+  const float center = w_center * (cs + (float)B * (float)(C - 1) * 1e-12f) / (float)B;
+  const float xent = w_xent * xs / (float)B;
+  out[1] = xent;
+  out[3] = center;
+  out[0] = center + xent + out[2];  // train_base_model.py:75 order
+  // train_base_model.py:91-94: means over the masked (real) anchors
+  out[4] = n_anchor > 0 ? sap / (float)n_anchor : 0.f;
+  out[5] = n_anchor > 0 ? san / (float)n_anchor : 0.f;
+  if (*bad)  // a label outside [0, C): poison every reported value (payload 1; the shim raises ValueError)
+    for (int i = 0; i < 6; ++i) out[i] = __int_as_float(0x7fc00001);
+}
+
+// dF = triplet term + BN/head term + center term.  The triplet term is rowsum_i F_i - (Cm F)_i (euclidean) or, for
+// cosine, already in dF (cosine_combine_kernel wrote the gradient through the row normalisation there).
+__global__ void __launch_bounds__(256) base_combine_kernel(const float* __restrict__ F, int B, int D, int cosine,
+                                                           const float* __restrict__ dEm, const float* __restrict__ rowsum,
+                                                           const float* __restrict__ dF_head,
+                                                           const int* __restrict__ labels,
+                                                           const float* __restrict__ centers,
+                                                           const unsigned char* __restrict__ row_sat, float w_center,
+                                                           float* __restrict__ dF) {
+  const int i = blockIdx.x;
+  const float gc = row_sat[i] ? 0.f : 2.f * w_center / (float)B;
+  const float* c = centers + (size_t)labels[i] * D;
+  for (int j = threadIdx.x; j < D; j += blockDim.x) {
+    const size_t k = (size_t)i * D + j;
+    const float f = F[k];
+    float g = cosine ? dF[k] : __fmaf_rn(rowsum[i], f, dEm[k]);
+    g = __fadd_rn(g, dF_head[k]);
+    if (gc != 0.f) g = __fmaf_rn(gc, f - c[j], g);
+    dF[k] = g;
+  }
+}
+
+struct BaseBuffers {
+  int* labels_safe;  // [B + 1]: range-checked labels, then the out-of-range flag
+  float *sq, *Xn, *norm, *G, *Cm, *rowsum, *dEm, *slot_w;
+  MineOut mine;
+  float *center_rows, *xent_rows, *xhat, *y, *inv_std, *logits, *dy, *dF_head;
+  unsigned char* row_sat;
+  bool ok;
+};
+
+static BaseBuffers carve_base(Workspace& ws, const ctl_base_loss_config& c) {
+  BaseBuffers b;
+  const int B = c.B, D = c.D;
+  b.labels_safe = ws.take<int>((size_t)B + 1);
+  b.sq = ws.take<float>(B);
+  b.Xn = c.cosine ? ws.take<float>((size_t)B * D) : nullptr;
+  b.norm = c.cosine ? ws.take<float>(B) : nullptr;
+  b.G = ws.take<float>((size_t)B * B);
+  b.Cm = ws.take<float>((size_t)B * B);
+  b.rowsum = ws.take<float>(B);
+  b.dEm = ws.take<float>((size_t)B * D);
+  b.slot_w = ws.take<float>(B);
+  b.mine = take_mine(ws, B);
+  b.center_rows = ws.take<float>(B);
+  b.xent_rows = ws.take<float>(B);
+  b.xhat = ws.take<float>((size_t)B * D);
+  b.y = ws.take<float>((size_t)B * D);
+  b.inv_std = ws.take<float>(D);
+  b.logits = ws.take<float>((size_t)B * c.C);
+  b.dy = ws.take<float>((size_t)B * D);
+  b.dF_head = ws.take<float>((size_t)B * D);
+  b.row_sat = ws.take<unsigned char>(B);
+  b.ok = b.labels_safe != nullptr && b.row_sat != nullptr;
+  return b;
+}
+
+static int check_base_cfg(const ctl_base_loss_config* c) {
+  CTL_CHECK_ARG(c != nullptr, "null config");
+  CTL_CHECK_ARG(c->B >= 2 && c->D >= 1 && c->C >= 1, "bad dims B=%d D=%d C=%d", c->B, c->D, c->C);
+  return 0;
+}
+
+}  // namespace ctl
+
+extern "C" {
+
+size_t ctl_base_loss_workspace_bytes(const ctl_base_loss_config* cfg) {
+  if (check_base_cfg(cfg)) return 0;
+  Workspace ws(nullptr, 0);
+  carve_base(ws, *cfg);
+  return ws.off;
+}
+
+int ctl_base_loss_step(const ctl_base_loss_config* cfg, const float* feats, const int32_t* labels,
+                       const uint8_t* is_real, const float* centers, const float* bn_weight, const float* bn_bias,
+                       float* bn_running_mean, float* bn_running_var, const float* fc_weight, float* out_losses,
+                       float* d_feats, float* d_centers, float* d_bn_weight, float* d_fc_weight, void* workspace,
+                       size_t workspace_bytes, ctl_stream_t stream_) {
+  int rc = check_base_cfg(cfg);
+  if (rc) return rc;
+  CTL_CHECK_ARG(feats && labels && is_real && centers && bn_weight && bn_bias && fc_weight && out_losses && d_feats &&
+                    d_centers && d_bn_weight && d_fc_weight && workspace,
+                "null pointer");
+  CTL_CHECK_ARG((bn_running_mean == nullptr) == (bn_running_var == nullptr), "running mean and var: both or neither");
+  if ((rc = ctl_device_check())) return rc;
+  cudaStream_t st = (cudaStream_t)stream_;
+  const ctl_base_loss_config& c = *cfg;
+  const int B = c.B, D = c.D, C = c.C;
+  const int cosine = c.cosine ? 1 : 0;
+  Workspace ws(workspace, workspace_bytes);
+  BaseBuffers b = carve_base(ws, c);
+  if (!b.ok) {
+    set_error("workspace too small: need %zu bytes, have %zu", ws.off, workspace_bytes);
+    return CTL_ERR_WORKSPACE;
+  }
+  // labels index `centers` and the logits: an out-of-range label becomes 0 here and poisons every output below
+  sanitize_labels_kernel<<<1, 256, 0, st>>>(labels, B, C, b.labels_safe, b.labels_safe + B);
+  CTL_LAUNCH_CHECK();
+  labels = b.labels_safe;
+  // ---- query triplet (train_base_model.py:60-65): Gram over all B rows, anchors masked to is_real ----------
+  const float* E = feats;
+  if (cosine) {
+    normalize_rows_kernel<<<B, 256, 0, st>>>(feats, D, b.Xn, b.norm);
+    E = b.Xn;
+  } else {
+    sqnorm_rows_kernel<<<B, 256, 0, st>>>(feats, D, b.sq);
+  }
+  CTL_LAUNCH_CHECK();
+  if ((rc = sgemm(st, B, B, D, E, D, 1, E, 1, D, b.G, B, 1.f, 0.f))) return rc;
+  mine_single_kernel<<<B, 128, 0, st>>>(b.G, b.sq, labels, is_real, B, c.margin, c.soft_margin ? 1 : 0, cosine, b.mine);
+  CTL_LAUNCH_CHECK();
+  single_reduce_kernel<<<1, 32, 0, st>>>(B, b.mine, c.triplet_weight, b.slot_w, out_losses + 2);
+  CTL_LAUNCH_CHECK();
+  build_coef_kernel<<<B, 128, 0, st>>>(B, 0, 0, 1, 1, b.mine, b.slot_w, b.Cm, b.rowsum);
+  CTL_LAUNCH_CHECK();
+  if ((rc = sgemm(st, B, D, B, b.Cm, B, 1, E, D, 1, b.dEm, D, -1.f, 0.f))) return rc;  // -Cm E
+  if (cosine) {
+    cosine_combine_kernel<<<B, 256, 0, st>>>(b.Xn, feats, D, b.dEm, b.norm, d_feats);
+    CTL_LAUNCH_CHECK();
+  }
+  // ---- center loss over all B rows (train_base_model.py:67-69) ------------------------------------------
+  center_rows_kernel<<<B, 256, 0, st>>>(feats, D, labels, nullptr, centers, b.center_rows, b.row_sat);
+  CTL_LAUNCH_CHECK();
+  CTL_CUDA(cudaMemsetAsync(d_centers, 0, (size_t)C * D * sizeof(float), st));
+  center_grad_kernel<<<B, 256, 0, st>>>(feats, B, D, labels, nullptr, b.row_sat, centers, nullptr, B, c.center_weight,
+                                        d_centers);
+  CTL_LAUNCH_CHECK();
+  // ---- head over all B rows (train_base_model.py:70-73): BN1d -> fc -> label-smoothed CE, and its backward --
+  bn_forward_kernel<<<(D + 255) / 256, 256, 0, st>>>(feats, B, D, nullptr, bn_weight, bn_bias, c.bn_eps, c.bn_momentum,
+                                                   1, bn_running_mean, bn_running_var, b.xhat, b.y, b.inv_std);
+  CTL_LAUNCH_CHECK();
+  if ((rc = sgemm(st, B, C, D, b.y, D, 1, fc_weight, 1, D, b.logits, C, 1.f, 0.f))) return rc;  // y W^T
+  xent_rows_kernel<<<B, 256, 0, st>>>(b.logits, C, labels, nullptr, nullptr, B, c.label_smooth, c.xent_weight,
+                                      b.xent_rows);
+  CTL_LAUNCH_CHECK();
+  // logits now hold d(loss)/d(logits)
+  if ((rc = sgemm(st, C, D, B, b.logits, 1, C, b.y, D, 1, d_fc_weight, D, 1.f, 0.f))) return rc;  // dZ^T y
+  if ((rc = sgemm(st, B, D, C, b.logits, C, 1, fc_weight, D, 1, b.dy, D, 1.f, 0.f))) return rc;   // dZ W
+  bn_backward_kernel<<<(D + 255) / 256, 256, 0, st>>>(b.dy, b.xhat, B, D, nullptr, bn_weight, b.inv_std, 1, d_bn_weight,
+                                                    b.dF_head);
+  CTL_LAUNCH_CHECK();
+  // ---- scalars + feature gradient ---------------------------------------------------------------------------
+  base_scalars_kernel<<<1, 32, 0, st>>>(B, C, b.mine, b.center_rows, b.xent_rows, c.center_weight, c.xent_weight,
+                                        b.labels_safe + B, out_losses);
+  CTL_LAUNCH_CHECK();
+  base_combine_kernel<<<B, 256, 0, st>>>(feats, B, D, cosine, b.dEm, b.rowsum, b.dF_head, labels, centers, b.row_sat,
+                                         c.center_weight, d_feats);
+  CTL_LAUNCH_CHECK();
+  return 0;
+}
+
+}  // extern "C"
+

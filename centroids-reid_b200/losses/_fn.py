@@ -130,6 +130,32 @@ class XentSmoothFn(torch.autograd.Function):
         return (dz * g).to(ctx.in_dtype), None, None
 
 
+def _fused_step(ctx, n_out, workspace_bytes, step, feats, centers, bn_weight, fc_weight, bn_bias, run_mean, run_var,
+                labels, is_real, cfg):
+    """Shared forward of the fused loss steps (ctl_loss_step, ctl_base_loss_step): one enqueue fills out[n_out] and the
+    gradients of out[0], which are saved for backward."""
+    N.require_cuda(feats, centers, bn_weight, fc_weight, labels, is_real)
+    f, c, bw, fw = _f32(feats), _f32(centers), _f32(bn_weight), _f32(fc_weight)
+    bb = _f32(bn_bias)
+    dev = f.device
+    out = torch.zeros(n_out, device=dev)
+    d_f, d_c, d_bw, d_fw = torch.empty_like(f), torch.empty_like(c), torch.empty_like(bw), torch.empty_like(fw)
+    ws_bytes = workspace_bytes(C.byref(cfg))
+    if ws_bytes == 0:
+        N.check(-1)
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    lab, real = _i32(labels), _u8(is_real)
+    with torch.cuda.device(dev):
+        N.check(step(C.byref(cfg), f.data_ptr(), lab.data_ptr(), real.data_ptr(), c.data_ptr(), bw.data_ptr(),
+                     bb.data_ptr(), N.ptr(run_mean), N.ptr(run_var), fw.data_ptr(), out.data_ptr(), d_f.data_ptr(),
+                     d_c.data_ptr(), d_bw.data_ptr(), d_fw.data_ptr(), ws.data_ptr(), ws_bytes, N.stream_ptr()))
+    ctx.save_for_backward(d_f, d_c, d_bw, d_fw)
+    ctx.in_dtype = feats.dtype
+    parts = out.detach()
+    ctx.mark_non_differentiable(parts)
+    return out[0], parts
+
+
 class CTLStepFn(torch.autograd.Function):
     """Everything between the trunk and manual_backward in CTLModel.training_step
     (train_ctl_model.py:54-152): returns (total, parts[8]) with gradients w.r.t.
@@ -137,31 +163,25 @@ class CTLStepFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, feats, centers, bn_weight, fc_weight, bn_bias, run_mean, run_var, labels, is_real, cfg):
-        N.require_cuda(feats, centers, bn_weight, fc_weight, labels, is_real)
-        f, c, bw, fw = _f32(feats), _f32(centers), _f32(bn_weight), _f32(fc_weight)
-        bb = _f32(bn_bias)
         L = N.lib()
-        dev = f.device
-        out = torch.zeros(8, device=dev)
-        d_f, d_c, d_bw, d_fw = torch.empty_like(f), torch.empty_like(c), torch.empty_like(bw), torch.empty_like(fw)
-        ws_bytes = L.ctl_loss_workspace_bytes(C.byref(cfg))
-        if ws_bytes == 0:
-            N.check(-1)
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-        lab, real = _i32(labels), _u8(is_real)
-        with torch.cuda.device(dev):
-            N.check(L.ctl_loss_step(C.byref(cfg), f.data_ptr(), lab.data_ptr(), real.data_ptr(), c.data_ptr(),
-                                    bw.data_ptr(), bb.data_ptr(), N.ptr(run_mean), N.ptr(run_var), fw.data_ptr(),
-                                    out.data_ptr(), d_f.data_ptr(), d_c.data_ptr(), d_bw.data_ptr(), d_fw.data_ptr(),
-                                    ws.data_ptr(), ws_bytes, N.stream_ptr()))
-        ctx.save_for_backward(d_f, d_c, d_bw, d_fw)
-        ctx.in_dtype = feats.dtype
-        parts = out.detach()
-        ctx.mark_non_differentiable(parts)
-        return out[0], parts
+        return _fused_step(ctx, 8, L.ctl_loss_workspace_bytes, L.ctl_loss_step, feats, centers, bn_weight, fc_weight,
+                           bn_bias, run_mean, run_var, labels, is_real, cfg)
 
     @staticmethod
     def backward(ctx, g_total, g_parts):
         d_f, d_c, d_bw, d_fw = ctx.saved_tensors
         return ((d_f * g_total).to(ctx.in_dtype), d_c * g_total, d_bw * g_total, d_fw * g_total,
                 None, None, None, None, None, None)
+
+
+class BaseStepFn(CTLStepFn):
+    """Everything between the trunk and manual_backward in the base model's training_step
+    (train_base_model.py:57-75): returns (total, parts[6] = total, xent, triplet, center, dist_ap, dist_an) with
+    gradients w.r.t. (features, centers, bn.weight, fc_query.weight); `cfg` is an N.BaseLossConfig.  Unlike the CTL step,
+    every row enters the center loss and the head; `is_real` only masks the triplet anchors."""
+
+    @staticmethod
+    def forward(ctx, feats, centers, bn_weight, fc_weight, bn_bias, run_mean, run_var, labels, is_real, cfg):
+        L = N.lib()
+        return _fused_step(ctx, 6, L.ctl_base_loss_workspace_bytes, L.ctl_base_loss_step, feats, centers, bn_weight,
+                           fc_weight, bn_bias, run_mean, run_var, labels, is_real, cfg)

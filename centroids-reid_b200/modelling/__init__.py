@@ -1,1 +1,1 @@
-"""Drop-ins for the reference's modelling/ package (backbones, Baseline, CTL model step)."""
+"""Drop-ins for the reference's modelling/ package (backbones, Baseline, CTL and base-model steps)."""

@@ -106,18 +106,23 @@ def ctl_losses(module, features, class_labels, is_real):
     total, parts = CTLStepFn.apply(features, module.center_loss.centers, module.bn.weight, module.fc_query.weight,
                                    module.bn.bias, module.bn.running_mean, module.bn.running_var, class_labels, is_real, cfg)
     # The kernels derive a row's class from its position (pid-major blocks of K, datasets/bases.py:346-406) and index the
-    # centers by label: a violated contract comes back as a NaN with a payload.  The sampler's layout does not change
-    # between steps, so the (synchronising) check runs on the FIRST step of a module only; CTL_VALIDATE_BATCH=1 checks
-    # every step.
+    # centers by label: a violated contract comes back as a NaN with a payload.
+    fused_step_done(module, parts, "CTL training step")
+    return total, parts
+
+
+def fused_step_done(module, parts, what):
+    """Host bookkeeping after a fused loss step wrote the head's running statistics through raw pointers.  The step
+    reports a violated batch contract as a NaN with a payload in parts[0]; the sampler's layout does not change between
+    steps, so the (synchronising) check runs on the FIRST step of a module only; CTL_VALIDATE_BATCH=1 checks every step."""
     if module.bn.num_batches_tracked is not None:
         module.bn.num_batches_tracked += 1  # nn.BatchNorm1d.forward bookkeeping (the running statistics moved)
     from ..solver.build import _bump_version
 
     _bump_version([module.bn.running_mean, module.bn.running_var])  # written by the kernel through raw pointers
     if not module.__dict__.get("_ctl_batch_checked", False) or os.environ.get("CTL_VALIDATE_BATCH") == "1":
-        raise_if_poisoned(parts[0], "CTL training step")
+        raise_if_poisoned(parts[0], what)
         module.__dict__["_ctl_batch_checked"] = True
-    return total, parts
 
 
 class CTLModel(_Base):
@@ -198,7 +203,10 @@ class CTLModel(_Base):
         else:
             total.backward()
         self.optimizer_step_manual(opt, opt_center, epoch=epoch)
-        parts = out["parts"].tolist()  # ONE read-back for everything the reference logs with float(...)
+        return self._log_step(total, out["parts"].tolist())  # ONE read-back for everything the reference logs
+
+    def _log_step(self, total, parts):
+        """train_ctl_model.py:161-179: the parts the reference logs with float(...), from the host copy of `parts`."""
         for name, val in zip(self.losses_names, (parts[1], parts[2], parts[3], parts[4])):
             self.losses_dict[name].append(val)
         return {"loss": total.detach(), "other": {"step_dist_ap": parts[5], "step_dist_an": parts[6],

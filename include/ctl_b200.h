@@ -229,6 +229,45 @@ int ctl_xent_smooth_step(const float* logits, int32_t b, int32_t c, const int32_
                          ctl_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Base-model training-step losses (the paper's baseline: no centroid rounds), forward + backward in one enqueue
+ * replaces: train_base_model.py:38-96 (everything between the trunk and manual_backward, and the gradients autograd
+ * derives from it); losses/triplet_loss.py:27-65,68-173,194-205; losses/center_loss.py:26-45.
+ * Rows: B feature rows, mock rows (is_real = 0) included; any label multiset, labels[B] in [0, C).
+ *   query triplet : batch-hard mining over all B rows (train_base_model.py:60-65), anchors masked to is_real; every
+ *                   TripletLoss variant: euclidean or cosine distance, MarginRankingLoss(margin) or SoftMarginLoss
+ *                   (soft_margin != 0, `margin` ignored);
+ *   center loss   : all B rows (:67-69), the clamp adds (C-1)*1e-12 per row;
+ *   head          : BatchNorm1d with batch statistics over all B rows (running statistics updated in place with
+ *                   n = B, unbiased var; both NULL = not tracked) -> bias-free fc -> label-smoothed CE over all B rows
+ *                   (:70-73).
+ * out_losses[6] = total (:75, center + xent + triplet), xent, triplet, center (each multiplied by its SOLVER weight),
+ * dist_ap, dist_an (means over the real anchors, :91-94).  Gradients are those of `total`: d_feats[B,D],
+ * d_centers[C,D] (dense, NOT yet rescaled by 1/center_weight -- train_base_model.py:80-81 does that in the step),
+ * d_bn_weight[D], d_fc_weight[C,D].  No host synchronisation, graph-capturable, fixed-order reductions (two calls give
+ * identical bits).  A label outside [0, C) writes a NaN with payload 1 to every out_losses entry; the centers and
+ * logits are never indexed out of range.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct ctl_base_loss_config {
+  int32_t B, D, C;
+  float margin;           /* SOLVER.MARGIN; ignored when soft_margin != 0 */
+  int32_t soft_margin;    /* SOLVER.MARGIN is None -> SoftMarginLoss */
+  int32_t cosine;         /* SOLVER.DISTANCE_FUNC == 'cosine' */
+  float center_weight;    /* SOLVER.CENTER_LOSS_WEIGHT */
+  float xent_weight;      /* SOLVER.QUERY_XENT_WEIGHT */
+  float triplet_weight;   /* SOLVER.QUERY_CONTRASTIVE_WEIGHT */
+  float bn_eps;           /* 1e-5 */
+  float bn_momentum;      /* 0.1 */
+  float label_smooth;     /* 0.1 */
+} ctl_base_loss_config;
+
+size_t ctl_base_loss_workspace_bytes(const ctl_base_loss_config* cfg);
+int ctl_base_loss_step(const ctl_base_loss_config* cfg, const float* feats, const int32_t* labels,
+                       const uint8_t* is_real, const float* centers, const float* bn_weight, const float* bn_bias,
+                       float* bn_running_mean, float* bn_running_var, const float* fc_weight, float* out_losses,
+                       float* d_feats, float* d_centers, float* d_bn_weight, float* d_fc_weight, void* workspace,
+                       size_t workspace_bytes, ctl_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Trunk inference forward (ResNet50 / ResNet50-IBN-A), NHWC fp16 activations
  * replaces: modelling/backbones/resnet.py:51-133, resnet_ibn_a.py:18-141,
  * modelling/baseline.py:91-96, modelling/bases.py:169-177, inference/inference_utils.py:104-113.
