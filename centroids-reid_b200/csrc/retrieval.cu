@@ -3,8 +3,8 @@
 // Replaces utils/reid_metric.py:25-33,51-59,112-136, utils/eval_reid.py:25-92 and
 // inference/get_similar.py:104-128 of the reference (see include/ctl_b200.h).
 //
-// Arithmetic.  The reference computes q.g in fp32.  Here every fp32 row x is split exactly as
-//     x * s = hi + 2^-11 * lo        (s: per-row power of two, hi/lo: fp16)
+// Arithmetic.  The reference computes q.g in fp32.  Here every fp32 row x is split to within 2^-23 |x s| as
+//     x * s = hi + 2^-11 * lo        (s: per-row power of two, hi/lo: fp16; exact for rows of <= 20 significant bits)
 // and q.g = (hi_q.hi_g + 2^-11 (hi_q.lo_g + lo_q.hi_g)) / (s_q s_g): three fp16 wgmma
 // passes with fp32 accumulation into TWO register accumulators (the 2^-11 terms never get swamped
 // by the leading term).  Dropped: 2^-22 lo.lo -- i.e. >= 22 significant bits per product,
@@ -112,7 +112,7 @@ __device__ __forceinline__ float warp_max(float v) {
 
 // One warp per row.  n_norm sequential L2 normalisations x <- x / max(|x|, 1e-12)
 // (F.normalize, reid_metric.py:113-115; cosine_similarity, reid_metric.py:43-46), then the
-// exact hi/lo split and the fp32 squared norm of the (normalised) row.
+// hi/lo split (DESIGN.md section 2: the bound) and the fp32 squared norm of the (normalised) row.
 __global__ void __launch_bounds__(128) planes_build_kernel(const float* __restrict__ x, int64_t n, int d, int n_norm,
                                                            __half* __restrict__ hi, __half* __restrict__ lo,
                                                            float* __restrict__ sq, float* __restrict__ inv_scale) {
@@ -156,7 +156,7 @@ __global__ void __launch_bounds__(128) planes_build_kernel(const float* __restri
     const __half h = __float2half_rn(vs);
     const float r = vs - __half2float(h);  // exact remainder
     hi[row * d + i] = h;
-    lo[row * d + i] = __float2half_rn(r * 2048.f);
+    lo[row * d + i] = __float2half_rn(r * 2048.f);  // one bit more than fp16 holds: off by <= 2^-23 |vs|
   }
   if (lane == 0) {
     sq[row] = ss;
