@@ -100,6 +100,16 @@ SIGNATURES = {
     "ctl_topk_emit": (C.c_int, [_p, _p, _i64, _i32, _i32, _p, _p, _p, _p]),
     "ctl_key_encode": (C.c_uint64, [C.c_float, C.c_uint32]),
     "ctl_key_decode": (None, [C.c_uint64, C.POINTER(C.c_float), C.POINTER(C.c_uint32)]),
+    "ctl_eval_matrix_collect": (C.c_int, [_p, _i64, _i64, _i64, _p, _p, _p, _p, _i32, _p, _p, _p, _p]),
+    "ctl_eval_matrix_count": (C.c_int, [_p, _i64, _i64, _i64, _p, _p, _p, _p, _i32, _p, _p, _p, _p]),
+    "ctl_rerank_plan": (C.c_int, [_i64, _i64, _i32, _i32] + [C.POINTER(_i32)] * 4),
+    "ctl_rerank_workspace_bytes": (_sz, [_i64, _i64, _i32, _i32]),
+    "ctl_rerank": (C.c_int, [_p, _i64, _i64, _i32, _i32, _i32, _i32, _f, _p, _i64, _p, _p, _sz, _p]),
+    "ctl_rerank_rank": (C.c_int, [_p, _i64, _i64, _i32, _p, _p, _p]),
+    "ctl_rerank_expand": (C.c_int, [_p, _i64, _i64, _p, _i32, _i32, _p, _p, _p, _p]),
+    "ctl_rerank_qe": (C.c_int, [_p, _i64, _i32, _i32, _p, _p, _p, _p, _p, _p, _p]),
+    "ctl_rerank_invert": (C.c_int, [_i64, _i64, _p, _p, _p, _i32, _p, _p, _p, _p, _p]),
+    "ctl_rerank_jaccard": (C.c_int, [_i64, _i64, _p, _p, _p, _i32, _p, _p, _p, _p, _i64, _f, _p, _i64, _p]),
     "ctl_segment_mean": (C.c_int, [_p, _i64, _i32, _p, _p, _i64, _p, _p]),
     "ctl_loss_workspace_bytes": (_sz, [_cfgp]),
     "ctl_loss_step": (C.c_int, [_cfgp] + [_p] * 14 + [_p, _sz, _p]),

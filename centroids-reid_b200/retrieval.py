@@ -795,3 +795,146 @@ def topk_and_eval_sharded(qp: Planes, gp_local: Planes, k: int, ids: EncodedIds,
     if ovf_h:
         raise OverflowError("a device-side list overflowed on some rank (exact ties at the k-th distance, or max_pos)")
     return idx, dst, _aggregate(ranks, ap_h, cnt_h, np.asarray(q_pids), total_gallery, max_rank, first=first_h)
+
+
+# ----------------------------------------------------------------------------------------
+# CMC / mAP from a materialised matrix; k-reciprocal re-ranking
+# ----------------------------------------------------------------------------------------
+
+
+def evaluate_matrix(distmat: torch.Tensor, q_pids, g_pids, q_camids, g_camids, max_rank: int = 50,
+                    respect_camids: bool = False) -> EvalResult:
+    """eval_func semantics (utils/eval_reid.py:25-92) for a [nq, ng] fp32 distance matrix already on the device (re-ranked
+    distances, or any distance the caller computed): the collect and count passes of evaluate_streamed read the matrix
+    instead of forming it (ctl_eval_matrix_collect / _count), then the same row sort, finalize and ONE packed read-back.
+    Ties are ordered by gallery index, as everywhere in this package."""
+    N.require_cuda(distmat)
+    if distmat.dim() != 2 or distmat.dtype != torch.float32 or distmat.stride(1) != 1:
+        raise ValueError("expected a [nq, ng] float32 matrix with unit column stride")
+    L = N.lib()
+    dev = distmat.device
+    nq, ng = distmat.shape
+    ld = distmat.stride(0)
+    ids = encode_ids(q_pids, g_pids, q_camids, g_camids, respect_camids, dev)
+    max_pos = ids.max_pos
+    pos_keys = torch.zeros(nq, max_pos, dtype=torch.int64, device=dev)
+    zeros = torch.zeros(nq + 1, dtype=torch.int32, device=dev)
+    pos_count, ovf = zeros[:nq], zeros[nq:]
+    buckets = torch.zeros(nq, max_pos + 1, dtype=torch.int32, device=dev)
+    idp = (ids.q_pid.data_ptr(), ids.q_cam.data_ptr(), ids.g_pid.data_ptr(), ids.g_mask.data_ptr(), max_pos)
+    with torch.cuda.device(dev):
+        s = N.stream_ptr()
+        N.check(L.ctl_eval_matrix_collect(distmat.data_ptr(), nq, ng, ld, *idp, pos_keys.data_ptr(), pos_count.data_ptr(),
+                                          ovf.data_ptr(), s))
+        N.check(L.ctl_sort_key_rows(pos_keys.data_ptr(), pos_count.data_ptr(), nq, max_pos, s))
+        N.check(L.ctl_eval_matrix_count(distmat.data_ptr(), nq, ng, ld, *idp, pos_keys.data_ptr(), pos_count.data_ptr(),
+                                        buckets.data_ptr(), s))
+        ranks, ap_h, first_h, cnt_h, ovf_h = _finalize_and_read_back(buckets, pos_count, nq, max_pos, ovf)
+    if ovf_h:
+        raise OverflowError("positives list overflowed (max_pos too small)")
+    return _aggregate(ranks, ap_h, cnt_h, np.asarray(q_pids), ng, max_rank, first=first_h)
+
+
+@dataclass
+class RerankPlan:
+    """ctl_rerank_plan: rank columns kept (kr = max(k1 + 1, k2)), h = round-half-even(k1 / 2), and the row capacities
+    of V (v_cap = (k1 + 1)(h + 2)) and of the query-expanded V (q_cap = k2 v_cap, or v_cap when k2 = 1)."""
+
+    kr: int
+    h: int
+    v_cap: int
+    q_cap: int
+
+
+def rerank_plan(nq: int, ng: int, k1: int, k2: int) -> RerankPlan:
+    import ctypes as C
+
+    v = [C.c_int32() for _ in range(4)]
+    N.check(N.lib().ctl_rerank_plan(int(nq), int(ng), int(k1), int(k2), *[C.byref(x) for x in v]))
+    return RerankPlan(*[x.value for x in v])
+
+
+def _rerank_inputs(q: torch.Tensor, g: torch.Tensor, normalize: bool):
+    N.require_cuda(q, g)
+    if q.dim() != 2 or g.dim() != 2 or q.shape[1] != g.shape[1]:
+        raise ValueError(f"expected [Q, d] and [G, d] features, got {tuple(q.shape)} and {tuple(g.shape)}")
+    return build_planes(torch.cat([q.detach().float(), g.detach().float().to(q.device)]), "euclidean", normalize)
+
+
+def _rerank_enqueue(planes: Planes, nq: int, ng: int, k1: int, k2: int, lambda_value: float, out: torch.Tensor,
+                    status: torch.Tensor, ws: torch.Tensor):
+    """ctl_rerank (enqueue only, capturable in a CUDA graph)."""
+    N.check(N.lib().ctl_rerank(planes.ptr, nq, ng, planes.d, planes.flags, int(k1), int(k2), float(lambda_value),
+                               out.data_ptr(), out.stride(0), status.data_ptr(), ws.data_ptr(), ws.numel(),
+                               N.stream_ptr()))
+
+
+def rerank(q: torch.Tensor, g: torch.Tensor, k1: int = 20, k2: int = 6, lambda_value: float = 0.3,
+           normalize: bool = False) -> torch.Tensor:
+    """k-reciprocal re-ranking (Zhong et al., CVPR 2017) of queries q [Q, d] against gallery g [G, d]: the [Q, G] float32
+    re-ranked distance matrix on the device (re_ranking(probFea, galFea, k1, k2, lambda_value) of the reid-strong-baseline
+    lineage; semantics in include/ctl_b200.h).  `normalize`: L2-normalise the features first (TEST.FEAT_NORM).
+    Differences from that function: V, the query expansion and the Jaccard sums are float32 instead of float16, and the
+    neighbour lists order equal distances by column index (np.argsort's default quicksort leaves their order
+    unspecified).  Needs N = Q + G rows of N^2 * 4 bytes of workspace (1.5 GB at Market-1501 size).  Raises ValueError
+    when a row of the distance matrix has no positive maximum (N = 1, or all features identical)."""
+    planes = _rerank_inputs(q, g, normalize)
+    nq, ng = q.shape[0], g.shape[0]
+    L = N.lib()
+    ws_bytes = L.ctl_rerank_workspace_bytes(nq, ng, int(k1), int(k2))
+    if ws_bytes == 0:
+        rerank_plan(nq, ng, k1, k2)  # raises with the reason
+    dev = q.device
+    out = torch.empty(nq, ng, dtype=torch.float32, device=dev)
+    status = torch.zeros(1, dtype=torch.int32, device=dev)
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _rerank_enqueue(planes, nq, ng, k1, k2, lambda_value, out, status, ws)
+        st = int(status.item())
+    if st:
+        raise ValueError("re-ranking: a row of the distance matrix has no positive maximum (N = 1 or identical features)")
+    return out
+
+
+def rerank_stages(q: torch.Tensor, g: torch.Tensor, k1: int = 20, k2: int = 6, lambda_value: float = 0.3,
+                  normalize: bool = False) -> dict:
+    """rerank() one stage entry point at a time, every stage reading the previous stage's device output, with every
+    intermediate kept: {nd [N, N], rank [N, kr], v_idx / v_val [N, v_cap], v_cnt, q_idx / q_val / q_cnt (the expanded
+    V; the same tensors as v_* when k2 = 1), col_ptr, inv_row, inv_val, out [Q, G], status, plan}.  For tests and
+    inspection: it holds every buffer at once."""
+    planes = _rerank_inputs(q, g, normalize)
+    nq, ng = q.shape[0], g.shape[0]
+    n = nq + ng
+    pl = rerank_plan(nq, ng, k1, k2)
+    L = N.lib()
+    dev = q.device
+    i32, f32 = dict(dtype=torch.int32, device=dev), dict(dtype=torch.float32, device=dev)
+    r = {"plan": pl, "nd": torch.empty(n, n, **f32), "rank": torch.empty(n, pl.kr, **i32),
+         "status": torch.zeros(1, **i32), "v_idx": torch.full((n, pl.v_cap), -1, **i32),
+         "v_val": torch.zeros(n, pl.v_cap, **f32), "v_cnt": torch.zeros(n, **i32)}
+    if k2 > 1:
+        r.update(q_idx=torch.full((n, pl.q_cap), -1, **i32), q_val=torch.zeros(n, pl.q_cap, **f32),
+                 q_cnt=torch.zeros(n, **i32))
+    else:
+        r.update(q_idx=r["v_idx"], q_val=r["v_val"], q_cnt=r["v_cnt"])
+    cap = r["q_idx"].shape[1]
+    r.update(col_ptr=torch.empty(n + 1, **i32), inv_row=torch.full((ng * cap,), -1, **i32),
+             inv_val=torch.zeros(ng * cap, **f32), out=torch.empty(nq, ng, **f32))
+    cursor = torch.empty(n, **i32)
+    with torch.cuda.device(dev):
+        s = N.stream_ptr()
+        N.check(L.ctl_dist_matrix(planes.ptr, n, planes.ptr, n, planes.d, planes.flags, r["nd"].data_ptr(), n, s))
+        N.check(L.ctl_rerank_rank(r["nd"].data_ptr(), n, n, pl.kr, r["rank"].data_ptr(), r["status"].data_ptr(), s))
+        N.check(L.ctl_rerank_expand(r["nd"].data_ptr(), n, n, r["rank"].data_ptr(), k1, k2, r["v_idx"].data_ptr(),
+                                    r["v_val"].data_ptr(), r["v_cnt"].data_ptr(), s))
+        if k2 > 1:
+            N.check(L.ctl_rerank_qe(r["rank"].data_ptr(), n, k1, k2, r["v_idx"].data_ptr(), r["v_val"].data_ptr(),
+                                    r["v_cnt"].data_ptr(), r["q_idx"].data_ptr(), r["q_val"].data_ptr(),
+                                    r["q_cnt"].data_ptr(), s))
+        N.check(L.ctl_rerank_invert(nq, ng, r["q_idx"].data_ptr(), r["q_val"].data_ptr(), r["q_cnt"].data_ptr(), cap,
+                                    r["col_ptr"].data_ptr(), cursor.data_ptr(), r["inv_row"].data_ptr(),
+                                    r["inv_val"].data_ptr(), s))
+        N.check(L.ctl_rerank_jaccard(nq, ng, r["q_idx"].data_ptr(), r["q_val"].data_ptr(), r["q_cnt"].data_ptr(), cap,
+                                     r["col_ptr"].data_ptr(), r["inv_row"].data_ptr(), r["inv_val"].data_ptr(),
+                                     r["nd"].data_ptr(), n, float(lambda_value), r["out"].data_ptr(), ng, s))
+    return r

@@ -82,3 +82,21 @@ def eval_streamed(q_feats, g_feats, q_pids, g_pids, q_camids, g_camids, max_rank
     gp = _R.build_planes(g, dist_func, feat_norm, order=go)
     res = _R.evaluate_streamed(qp, gp, q_pids, g_pids, q_camids, g_camids, max_rank, respect_camids)
     return res.cmc, res.mAP, res.all_topk, res.single_performance
+
+
+def eval_reranked(q_feats, g_feats, q_pids, g_pids, q_camids, g_camids, max_rank=50, respect_camids=False, k1=20, k2=6,
+                  lambda_value=0.3, feat_norm=False):
+    """eval_func's results on k-reciprocal re-ranked distances (retrieval.rerank, then retrieval.evaluate_matrix on the
+    [Q, G] matrix, both on the H100).  Same 4-tuple as eval_streamed.  Host tensors are staged to the current CUDA
+    device."""
+    import torch
+
+    q = torch.as_tensor(q_feats)
+    g = torch.as_tensor(g_feats)
+    if not q.is_cuda:
+        q = q.cuda(non_blocking=True)
+    if not g.is_cuda:
+        g = g.to(q.device, non_blocking=True)
+    dist = _R.rerank(q, g, k1, k2, lambda_value, feat_norm)
+    res = _R.evaluate_matrix(dist, q_pids, g_pids, q_camids, g_camids, max_rank, respect_camids)
+    return res.cmc, res.mAP, res.all_topk, res.single_performance

@@ -164,6 +164,65 @@ uint64_t ctl_key_encode(float dist, uint32_t index);
 void ctl_key_decode(uint64_t key, float* dist, uint32_t* index);
 
 /* ------------------------------------------------------------------------------------------
+ * CMC / mAP over a materialised distance matrix
+ * replaces: utils/eval_reid.py:25-92 (eval_func) for a [nq, ld] fp32 matrix the caller computed (re-ranked distances,
+ * or any other): np.argsort + the per-query loop.  The collect and count passes of ctl_dist_pass reading the matrix
+ * instead of forming it: same identity arrays and junk rule (see ctl_eval_collect), same (distance, column) keys, so
+ * ctl_sort_key_rows and ctl_eval_finalize_packed complete them unchanged.  pos_count and buckets are zeroed by the caller.
+ * ---------------------------------------------------------------------------------------- */
+int ctl_eval_matrix_collect(const float* dist, int64_t nq, int64_t ng, int64_t ld, const int32_t* q_pid,
+                            const int32_t* q_cam, const int32_t* g_pid, const uint64_t* g_cammask, int32_t max_pos,
+                            uint64_t* pos_keys, int32_t* pos_count, int32_t* overflow, ctl_stream_t stream);
+int ctl_eval_matrix_count(const float* dist, int64_t nq, int64_t ng, int64_t ld, const int32_t* q_pid,
+                          const int32_t* q_cam, const int32_t* g_pid, const uint64_t* g_cammask, int32_t max_pos,
+                          const uint64_t* pos_keys_sorted, const int32_t* pos_count, int32_t* buckets,
+                          ctl_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * k-reciprocal re-ranking (Zhong, Zheng, Cao, Li, CVPR 2017)
+ * replaces: re_ranking(probFea, galFea, k1, k2, lambda_value) of the reid-strong-baseline lineage credited in
+ * utils/reid_metric.py (the CTL reference dropped it): dense N x N float16 V, Python loops over the N rows, Jaccard
+ * through an inverted index.
+ * F = [q; g] (planes of nq + ng rows built with CTL_DIST_EUCLIDEAN [| CTL_FLAG_NORMALIZE]), N = nq + ng:
+ *   1. D = ctl_dist_matrix(F, F), squared euclidean, unclamped, materialised (N^2 * 4 bytes of the workspace);
+ *   2. nd[i, :] = D[i, :] / max_j D[i, j] (fp32 division); a row maximum <= 0 sets bit 0 of *status;
+ *   3. rank[i, :kr] = the first kr = max(k1 + 1, k2) columns of row i sorted by (nd, column index);
+ *   4. R(i) = {j in rank[i, :k1+1] : i in rank[j, :k1+1]}; h = round-half-even(k1 / 2); R_h(c) likewise with h + 1
+ *      neighbours; E(i) = R(i) united with every R_h(c), c in R(i), for which 3 |R_h(c) & R(i)| > 2 |R_h(c)|;
+ *      V[i, j] = exp(-nd[i, j]) / sum_{j' in E(i)} exp(-nd[i, j']) on E(i), 0 elsewhere;
+ *   5. k2 > 1: V[i] <- mean over t < k2 of V[rank[i, t]];
+ *   6. out[i, j] = (1 - lambda) (1 - s / (2 - s)) + lambda nd[i, nq + j], s = sum_c min(V[i, c], V[nq + j, c]).
+ * V and its sums are fp32; rows are padded (index, value) lists in ascending column order, capacities from
+ * ctl_rerank_plan.  No host synchronisation, no data-dependent allocation, fixed accumulation order (bit-identical
+ * repeats and graph replays).  ctl_rerank zeroes *status; the caller reads it back and rejects the result if non-zero.
+ * ctl_rerank_plan / ctl_rerank_workspace_bytes are host-only; unsupported arguments (k1 < 1, k2 < 1, N < 2, or beyond
+ * kr <= 128, (k1 + 1)(h + 2) <= 8192, k2 (k1 + 1)(h + 2) <= 16384) give CTL_ERR_* / 0 bytes. */
+int ctl_rerank_plan(int64_t nq, int64_t ng, int32_t k1, int32_t k2, int32_t* kr, int32_t* h, int32_t* v_cap,
+                    int32_t* q_cap);
+size_t ctl_rerank_workspace_bytes(int64_t nq, int64_t ng, int32_t k1, int32_t k2);
+int ctl_rerank(const void* planes, int64_t nq, int64_t ng, int32_t d, int32_t flags, int32_t k1, int32_t k2,
+               float lambda_value, float* out, int64_t ld_out, int32_t* status, void* workspace, size_t workspace_bytes,
+               ctl_stream_t stream);
+/* The stages of ctl_rerank, each on the previous stage's device output (buffers as laid out by ctl_rerank_plan):
+ *   rank   : steps 2 + 3, dist [n, ld] -> nd in place, rank [n, kr] (-1 beyond n columns); *status is OR-ed;
+ *   expand : step 4, V rows v_idx / v_val [n, v_cap], v_cnt [n];
+ *   qe     : step 5 (k2 > 1), rows [n, q_cap];
+ *   invert : CSC of the gallery rows (nq <= r < nq + ng) of a row-padded V of capacity cap: col_ptr [nq + ng + 1],
+ *            inv_row (gallery-local row) / inv_val [ng * cap]; cursor [nq + ng] is scratch.  The set of each column is
+ *            fixed, the order inside a column is not (it does not enter the Jaccard sums);
+ *   jaccard: step 6, out [nq, ld_out]. */
+int ctl_rerank_rank(float* dist, int64_t n, int64_t ld, int32_t kr, int32_t* rank, int32_t* status, ctl_stream_t stream);
+int ctl_rerank_expand(const float* nd, int64_t n, int64_t ld, const int32_t* rank, int32_t k1, int32_t k2,
+                      int32_t* v_idx, float* v_val, int32_t* v_cnt, ctl_stream_t stream);
+int ctl_rerank_qe(const int32_t* rank, int64_t n, int32_t k1, int32_t k2, const int32_t* v_idx, const float* v_val,
+                  const int32_t* v_cnt, int32_t* q_idx, float* q_val, int32_t* q_cnt, ctl_stream_t stream);
+int ctl_rerank_invert(int64_t nq, int64_t ng, const int32_t* idx, const float* val, const int32_t* cnt, int32_t cap,
+                      int32_t* col_ptr, int32_t* cursor, int32_t* inv_row, float* inv_val, ctl_stream_t stream);
+int ctl_rerank_jaccard(int64_t nq, int64_t ng, const int32_t* idx, const float* val, const int32_t* cnt, int32_t cap,
+                       const int32_t* col_ptr, const int32_t* inv_row, const float* inv_val, const float* nd,
+                       int64_t ld_nd, float lambda_value, float* out, int64_t ld_out, ctl_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Per-identity centroid mean (segmented reduction)
  * replaces: modelling/bases.py:92-95 (_calculate_centroids), the tensor part of
  * :179-262 (validation_create_centroids), inference/inference_utils.py:147-159.
