@@ -110,6 +110,15 @@ SIGNATURES = {
     "ctl_rerank_qe": (C.c_int, [_p, _i64, _i32, _i32, _p, _p, _p, _p, _p, _p, _p]),
     "ctl_rerank_invert": (C.c_int, [_i64, _i64, _p, _p, _p, _i32, _p, _p, _p, _p, _p]),
     "ctl_rerank_jaccard": (C.c_int, [_i64, _i64, _p, _p, _p, _i32, _p, _p, _p, _p, _i64, _f, _p, _i64, _p]),
+    "ctl_rerank_topk_workspace_bytes": (_sz, [_i64, _i64, _i32, _i32, _i32, _i32, _i64]),
+    "ctl_rerank_topk": (C.c_int, [_p, _i64, _i64, _i32, _i32, _i32, _i32, _f, _i32, _i64, _p, _p,
+                                  _p, _p, _p, _p, _i32, _p, _p, _p, _p, _p, _p, _sz, _p]),
+    "ctl_rerank_dist_rows": (C.c_int, [_p, _i64, _i32, _i32, _i64, _i64, _i64, _i64, _p, _p, _i64, _p]),
+    "ctl_rerank_rank_rows": (C.c_int, [_p, _i64, _i64, _i64, _i64, _i32, _p, _p, _p, _p]),
+    "ctl_rerank_expand_rows": (C.c_int, [_p, _i64, _i64, _i64, _i64, _p, _i32, _i32, _p, _p, _p, _p]),
+    "ctl_rerank_jaccard_rows": (C.c_int, [_i64, _i64, _i64, _i64, _p, _p, _p, _i32, _p, _p, _p, _p, _i64, _f, _p,
+                                          _i64, _p]),
+    "ctl_rerank_topk_rows": (C.c_int, [_p, _i64, _i64, _i64, _i64, _i32, _p, _p, _p]),
     "ctl_segment_mean": (C.c_int, [_p, _i64, _i32, _p, _p, _i64, _p, _p]),
     "ctl_loss_workspace_bytes": (_sz, [_cfgp]),
     "ctl_loss_step": (C.c_int, [_cfgp] + [_p] * 14 + [_p, _sz, _p]),

@@ -51,6 +51,11 @@ int encode_tensor_map(CUtensorMap* map, CUtensorMapDataType dtype, uint32_t elem
 
 int sm_count();
 
+// retrieval.cu: distances of rows [r0, r0 + rows) against rows [c0, c0 + cols) of one planes buffer of n rows (the
+// row-sliced planes go straight to the GEMM, nothing is copied), bit-identical to those rows of ctl_dist_matrix.
+int dist_matrix_rows(const void* planes, int64_t n, int32_t d, int32_t flags, int64_t r0, int64_t rows, int64_t c0,
+                     int64_t cols, float* out, int64_t ld_out, cudaStream_t stream);
+
 // bump allocator over a caller-provided workspace (256-byte aligned slices)
 struct Workspace {
   char* base;

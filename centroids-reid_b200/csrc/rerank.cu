@@ -14,6 +14,8 @@
 //   invert : CSC of the gallery rows of V (column -> gallery rows, values)
 //   jaccard: out[i, j] = (1 - lambda) (1 - s / (2 - s)) + lambda nd[i, Q + j], s = sum_c min(V[i, c], V[Q + j, c])
 // V rows are row-padded (index, value) lists in ascending column order, capacities fixed by (k1, k2): see plan_rerank.
+// ctl_rerank_topk runs the same kernels over [block_rows, N] row blocks of D (rank, then expand in a second sweep, then
+// Jaccard + top-k per query block), so only a block of the matrix is alive, with bit-identical results.
 #include <limits.h>
 #include <math_constants.h>
 #include <math.h>
@@ -100,8 +102,17 @@ __device__ void warp_bitonic(int* s, int n_pow2) {
 // ---------------------------------------------------------------------------------------
 // The kr-th smallest orderable key comes from a 4 x 8-bit radix select; the selected set is every key below it plus the
 // first ties in column order (a block-wide ordered scan), so exactly min(kr, n) entries, sorted as (value, column) keys.
+// One CTA per row of a [rows, ld] block (the whole matrix, or a row block of it: rank / rowmax point at the block's
+// first row).
+//   NORMALISE: row maximum (exact, so independent of the block) -> rowmax (when given), nd = D / max in place, rank;
+//   otherwise: the first kr columns of the row as it is -> out_idx (int64) / out_dist, the top-k of the final distances.
+__device__ __forceinline__ float normalise_nd(float v, float mx) { return __fadd_rn(__fdiv_rn(v, mx), 0.f); }  // no -0
+
+template <bool NORMALISE>
 __global__ void __launch_bounds__(RK_THREADS) rerank_rank_kernel(float* __restrict__ d, int n, long long ld, int kr,
-                                                                 int* __restrict__ rank, int* __restrict__ status) {
+                                                                 int* __restrict__ rank, float* __restrict__ rowmax,
+                                                                 int* __restrict__ status, long long* __restrict__ out_idx,
+                                                                 float* __restrict__ out_dist) {
   __shared__ float s_red[RK_THREADS / 32];
   __shared__ int hist[256];
   __shared__ int s_bucket, s_k, s_cnt, s_eq;
@@ -109,16 +120,18 @@ __global__ void __launch_bounds__(RK_THREADS) rerank_rank_kernel(float* __restri
   __shared__ unsigned long long s_keys[KR_MAX];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   float* r = d + (size_t)blockIdx.x * ld;
-  float mx = -CUDART_INF_F;
-  for (int j = tid; j < n; j += RK_THREADS) mx = fmaxf(mx, r[j]);
-  mx = wmax(mx);
-  if (lane == 0) s_red[warp] = mx;
-  __syncthreads();
-  mx = s_red[0];
-  for (int w = 1; w < RK_THREADS / 32; ++w) mx = fmaxf(mx, s_red[w]);
-  if (!(mx > 0.f) && tid == 0) atomicOr(status, 1);
-  for (int j = tid; j < n; j += RK_THREADS) r[j] = __fadd_rn(__fdiv_rn(r[j], mx), 0.f);  // (+ 0: no -0 keys)
-  __syncthreads();  // the row is re-read by other threads of the block
+  if (NORMALISE) {
+    float mx = -CUDART_INF_F;
+    for (int j = tid; j < n; j += RK_THREADS) mx = fmaxf(mx, r[j]);
+    mx = wmax(mx);
+    if (lane == 0) s_red[warp] = mx;
+    __syncthreads();
+    mx = s_red[0];
+    for (int w = 1; w < RK_THREADS / 32; ++w) mx = fmaxf(mx, s_red[w]);
+    if (!(mx > 0.f) && tid == 0) atomicOr(status, 1);
+    for (int j = tid; j < n; j += RK_THREADS) r[j] = normalise_nd(r[j], mx);
+    __syncthreads();  // the row is re-read by other threads of the block
+  }
 
   const int k = min(kr, n);
   uint32_t prefix = 0, mask = 0;
@@ -188,22 +201,46 @@ __global__ void __launch_bounds__(RK_THREADS) rerank_rank_kernel(float* __restri
   for (int t = k + tid; t < KR_MAX; t += RK_THREADS) s_keys[t] = ~0ull;
   __syncthreads();
   block_bitonic(s_keys, KR_MAX);
-  for (int t = tid; t < kr; t += RK_THREADS)
-    rank[(size_t)blockIdx.x * kr + t] = t < k ? (int)(uint32_t)(s_keys[t] & 0xFFFFFFFFull) : -1;
+  if (NORMALISE) {
+    for (int t = tid; t < kr; t += RK_THREADS)
+      rank[(size_t)blockIdx.x * kr + t] = t < k ? (int)(uint32_t)(s_keys[t] & 0xFFFFFFFFull) : -1;
+    if (rowmax && tid == 0) {  // the maximum again from s_red (kept out of the select's registers)
+      float mx = s_red[0];
+      for (int w = 1; w < RK_THREADS / 32; ++w) mx = fmaxf(mx, s_red[w]);
+      rowmax[blockIdx.x] = mx;
+    }
+  } else {  // kr <= n (checked by the host): every slot holds a column
+    for (int t = tid; t < kr; t += RK_THREADS) {
+      const int j = (int)(uint32_t)(s_keys[t] & 0xFFFFFFFFull);
+      out_idx[(size_t)blockIdx.x * kr + t] = j;
+      out_dist[(size_t)blockIdx.x * kr + t] = r[j];
+    }
+  }
+}
+
+// nd = D / rowmax of a [rows, cols] block whose row maxima were stored by the NORMALISE rank sweep: the same division
+// as that sweep, so the block equals the same rows (and columns) of the dense nd bit for bit
+__global__ void rerank_normalise_kernel(float* __restrict__ d, int cols, long long ld, const float* __restrict__ rowmax) {
+  float* r = d + (size_t)blockIdx.x * ld;
+  const float mx = rowmax[blockIdx.x];
+  for (int j = blockIdx.y * blockDim.x + threadIdx.x; j < cols; j += gridDim.y * blockDim.x) r[j] = normalise_nd(r[j], mx);
 }
 
 // ---------------------------------------------------------------------------------------
 // step 4: k-reciprocal sets, expansion, weights -- one warp per row
 // ---------------------------------------------------------------------------------------
 // Shared memory per warp: buf[buf_pow2] (candidates, then the sorted unique set), R[KR_MAX], T[KR_MAX].
+// Rows r0 .. r0 + rows - 1 of the n: the global row i indexes rank and V, the local row i - r0 the nd block.
 __global__ void __launch_bounds__(EX_WARPS * 32) rerank_expand_kernel(const float* __restrict__ nd, int n, long long ld,
+                                                                      int r0, int rows,
                                                                       const int* __restrict__ rank, int kr, int k1, int h,
                                                                       int* __restrict__ v_idx, float* __restrict__ v_val,
                                                                       int* __restrict__ v_cnt, int v_cap, int buf_pow2) {
   extern __shared__ int ex_smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int i = blockIdx.x * EX_WARPS + warp;
-  if (i >= n) return;  // warp-uniform; no block-wide barrier below
+  const int local = blockIdx.x * EX_WARPS + warp;
+  if (local >= rows) return;  // warp-uniform; no block-wide barrier below
+  const int i = r0 + local;
   int* buf = ex_smem + warp * (buf_pow2 + 2 * KR_MAX);
   int* R = buf + buf_pow2;
   int* T = R + KR_MAX;
@@ -273,7 +310,7 @@ __global__ void __launch_bounds__(EX_WARPS * 32) rerank_expand_kernel(const floa
     ne += __popc(b);
     __syncwarp();
   }
-  const float* ndi = nd + (size_t)i * ld;
+  const float* ndi = nd + (size_t)local * ld;
   float s = 0.f;
   for (int t = lane; t < ne; t += 32) s += expf(-ndi[buf[t]]);
   s = wsum(s);
@@ -403,8 +440,9 @@ __global__ void rerank_colfill_kernel(const int* __restrict__ idx, const float* 
 // step 6: Jaccard + blend.  CTA (query i, gallery tile y).  The query's columns are walked in ascending order; inside one
 // column every gallery row is distinct, so the shared-memory adds of one column need no atomics, and the barrier after
 // each column fixes the accumulation order of every gallery row (ascending column).
+// CTA x handles query q0 + x (its V row), and row x of nd (gallery columns from nd_col0) and of out.
 // ---------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(JC_THREADS) rerank_jaccard_kernel(int nq, int ng, const int* __restrict__ q_idx,
+__global__ void __launch_bounds__(JC_THREADS) rerank_jaccard_kernel(int q0, int nd_col0, int ng, const int* __restrict__ q_idx,
                                                                     const float* __restrict__ q_val,
                                                                     const int* __restrict__ q_cnt, int q_cap,
                                                                     const int* __restrict__ col_ptr,
@@ -416,7 +454,7 @@ __global__ void __launch_bounds__(JC_THREADS) rerank_jaccard_kernel(int nq, int 
   extern __shared__ float acc[];
   __shared__ int s_lo[JC_THREADS], s_hi[JC_THREADS];
   __shared__ float s_v[JC_THREADS];
-  const int i = blockIdx.x, tid = threadIdx.x;
+  const int i = q0 + blockIdx.x, tid = threadIdx.x;
   const int t0 = blockIdx.y * tile, tw = min(tile, ng - t0);
   for (int t = tid; t < tw; t += JC_THREADS) acc[t] = 0.f;
   const int cnt = q_cnt[i];
@@ -441,8 +479,8 @@ __global__ void __launch_bounds__(JC_THREADS) rerank_jaccard_kernel(int nq, int 
   }
   __syncthreads();
   const float a = __fsub_rn(1.f, lambda);
-  const float* ndr = nd + (size_t)i * ld_nd + nq + t0;
-  float* o = out + (size_t)i * ld_out + t0;
+  const float* ndr = nd + (size_t)blockIdx.x * ld_nd + nd_col0 + t0;
+  float* o = out + (size_t)blockIdx.x * ld_out + t0;
   for (int t = tid; t < tw; t += JC_THREADS) {
     const float s = acc[t];
     const float jac = __fsub_rn(1.f, __fdiv_rn(s, __fsub_rn(2.f, s)));
@@ -573,19 +611,39 @@ int set_smem(const void* fn, size_t bytes) {
   return 0;
 }
 
-int launch_rank(float* d, int64_t n, int64_t ld, int kr, int* rank, int* status, cudaStream_t st) {
-  rerank_rank_kernel<<<(unsigned)n, RK_THREADS, 0, st>>>(d, (int)n, ld, kr, rank, status);
+// rows of a [rows, n] block (the first of them: rank / rowmax point there); rowmax may be null
+int launch_rank(float* d, int64_t rows, int64_t n, int64_t ld, int kr, int* rank, float* rowmax, int* status,
+                cudaStream_t st) {
+  rerank_rank_kernel<true><<<(unsigned)rows, RK_THREADS, 0, st>>>(d, (int)n, ld, kr, rank, rowmax, status, nullptr,
+                                                                  nullptr);
   CTL_LAUNCH_CHECK();
   return 0;
 }
 
-int launch_expand(const float* nd, int64_t n, int64_t ld, const int* rank, int k1, const RerankPlan& pl, int* v_idx,
-                  float* v_val, int* v_cnt, cudaStream_t st) {
+// the k <= min(KR_MAX, n) smallest (value, column) of each row of a [rows, n] block, as they are
+int launch_topk(float* d, int64_t rows, int64_t n, int64_t ld, int k, long long* out_idx, float* out_dist,
+                cudaStream_t st) {
+  rerank_rank_kernel<false><<<(unsigned)rows, RK_THREADS, 0, st>>>(d, (int)n, ld, k, nullptr, nullptr, nullptr, out_idx,
+                                                                   out_dist);
+  CTL_LAUNCH_CHECK();
+  return 0;
+}
+
+int launch_normalise(float* d, int64_t rows, int64_t cols, int64_t ld, const float* rowmax, cudaStream_t st) {
+  const dim3 grid((unsigned)rows, (unsigned)std::min<int64_t>((cols + 1023) / 1024, 64));
+  rerank_normalise_kernel<<<grid, 256, 0, st>>>(d, (int)cols, ld, rowmax);
+  CTL_LAUNCH_CHECK();
+  return 0;
+}
+
+// rows [r0, r0 + rows) of the n; nd is the block of those rows
+int launch_expand(const float* nd, int64_t r0, int64_t rows, int64_t n, int64_t ld, const int* rank, int k1,
+                  const RerankPlan& pl, int* v_idx, float* v_val, int* v_cnt, cudaStream_t st) {
   const size_t smem = (size_t)EX_WARPS * (pl.buf_pow2 + 2 * KR_MAX) * sizeof(int);
   int rc = set_smem((const void*)rerank_expand_kernel, smem);
   if (rc) return rc;
-  rerank_expand_kernel<<<(unsigned)((n + EX_WARPS - 1) / EX_WARPS), EX_WARPS * 32, smem, st>>>(
-      nd, (int)n, ld, rank, pl.kr, k1, pl.h, v_idx, v_val, v_cnt, pl.v_cap, pl.buf_pow2);
+  rerank_expand_kernel<<<(unsigned)((rows + EX_WARPS - 1) / EX_WARPS), EX_WARPS * 32, smem, st>>>(
+      nd, (int)n, ld, (int)r0, (int)rows, rank, pl.kr, k1, pl.h, v_idx, v_val, v_cnt, pl.v_cap, pl.buf_pow2);
   CTL_LAUNCH_CHECK();
   return 0;
 }
@@ -615,18 +673,70 @@ int launch_invert(int64_t nq, int64_t ng, const int* idx, const float* val, cons
   return 0;
 }
 
-int launch_jaccard(int64_t nq, int64_t ng, const int* q_idx, const float* q_val, const int* q_cnt, int q_cap,
-                   const int* col_ptr, const int* inv_row, const float* inv_val, const float* nd, int64_t ld_nd,
-                   float lambda, float* out, int64_t ld_out, cudaStream_t st) {
+// queries [q0, q0 + rows): nd and out are blocks of those rows, nd's gallery columns start at nd_col0
+int launch_jaccard(int64_t q0, int64_t rows, int64_t ng, const int* q_idx, const float* q_val, const int* q_cnt,
+                   int q_cap, const int* col_ptr, const int* inv_row, const float* inv_val, const float* nd,
+                   int64_t nd_col0, int64_t ld_nd, float lambda, float* out, int64_t ld_out, cudaStream_t st) {
   const int tile = (int)std::min<int64_t>(ng, JC_TILE);
   const size_t smem = (size_t)tile * sizeof(float);
   int rc = set_smem((const void*)rerank_jaccard_kernel, (size_t)JC_TILE * sizeof(float));
   if (rc) return rc;
-  const dim3 grid((unsigned)nq, (unsigned)((ng + tile - 1) / tile));
-  rerank_jaccard_kernel<<<grid, JC_THREADS, smem, st>>>((int)nq, (int)ng, q_idx, q_val, q_cnt, q_cap, col_ptr, inv_row,
-                                                        inv_val, nd, ld_nd, lambda, out, ld_out, tile);
+  const dim3 grid((unsigned)rows, (unsigned)((ng + tile - 1) / tile));
+  rerank_jaccard_kernel<<<grid, JC_THREADS, smem, st>>>((int)q0, (int)nd_col0, (int)ng, q_idx, q_val, q_cnt, q_cap,
+                                                        col_ptr, inv_row, inv_val, nd, ld_nd, lambda, out, ld_out, tile);
   CTL_LAUNCH_CHECK();
   return 0;
+}
+
+// ---------------------------------------------------------------------------------------
+// row-blocked re-ranking (ctl_rerank_topk): the N x N matrix is never held, only a [block, N] slice of it
+// ---------------------------------------------------------------------------------------
+struct BlockedBuffers {
+  int* rank;
+  float* rowmax;
+  int *v_idx, *v_cnt;
+  float* v_val;
+  int *q_idx, *q_cnt;
+  float* q_val;
+  int *col_ptr, *cursor, *inv_row;
+  float* inv_val;
+  float* blk;  // [R, N]: sweeps A and B; [Rq, G] nd rows in sweep C
+  float* fin;  // [Rq, G] final distances of sweep C
+};
+
+int plan_blocked(int64_t nq, int64_t ng, int32_t d, int k1, int k2, int k, int64_t block_rows, RerankPlan* pl) {
+  int rc = plan_rerank(nq, ng, k1, k2, pl);
+  if (rc) return rc;
+  if (d < 8 || d % 8 || k < 1 || k > std::min<int64_t>(KR_MAX, ng) || block_rows < 1) return CTL_ERR_INVALID_ARGUMENT;
+  return 0;
+}
+
+size_t blocked_layout(int64_t nq, int64_t ng, int k2, int64_t block_rows, const RerankPlan& pl, void* base, size_t bytes,
+                      BlockedBuffers* b) {
+  const int64_t n = nq + ng;
+  const int64_t r = std::min(block_rows, n), rq = std::min(block_rows, nq);
+  Workspace ws(base, bytes);
+  b->rank = ws.take<int>((size_t)n * pl.kr);
+  b->rowmax = ws.take<float>((size_t)n);
+  b->v_idx = ws.take<int>((size_t)n * pl.v_cap);
+  b->v_val = ws.take<float>((size_t)n * pl.v_cap);
+  b->v_cnt = ws.take<int>((size_t)n);
+  if (k2 > 1) {
+    b->q_idx = ws.take<int>((size_t)n * pl.q_cap);
+    b->q_val = ws.take<float>((size_t)n * pl.q_cap);
+    b->q_cnt = ws.take<int>((size_t)n);
+  } else {
+    b->q_idx = b->v_idx;
+    b->q_val = b->v_val;
+    b->q_cnt = b->v_cnt;
+  }
+  b->col_ptr = ws.take<int>((size_t)n + 1);
+  b->cursor = ws.take<int>((size_t)n);
+  b->inv_row = ws.take<int>((size_t)ng * pl.q_cap);
+  b->inv_val = ws.take<float>((size_t)ng * pl.q_cap);
+  b->blk = ws.take<float>((size_t)r * n);
+  b->fin = ws.take<float>((size_t)rq * ng);
+  return ws.off;
 }
 
 }  // namespace
@@ -670,7 +780,7 @@ int ctl_rerank_rank(float* dist, int64_t n, int64_t ld, int32_t kr, int32_t* ran
   CTL_CHECK_ARG(kr >= 1 && kr <= KR_MAX, "kr=%d must be in [1, %d]", kr, KR_MAX);
   int rc = ctl_device_check();
   if (rc) return rc;
-  return launch_rank(dist, n, ld, kr, rank, status, (cudaStream_t)stream);
+  return launch_rank(dist, n, n, ld, kr, rank, nullptr, status, (cudaStream_t)stream);
 }
 
 int ctl_rerank_expand(const float* nd, int64_t n, int64_t ld, const int32_t* rank, int32_t k1, int32_t k2,
@@ -681,7 +791,7 @@ int ctl_rerank_expand(const float* nd, int64_t n, int64_t ld, const int32_t* ran
   CTL_CHECK_ARG(plan_rerank(1, n - 1, k1, k2, &pl) == 0, "unsupported k1=%d k2=%d", k1, k2);
   int rc = ctl_device_check();
   if (rc) return rc;
-  return launch_expand(nd, n, ld, rank, k1, pl, v_idx, v_val, v_cnt, (cudaStream_t)stream);
+  return launch_expand(nd, 0, n, n, ld, rank, k1, pl, v_idx, v_val, v_cnt, (cudaStream_t)stream);
 }
 
 int ctl_rerank_qe(const int32_t* rank, int64_t n, int32_t k1, int32_t k2, const int32_t* v_idx, const float* v_val,
@@ -712,8 +822,8 @@ int ctl_rerank_jaccard(int64_t nq, int64_t ng, const int32_t* idx, const float* 
   CTL_CHECK_ARG(nq >= 1 && ng >= 1 && nq + ng < (1ll << 31) && ld_nd >= nq + ng && ld_out >= ng && cap >= 1, "bad shape");
   int rc = ctl_device_check();
   if (rc) return rc;
-  return launch_jaccard(nq, ng, idx, val, cnt, cap, col_ptr, inv_row, inv_val, nd, ld_nd, lambda_value, out, ld_out,
-                        (cudaStream_t)stream);
+  return launch_jaccard(0, nq, ng, idx, val, cnt, cap, col_ptr, inv_row, inv_val, nd, nq, ld_nd, lambda_value, out,
+                        ld_out, (cudaStream_t)stream);
 }
 
 int ctl_rerank(const void* planes, int64_t nq, int64_t ng, int32_t d, int32_t flags, int32_t k1, int32_t k2,
@@ -738,14 +848,14 @@ int ctl_rerank(const void* planes, int64_t nq, int64_t ng, int32_t d, int32_t fl
   const int64_t n = nq + ng;
   CTL_CUDA(cudaMemsetAsync(status, 0, sizeof(int32_t), st));
   if ((rc = ctl_dist_matrix(planes, n, planes, n, d, flags, bf.nd, n, stream_))) return rc;
-  if ((rc = launch_rank(bf.nd, n, n, pl.kr, bf.rank, status, st))) return rc;
-  if ((rc = launch_expand(bf.nd, n, n, bf.rank, k1, pl, bf.v_idx, bf.v_val, bf.v_cnt, st))) return rc;
+  if ((rc = launch_rank(bf.nd, n, n, n, pl.kr, bf.rank, nullptr, status, st))) return rc;
+  if ((rc = launch_expand(bf.nd, 0, n, n, n, bf.rank, k1, pl, bf.v_idx, bf.v_val, bf.v_cnt, st))) return rc;
   if (k2 > 1 && (rc = launch_qe(bf.rank, n, k2, pl, bf.v_idx, bf.v_val, bf.v_cnt, bf.q_idx, bf.q_val, bf.q_cnt, st)))
     return rc;
   const int cap = k2 > 1 ? pl.q_cap : pl.v_cap;
   if ((rc = launch_invert(nq, ng, bf.q_idx, bf.q_val, bf.q_cnt, cap, bf.col_ptr, bf.cursor, bf.inv_row, bf.inv_val, st)))
     return rc;
-  return launch_jaccard(nq, ng, bf.q_idx, bf.q_val, bf.q_cnt, cap, bf.col_ptr, bf.inv_row, bf.inv_val, bf.nd, n,
+  return launch_jaccard(0, nq, ng, bf.q_idx, bf.q_val, bf.q_cnt, cap, bf.col_ptr, bf.inv_row, bf.inv_val, bf.nd, nq, n,
                         lambda_value, out, ld_out, st);
 }
 
@@ -783,6 +893,158 @@ int ctl_eval_matrix_count(const float* dist, int64_t nq, int64_t ng, int64_t ld,
       dist, (int)ng, ld, q_pid, q_cam, g_pid, reinterpret_cast<const unsigned long long*>(g_cammask), max_pos,
       reinterpret_cast<const unsigned long long*>(pos_keys_sorted), pos_count, buckets);
   CTL_LAUNCH_CHECK();
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------
+// row-blocked re-ranking: stage entry points over row blocks, and the one-call ctl_rerank_topk
+// ---------------------------------------------------------------------------------------
+size_t ctl_rerank_topk_workspace_bytes(int64_t nq, int64_t ng, int32_t d, int32_t k1, int32_t k2, int32_t k,
+                                       int64_t block_rows) {
+  RerankPlan pl;
+  if (plan_blocked(nq, ng, d, k1, k2, k, block_rows, &pl)) return 0;
+  BlockedBuffers b;
+  return blocked_layout(nq, ng, k2, block_rows, pl, nullptr, 0, &b);
+}
+
+int ctl_rerank_dist_rows(const void* planes, int64_t n, int32_t d, int32_t flags, int64_t r0, int64_t rows, int64_t c0,
+                         int64_t cols, const float* rowmax, float* out, int64_t ld_out, ctl_stream_t stream) {
+  CTL_CHECK_ARG(!(flags & (CTL_DIST_COSINE | CTL_DIST_SQRT)), "re-ranking starts from squared euclidean distances");
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc = dist_matrix_rows(planes, n, d, flags, r0, rows, c0, cols, out, ld_out, st);
+  if (rc || !rowmax) return rc;
+  return launch_normalise(out, rows, cols, ld_out, rowmax + r0, st);
+}
+
+int ctl_rerank_rank_rows(float* dist, int64_t r0, int64_t rows, int64_t n, int64_t ld, int32_t kr, int32_t* rank,
+                         float* rowmax, int32_t* status, ctl_stream_t stream) {
+  CTL_CHECK_ARG(dist && rank && rowmax && status, "null pointer");
+  CTL_CHECK_ARG(n >= 2 && n < (1ll << 31) && r0 >= 0 && rows >= 1 && r0 + rows <= n && ld >= n,
+                "bad row block r0=%lld rows=%lld n=%lld ld=%lld", (long long)r0, (long long)rows, (long long)n,
+                (long long)ld);
+  CTL_CHECK_ARG(kr >= 1 && kr <= KR_MAX, "kr=%d must be in [1, %d]", kr, KR_MAX);
+  int rc = ctl_device_check();
+  if (rc) return rc;
+  return launch_rank(dist, rows, n, ld, kr, rank + r0 * kr, rowmax + r0, status, (cudaStream_t)stream);
+}
+
+int ctl_rerank_expand_rows(const float* nd, int64_t r0, int64_t rows, int64_t n, int64_t ld, const int32_t* rank,
+                           int32_t k1, int32_t k2, int32_t* v_idx, float* v_val, int32_t* v_cnt, ctl_stream_t stream) {
+  CTL_CHECK_ARG(nd && rank && v_idx && v_val && v_cnt, "null pointer");
+  CTL_CHECK_ARG(n >= 2 && n < (1ll << 31) && r0 >= 0 && rows >= 1 && r0 + rows <= n && ld >= n,
+                "bad row block r0=%lld rows=%lld n=%lld ld=%lld", (long long)r0, (long long)rows, (long long)n,
+                (long long)ld);
+  RerankPlan pl;
+  CTL_CHECK_ARG(plan_rerank(1, n - 1, k1, k2, &pl) == 0, "unsupported k1=%d k2=%d", k1, k2);
+  int rc = ctl_device_check();
+  if (rc) return rc;
+  return launch_expand(nd, r0, rows, n, ld, rank, k1, pl, v_idx, v_val, v_cnt, (cudaStream_t)stream);
+}
+
+int ctl_rerank_jaccard_rows(int64_t nq, int64_t ng, int64_t q0, int64_t rows, const int32_t* idx, const float* val,
+                            const int32_t* cnt, int32_t cap, const int32_t* col_ptr, const int32_t* inv_row,
+                            const float* inv_val, const float* nd, int64_t ld_nd, float lambda_value, float* out,
+                            int64_t ld_out, ctl_stream_t stream) {
+  CTL_CHECK_ARG(idx && val && cnt && col_ptr && inv_row && inv_val && nd && out, "null pointer");
+  CTL_CHECK_ARG(nq >= 1 && ng >= 1 && nq + ng < (1ll << 31) && q0 >= 0 && rows >= 1 && q0 + rows <= nq && ld_nd >= ng &&
+                    ld_out >= ng && cap >= 1,
+                "bad shape");
+  int rc = ctl_device_check();
+  if (rc) return rc;
+  return launch_jaccard(q0, rows, ng, idx, val, cnt, cap, col_ptr, inv_row, inv_val, nd, 0, ld_nd, lambda_value, out,
+                        ld_out, (cudaStream_t)stream);
+}
+
+int ctl_rerank_topk_rows(float* dist, int64_t r0, int64_t rows, int64_t n, int64_t ld, int32_t k, int64_t* out_idx,
+                         float* out_dist, ctl_stream_t stream) {
+  CTL_CHECK_ARG(dist && out_idx && out_dist, "null pointer");
+  CTL_CHECK_ARG(n >= 1 && n < (1ll << 31) && r0 >= 0 && rows >= 1 && ld >= n, "bad shape r0=%lld rows=%lld n=%lld",
+                (long long)r0, (long long)rows, (long long)n);
+  CTL_CHECK_ARG(k >= 1 && k <= KR_MAX && k <= n, "k=%d must be in [1, min(%d, n=%lld)]", k, KR_MAX, (long long)n);
+  int rc = ctl_device_check();
+  if (rc) return rc;
+  return launch_topk(dist, rows, n, ld, k, reinterpret_cast<long long*>(out_idx) + r0 * k, out_dist + r0 * k,
+                     (cudaStream_t)stream);
+}
+
+int ctl_rerank_topk(const void* planes, int64_t nq, int64_t ng, int32_t d, int32_t flags, int32_t k1, int32_t k2,
+                    float lambda_value, int32_t k, int64_t block_rows, int64_t* out_idx, float* out_dist,
+                    const int32_t* q_pid, const int32_t* q_cam, const int32_t* g_pid, const uint64_t* g_cammask,
+                    int32_t max_pos, uint64_t* pos_keys, int32_t* pos_count, int32_t* buckets, int32_t* overflow,
+                    int32_t* status, void* workspace, size_t workspace_bytes, ctl_stream_t stream_) {
+  cudaStream_t st = (cudaStream_t)stream_;
+  CTL_CHECK_ARG(planes && out_idx && out_dist && status && workspace, "null pointer");
+  CTL_CHECK_ARG(!(flags & (CTL_DIST_COSINE | CTL_DIST_SQRT)), "re-ranking starts from squared euclidean distances");
+  const bool eval = q_pid != nullptr;
+  CTL_CHECK_ARG(!eval || (q_cam && g_pid && g_cammask && pos_keys && pos_count && buckets && overflow && max_pos >= 1),
+                "evaluation needs every identity array and output (max_pos >= 1)");
+  RerankPlan pl;
+  int rc = plan_blocked(nq, ng, d, k1, k2, k, block_rows, &pl);
+  if (rc == CTL_ERR_INVALID_ARGUMENT && plan_rerank(nq, ng, k1, k2, &pl) == 0) {
+    set_error("blocked re-ranking needs d a positive multiple of 8, 1 <= k <= min(%d, ng) and block_rows >= 1 "
+              "(d=%d k=%d ng=%lld block_rows=%lld)", KR_MAX, d, k, (long long)ng, (long long)block_rows);
+    return rc;
+  }
+  if (rc) {
+    int32_t a, b, c, e;
+    return ctl_rerank_plan(nq, ng, k1, k2, &a, &b, &c, &e);  // the same status, with its message
+  }
+  BlockedBuffers bf;
+  const size_t need = blocked_layout(nq, ng, k2, block_rows, pl, workspace, workspace_bytes, &bf);
+  if (need > workspace_bytes) {
+    set_error("workspace too small: need %zu bytes, have %zu", need, workspace_bytes);
+    return CTL_ERR_WORKSPACE;
+  }
+  if ((rc = ctl_device_check())) return rc;
+  const int64_t n = nq + ng, R = std::min<int64_t>(block_rows, n);
+  CTL_CUDA(cudaMemsetAsync(status, 0, sizeof(int32_t), st));
+  if (eval) {
+    CTL_CUDA(cudaMemsetAsync(pos_count, 0, (size_t)nq * sizeof(int32_t), st));
+    CTL_CUDA(cudaMemsetAsync(buckets, 0, (size_t)nq * (max_pos + 1) * sizeof(int32_t), st));
+    CTL_CUDA(cudaMemsetAsync(overflow, 0, sizeof(int32_t), st));
+  }
+  // sweep A: the row maxima and the rank table, one [R, N] block at a time
+  for (int64_t r0 = 0; r0 < n; r0 += R) {
+    const int64_t rows = std::min(R, n - r0);
+    if ((rc = dist_matrix_rows(planes, n, d, flags, r0, rows, 0, n, bf.blk, n, st))) return rc;
+    if ((rc = launch_rank(bf.blk, rows, n, n, pl.kr, bf.rank + r0 * pl.kr, bf.rowmax + r0, status, st))) return rc;
+  }
+  // sweep B: the same blocks again, normalised by the stored maxima; the expansion reads the rank table of all rows
+  for (int64_t r0 = 0; r0 < n; r0 += R) {
+    const int64_t rows = std::min(R, n - r0);
+    if ((rc = dist_matrix_rows(planes, n, d, flags, r0, rows, 0, n, bf.blk, n, st))) return rc;
+    if ((rc = launch_normalise(bf.blk, rows, n, n, bf.rowmax + r0, st))) return rc;
+    if ((rc = launch_expand(bf.blk, r0, rows, n, n, bf.rank, k1, pl, bf.v_idx, bf.v_val, bf.v_cnt, st))) return rc;
+  }
+  if (k2 > 1 && (rc = launch_qe(bf.rank, n, k2, pl, bf.v_idx, bf.v_val, bf.v_cnt, bf.q_idx, bf.q_val, bf.q_cnt, st)))
+    return rc;
+  const int cap = k2 > 1 ? pl.q_cap : pl.v_cap;
+  if ((rc = launch_invert(nq, ng, bf.q_idx, bf.q_val, bf.q_cnt, cap, bf.col_ptr, bf.cursor, bf.inv_row, bf.inv_val, st)))
+    return rc;
+  // sweep C: query blocks against the gallery only -> final distances -> top-k (and the evaluation passes)
+  const int64_t Rq = std::min<int64_t>(block_rows, nq);
+  const unsigned long long* gm = reinterpret_cast<const unsigned long long*>(g_cammask);
+  for (int64_t q0 = 0; q0 < nq; q0 += Rq) {
+    const int64_t rows = std::min(Rq, nq - q0);
+    if ((rc = dist_matrix_rows(planes, n, d, flags, q0, rows, nq, ng, bf.blk, ng, st))) return rc;
+    if ((rc = launch_normalise(bf.blk, rows, ng, ng, bf.rowmax + q0, st))) return rc;
+    if ((rc = launch_jaccard(q0, rows, ng, bf.q_idx, bf.q_val, bf.q_cnt, cap, bf.col_ptr, bf.inv_row, bf.inv_val, bf.blk,
+                             0, ng, lambda_value, bf.fin, ng, st)))
+      return rc;
+    if ((rc = launch_topk(bf.fin, rows, ng, ng, k, reinterpret_cast<long long*>(out_idx) + q0 * k, out_dist + q0 * k, st)))
+      return rc;
+    if (!eval) continue;
+    unsigned long long* pk = reinterpret_cast<unsigned long long*>(pos_keys) + q0 * max_pos;
+    eval_matrix_collect_kernel<<<(unsigned)rows, EM_THREADS, 0, st>>>(bf.fin, (int)ng, ng, q_pid + q0, q_cam + q0, g_pid,
+                                                                      gm, max_pos, pk, pos_count + q0, overflow);
+    CTL_LAUNCH_CHECK();
+    if ((rc = ctl_sort_key_rows(reinterpret_cast<uint64_t*>(pk), pos_count + q0, rows, max_pos, stream_))) return rc;
+    const size_t smem = max_pos + 1 <= EM_HIST_MAX ? (size_t)(max_pos + 1) * sizeof(int) : 0;
+    eval_matrix_count_kernel<<<(unsigned)rows, EM_THREADS, smem, st>>>(bf.fin, (int)ng, ng, q_pid + q0, q_cam + q0, g_pid,
+                                                                       gm, max_pos, pk, pos_count + q0,
+                                                                       buckets + q0 * (max_pos + 1));
+    CTL_LAUNCH_CHECK();
+  }
   return 0;
 }
 

@@ -833,6 +833,20 @@ static int make_plane_maps(GemmMaps* m, const PlanesView& q, int64_t nq, const P
   return 0;
 }
 
+// rows [r0, ...) of a planes view: every plane is row-major, so the slice is a pointer offset (r0 d halves stay 16-byte
+// aligned for TMA because d % 8 == 0)
+static PlanesView planes_rows(const PlanesView& v, int64_t r0, int32_t d) {
+  PlanesView s;
+  s.hi = v.hi + (size_t)r0 * d;
+  s.lo = v.lo + (size_t)r0 * d;
+  s.sq = v.sq + r0;
+  s.inv_scale = v.inv_scale + r0;
+  return s;
+}
+
+static int launch_gemm_views(const PlanesView& q, int64_t nq, const PlanesView& g, int64_t ng, int32_t d, int32_t flags,
+                             GemmPass p, cudaStream_t stream);
+
 static int launch_gemm_pass(const void* q_planes, int64_t nq, const void* g_planes, int64_t ng, int32_t d, int32_t flags,
                             GemmPass p, cudaStream_t stream) {
   CTL_CHECK_ARG(q_planes && g_planes, "null planes");
@@ -840,7 +854,31 @@ static int launch_gemm_pass(const void* q_planes, int64_t nq, const void* g_plan
   CTL_CHECK_ARG(d > 0 && d % 8 == 0, "feature dim %d must be a positive multiple of 8", d);
   int rc = ctl_device_check();
   if (rc) return rc;
-  const PlanesView q = planes_view(q_planes, nq, d), g = planes_view(g_planes, ng, d);
+  return launch_gemm_views(planes_view(q_planes, nq, d), nq, planes_view(g_planes, ng, d), ng, d, flags, p, stream);
+}
+
+// Distances of rows [r0, r0 + rows) against rows [c0, c0 + cols) of ONE planes buffer of n rows, into out [rows, ld_out].
+// The GEMM runs the same plan and k-order for every shape, so an element depends only on its two rows: a row block is
+// bit-identical to the same rows of the full matrix (tests/test_rerank_blocked_gpu.py asserts it).
+int dist_matrix_rows(const void* planes, int64_t n, int32_t d, int32_t flags, int64_t r0, int64_t rows, int64_t c0,
+                     int64_t cols, float* out, int64_t ld_out, cudaStream_t stream) {
+  CTL_CHECK_ARG(planes && out, "null pointer");
+  CTL_CHECK_ARG(n > 0 && n < (1ll << 31) && d > 0 && d % 8 == 0, "bad planes n=%lld d=%d", (long long)n, d);
+  CTL_CHECK_ARG(r0 >= 0 && rows > 0 && r0 + rows <= n && c0 >= 0 && cols > 0 && c0 + cols <= n && ld_out >= cols,
+                "bad row block r0=%lld rows=%lld c0=%lld cols=%lld n=%lld ld=%lld", (long long)r0, (long long)rows,
+                (long long)c0, (long long)cols, (long long)n, (long long)ld_out);
+  int rc = ctl_device_check();
+  if (rc) return rc;
+  const PlanesView all = planes_view(planes, n, d);
+  GemmPass p = {};
+  p.dist_out = out;
+  p.ld_out = ld_out;
+  return launch_gemm_views(planes_rows(all, r0, d), rows, planes_rows(all, c0, d), cols, d, flags, p, stream);
+}
+
+static int launch_gemm_views(const PlanesView& q, int64_t nq, const PlanesView& g, int64_t ng, int32_t d, int32_t flags,
+                             GemmPass p, cudaStream_t stream) {
+  int rc;
   GemmMaps maps;
   if ((rc = make_plane_maps(&maps, q, nq, g, ng, d))) return rc;
   p.nq = (int)nq;

@@ -938,3 +938,235 @@ def rerank_stages(q: torch.Tensor, g: torch.Tensor, k1: int = 20, k2: int = 6, l
                                      r["col_ptr"].data_ptr(), r["inv_row"].data_ptr(), r["inv_val"].data_ptr(),
                                      r["nd"].data_ptr(), n, float(lambda_value), r["out"].data_ptr(), ng, s))
     return r
+
+
+# ----------------------------------------------------------------------------------------
+# row-blocked re-ranking: galleries beyond the N^2 bound
+# ----------------------------------------------------------------------------------------
+
+RERANK_BLOCK_BYTES = 2 << 30  # default size of the [block_rows, N] fp32 slice of the distance matrix
+
+
+def rerank_block_rows(nq: int, ng: int, budget: int = RERANK_BLOCK_BYTES) -> int:
+    """The default block of rerank_topk: the largest multiple of 128 rows whose [R, N] fp32 block fits in `budget`
+    bytes (fewer rows, at least 1, when not even 128 fit), and never more than N = nq + ng."""
+    n = int(nq) + int(ng)
+    rows = int(budget) // (4 * n)
+    r = rows // 128 * 128 if rows >= 128 else max(1, rows)
+    return int(min(r, n))
+
+
+def rerank_fits_dense(nq: int, ng: int, k1: int, k2: int, free_bytes: int) -> bool:
+    """Which re-ranking eval_reranked runs: the dense ctl_rerank (plus its [Q, G] result) when its workspace and output
+    fit in `free_bytes` of device memory, otherwise the row-blocked ctl_rerank_topk (bit-identical results, workspace
+    linear in N).  Host-only."""
+    ws = N.lib().ctl_rerank_workspace_bytes(int(nq), int(ng), int(k1), int(k2))
+    return ws > 0 and ws + 4 * int(nq) * int(ng) <= int(free_bytes)
+
+
+def rerank_topk_workspace_bytes(nq: int, ng: int, d: int, k1: int, k2: int, k: int, block_rows: int) -> int:
+    """ctl_rerank_topk_workspace_bytes (host-only; 0 for unsupported arguments)."""
+    return int(N.lib().ctl_rerank_topk_workspace_bytes(int(nq), int(ng), int(d), int(k1), int(k2), int(k),
+                                                        int(block_rows)))
+
+
+def _rerank_topk_args(nq, ng, d, k1, k2, k, block_rows):
+    """validated (k, block_rows, workspace bytes); raises with the library's reason."""
+    block_rows = rerank_block_rows(nq, ng) if block_rows is None else int(block_rows)
+    ws_bytes = rerank_topk_workspace_bytes(nq, ng, d, k1, k2, k, block_rows)
+    if ws_bytes == 0:
+        rerank_plan(nq, ng, k1, k2)  # raises for what the dense plan rejects
+        raise ValueError(f"blocked re-ranking needs 1 <= k <= min(128, ng) and block_rows >= 1 (k={k}, ng={ng}, "
+                         f"block_rows={block_rows}) and d a positive multiple of 8 (d={d})")
+    return int(k), block_rows, ws_bytes
+
+
+def _rerank_topk_enqueue(planes: Planes, nq: int, ng: int, k1: int, k2: int, lambda_value: float, k: int,
+                         block_rows: int, idx: torch.Tensor, dst: torch.Tensor, ev: Optional[dict], status: torch.Tensor,
+                         ws: torch.Tensor):
+    """ctl_rerank_topk (enqueue only, capturable in a CUDA graph).  `ev`: {ids, pos_keys, pos_count, buckets, ovf} or
+    None."""
+    if ev is None:
+        e = [0, 0, 0, 0, 1, 0, 0, 0, 0]
+    else:
+        ids = ev["ids"]
+        e = [ids.q_pid.data_ptr(), ids.q_cam.data_ptr(), ids.g_pid.data_ptr(), ids.g_mask.data_ptr(), ids.max_pos,
+             ev["pos_keys"].data_ptr(), ev["pos_count"].data_ptr(), ev["buckets"].data_ptr(), ev["ovf"].data_ptr()]
+    N.check(N.lib().ctl_rerank_topk(planes.ptr, nq, ng, planes.d, planes.flags, int(k1), int(k2), float(lambda_value),
+                                    int(k), int(block_rows), idx.data_ptr(), dst.data_ptr(), *e, status.data_ptr(),
+                                    ws.data_ptr(), ws.numel(), N.stream_ptr()))
+
+
+def _eval_buffers(ids: "EncodedIds", nq: int, dev) -> dict:
+    return {"ids": ids, "pos_keys": torch.zeros(nq, ids.max_pos, dtype=torch.int64, device=dev),
+            "pos_count": torch.zeros(nq, dtype=torch.int32, device=dev),
+            "buckets": torch.zeros(nq, ids.max_pos + 1, dtype=torch.int32, device=dev),
+            "ovf": torch.zeros(1, dtype=torch.int32, device=dev)}
+
+
+def _rerank_topk_run(q, g, k, k1, k2, lambda_value, normalize, block_rows, ids_args=None, max_rank=50):
+    """ctl_rerank_topk from features; ids_args = (q_pids, g_pids, q_camids, g_camids, respect_camids) adds the
+    evaluation."""
+    planes = _rerank_inputs(q, g, normalize)
+    nq, ng = q.shape[0], g.shape[0]
+    k, block_rows, ws_bytes = _rerank_topk_args(nq, ng, planes.d, k1, k2, k, block_rows)
+    dev = q.device
+    idx = torch.empty(nq, k, dtype=torch.int64, device=dev)
+    dst = torch.empty(nq, k, dtype=torch.float32, device=dev)
+    status = torch.zeros(1, dtype=torch.int32, device=dev)
+    ev = None
+    if ids_args is not None:
+        ev = _eval_buffers(encode_ids(*ids_args, dev), nq, dev)
+    with torch.cuda.device(dev):
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+        _rerank_topk_enqueue(planes, nq, ng, k1, k2, lambda_value, k, block_rows, idx, dst, ev, status, ws)
+        del ws
+        if ev is not None:
+            ranks, pack = _finalize(ev["buckets"], ev["pos_count"], nq, ev["ids"].max_pos, ev["ovf"])
+        st = int(status.item())
+    if st:
+        raise ValueError("re-ranking: a row of the distance matrix has no positive maximum (N = 1 or identical features)")
+    if ev is None:
+        return idx, dst, None
+    ap_h, first_h, cnt_h, ovf_h = _unpack(pack.cpu().numpy(), nq)
+    if ovf_h:
+        raise OverflowError("positives list overflowed (max_pos too small)")
+    return idx, dst, _aggregate(ranks, ap_h, cnt_h, np.asarray(ids_args[0]), ng, max_rank, first=first_h)
+
+
+def rerank_topk(q: torch.Tensor, g: torch.Tensor, k: int, k1: int = 20, k2: int = 6, lambda_value: float = 0.3,
+                normalize: bool = False, block_rows: Optional[int] = None):
+    """Each query's k <= 128 nearest gallery rows under k-reciprocal re-ranking, without the N x N or the [Q, G] matrix:
+    (idx [Q, k] int64, dist [Q, k] float32) on the device, ascending (distance, gallery index) -- the first k columns of
+    the stable sort of rerank()'s output, bit for bit, for any block_rows.  Three sweeps over [block_rows, N] blocks of
+    the distance matrix (ctl_rerank_topk); memory grows linearly in N = Q + G.  block_rows defaults to
+    rerank_block_rows (a 2 GiB block)."""
+    idx, dst, _ = _rerank_topk_run(q, g, k, k1, k2, lambda_value, normalize, block_rows)
+    return idx, dst
+
+
+def rerank_topk_and_eval(q: torch.Tensor, g: torch.Tensor, k: int, q_pids, g_pids, q_camids, g_camids, k1: int = 20,
+                         k2: int = 6, lambda_value: float = 0.3, normalize: bool = False, max_rank: int = 50,
+                         respect_camids: bool = False, block_rows: Optional[int] = None):
+    """rerank_topk plus eval_func's CMC / mAP of the re-ranked distances, computed block by block from the final
+    distances of sweep C: (idx, dist, EvalResult) as topk_and_eval.  The EvalResult equals
+    evaluate_matrix(rerank(...)) bit for bit."""
+    ids_args = (q_pids, g_pids, q_camids, g_camids, respect_camids)
+    return _rerank_topk_run(q, g, k, k1, k2, lambda_value, normalize, block_rows, ids_args, max_rank)
+
+
+def rerank_blocked_stages(q: torch.Tensor, g: torch.Tensor, k: int, k1: int = 20, k2: int = 6,
+                          lambda_value: float = 0.3, normalize: bool = False, block_rows: Optional[int] = None,
+                          q_pids=None, g_pids=None, q_camids=None, g_camids=None, max_rank: int = 50,
+                          respect_camids: bool = False, events: Optional[list] = None) -> dict:
+    """rerank_topk one row-block stage entry point at a time (ctl_rerank_dist_rows / _rank_rows / _expand_rows, qe,
+    invert, _jaccard_rows / _topk_rows), keeping every intermediate that is linear in N: {rank [N, kr], rowmax [N],
+    v_idx / v_val / v_cnt, q_idx / q_val / q_cnt, col_ptr, inv_row, inv_val, idx / dist [Q, k], status, plan, planes,
+    block_rows}, plus `eval` (the EvalResult) when identities are given.  For tests and inspection: `events`, a list,
+    receives (name, CUDA event) pairs recorded after each sweep ("A", "B", "qe_invert", "C")."""
+    planes = _rerank_inputs(q, g, normalize)
+    nq, ng = q.shape[0], g.shape[0]
+    n = nq + ng
+    k, R, _ = _rerank_topk_args(nq, ng, planes.d, k1, k2, k, block_rows)
+    pl = rerank_plan(nq, ng, k1, k2)
+    L = N.lib()
+    dev = q.device
+    i32, f32 = dict(dtype=torch.int32, device=dev), dict(dtype=torch.float32, device=dev)
+    r = {"plan": pl, "planes": planes, "block_rows": R, "lambda": float(lambda_value), "rank": torch.empty(n, pl.kr, **i32),
+         "rowmax": torch.empty(n, **f32), "status": torch.zeros(1, **i32), "v_idx": torch.full((n, pl.v_cap), -1, **i32),
+         "v_val": torch.zeros(n, pl.v_cap, **f32), "v_cnt": torch.zeros(n, **i32),
+         "idx": torch.empty(nq, k, dtype=torch.int64, device=dev), "dist": torch.empty(nq, k, **f32)}
+    if k2 > 1:
+        r.update(q_idx=torch.full((n, pl.q_cap), -1, **i32), q_val=torch.zeros(n, pl.q_cap, **f32),
+                 q_cnt=torch.zeros(n, **i32))
+    else:
+        r.update(q_idx=r["v_idx"], q_val=r["v_val"], q_cnt=r["v_cnt"])
+    cap = r["q_idx"].shape[1]
+    r.update(col_ptr=torch.empty(n + 1, **i32), inv_row=torch.full((ng * cap,), -1, **i32),
+             inv_val=torch.zeros(ng * cap, **f32))
+    ev = None
+    if q_pids is not None:
+        ev = _eval_buffers(encode_ids(q_pids, g_pids, q_camids, g_camids, respect_camids, dev), nq, dev)
+    cursor = torch.empty(n, **i32)
+    blk = torch.empty(min(R, n) * n, **f32)
+
+    def mark(name):
+        if events is not None:
+            e = torch.cuda.Event(enable_timing=True)
+            e.record()
+            events.append((name, e))
+
+    with torch.cuda.device(dev):
+        s = N.stream_ptr()
+        mark("start")
+        for r0 in range(0, n, R):  # sweep A
+            rows = min(R, n - r0)
+            N.check(L.ctl_rerank_dist_rows(planes.ptr, n, planes.d, planes.flags, r0, rows, 0, n, None,
+                                           blk.data_ptr(), n, s))
+            N.check(L.ctl_rerank_rank_rows(blk.data_ptr(), r0, rows, n, n, pl.kr, r["rank"].data_ptr(),
+                                           r["rowmax"].data_ptr(), r["status"].data_ptr(), s))
+        mark("A")
+        for r0 in range(0, n, R):  # sweep B
+            rows = min(R, n - r0)
+            N.check(L.ctl_rerank_dist_rows(planes.ptr, n, planes.d, planes.flags, r0, rows, 0, n,
+                                           r["rowmax"].data_ptr(), blk.data_ptr(), n, s))
+            N.check(L.ctl_rerank_expand_rows(blk.data_ptr(), r0, rows, n, n, r["rank"].data_ptr(), k1, k2,
+                                             r["v_idx"].data_ptr(), r["v_val"].data_ptr(), r["v_cnt"].data_ptr(), s))
+        mark("B")
+        if k2 > 1:
+            N.check(L.ctl_rerank_qe(r["rank"].data_ptr(), n, k1, k2, r["v_idx"].data_ptr(), r["v_val"].data_ptr(),
+                                    r["v_cnt"].data_ptr(), r["q_idx"].data_ptr(), r["q_val"].data_ptr(),
+                                    r["q_cnt"].data_ptr(), s))
+        N.check(L.ctl_rerank_invert(nq, ng, r["q_idx"].data_ptr(), r["q_val"].data_ptr(), r["q_cnt"].data_ptr(), cap,
+                                    r["col_ptr"].data_ptr(), cursor.data_ptr(), r["inv_row"].data_ptr(),
+                                    r["inv_val"].data_ptr(), s))
+        mark("qe_invert")
+        del blk
+        Rq = min(R, nq)
+        fin = torch.empty(Rq, ng, **f32)
+        for q0 in range(0, nq, Rq):  # sweep C
+            rows = min(Rq, nq - q0)
+            out = rerank_final_rows(r, q0, rows, out=fin)
+            N.check(L.ctl_rerank_topk_rows(out.data_ptr(), q0, rows, ng, ng, k, r["idx"].data_ptr(),
+                                           r["dist"].data_ptr(), s))
+            if ev is not None:
+                ids, mp = ev["ids"], ev["ids"].max_pos
+                idp = (ids.q_pid.data_ptr() + 4 * q0, ids.q_cam.data_ptr() + 4 * q0, ids.g_pid.data_ptr(),
+                       ids.g_mask.data_ptr(), mp)
+                pk, pc = ev["pos_keys"][q0:].data_ptr(), ev["pos_count"][q0:].data_ptr()
+                N.check(L.ctl_eval_matrix_collect(out.data_ptr(), rows, ng, ng, *idp, pk, pc, ev["ovf"].data_ptr(), s))
+                N.check(L.ctl_sort_key_rows(pk, pc, rows, mp, s))
+                N.check(L.ctl_eval_matrix_count(out.data_ptr(), rows, ng, ng, *idp, pk, pc,
+                                                ev["buckets"][q0:].data_ptr(), s))
+        mark("C")
+        if ev is not None:
+            ranks, ap_h, first_h, cnt_h, ovf_h = _finalize_and_read_back(ev["buckets"], ev["pos_count"], nq,
+                                                                          ev["ids"].max_pos, ev["ovf"])
+            if ovf_h:
+                raise OverflowError("positives list overflowed (max_pos too small)")
+            r["eval"] = _aggregate(ranks, ap_h, cnt_h, np.asarray(q_pids), ng, max_rank, first=first_h)
+    return r
+
+
+def rerank_final_rows(r: dict, q0: int, rows: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The re-ranked distances of queries [q0, q0 + rows) against the whole gallery, [rows, G] float32, from the tables of
+    rerank_blocked_stages (sweep C of one query block: ctl_rerank_dist_rows normalised by the stored row maxima, then
+    ctl_rerank_jaccard_rows) -- the same rows of rerank()'s output, bit for bit."""
+    L = N.lib()
+    planes = r["planes"]
+    nq, ng = r["idx"].shape[0], r["inv_row"].numel() // r["q_idx"].shape[1]
+    n = nq + ng
+    dev = r["rank"].device
+    nd = torch.empty(rows, ng, dtype=torch.float32, device=dev)
+    if out is None:
+        out = torch.empty(rows, ng, dtype=torch.float32, device=dev)
+    out = out[:rows]
+    with torch.cuda.device(dev):
+        s = N.stream_ptr()
+        N.check(L.ctl_rerank_dist_rows(planes.ptr, n, planes.d, planes.flags, q0, rows, nq, ng, r["rowmax"].data_ptr(),
+                                       nd.data_ptr(), ng, s))
+        N.check(L.ctl_rerank_jaccard_rows(nq, ng, q0, rows, r["q_idx"].data_ptr(), r["q_val"].data_ptr(),
+                                          r["q_cnt"].data_ptr(), r["q_idx"].shape[1], r["col_ptr"].data_ptr(),
+                                          r["inv_row"].data_ptr(), r["inv_val"].data_ptr(), nd.data_ptr(), ng,
+                                          r["lambda"], out.data_ptr(), ng, s))
+    return out

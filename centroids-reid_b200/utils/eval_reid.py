@@ -86,9 +86,10 @@ def eval_streamed(q_feats, g_feats, q_pids, g_pids, q_camids, g_camids, max_rank
 
 def eval_reranked(q_feats, g_feats, q_pids, g_pids, q_camids, g_camids, max_rank=50, respect_camids=False, k1=20, k2=6,
                   lambda_value=0.3, feat_norm=False):
-    """eval_func's results on k-reciprocal re-ranked distances (retrieval.rerank, then retrieval.evaluate_matrix on the
-    [Q, G] matrix, both on the H100).  Same 4-tuple as eval_streamed.  Host tensors are staged to the current CUDA
-    device."""
+    """eval_func's results on k-reciprocal re-ranked distances, on the H100.  Same 4-tuple as eval_streamed.  Host
+    tensors are staged to the current CUDA device.  When the dense re-ranking and its [Q, G] matrix fit in the device's
+    free memory (retrieval.rerank_fits_dense): retrieval.rerank, then retrieval.evaluate_matrix; otherwise (galleries
+    beyond the N^2 bound) the row-blocked retrieval.rerank_topk_and_eval, whose results are bit-identical."""
     import torch
 
     q = torch.as_tensor(q_feats)
@@ -97,6 +98,11 @@ def eval_reranked(q_feats, g_feats, q_pids, g_pids, q_camids, g_camids, max_rank
         q = q.cuda(non_blocking=True)
     if not g.is_cuda:
         g = g.to(q.device, non_blocking=True)
-    dist = _R.rerank(q, g, k1, k2, lambda_value, feat_norm)
-    res = _R.evaluate_matrix(dist, q_pids, g_pids, q_camids, g_camids, max_rank, respect_camids)
+    free, _ = torch.cuda.mem_get_info(q.device)
+    if _R.rerank_fits_dense(q.shape[0], g.shape[0], k1, k2, free):
+        dist = _R.rerank(q, g, k1, k2, lambda_value, feat_norm)
+        res = _R.evaluate_matrix(dist, q_pids, g_pids, q_camids, g_camids, max_rank, respect_camids)
+    else:
+        _, _, res = _R.rerank_topk_and_eval(q, g, 1, q_pids, g_pids, q_camids, g_camids, k1, k2, lambda_value, feat_norm,
+                                            max_rank, respect_camids)
     return res.cmc, res.mAP, res.all_topk, res.single_performance

@@ -222,6 +222,51 @@ int ctl_rerank_jaccard(int64_t nq, int64_t ng, const int32_t* idx, const float* 
                        const int32_t* col_ptr, const int32_t* inv_row, const float* inv_val, const float* nd,
                        int64_t ld_nd, float lambda_value, float* out, int64_t ld_out, ctl_stream_t stream);
 
+/* Row-blocked re-ranking: the steps above with at most a [block_rows, N] slice of the distance matrix alive, so the
+ * workspace grows linearly in N (ctl_rerank's grows as N^2), and only each query's top-k of the re-ranked [Q, G] matrix
+ * (and, optionally, the evaluation passes over it) is kept.  Bit-identical to ctl_rerank for every block_rows:
+ *   sweep A, each row block: D rows (ctl_dist_matrix rows of [q; g] against all N) -> row maxima, nd, rank;
+ *   sweep B, each row block: the same D rows again, normalised by the stored maxima -> expansion (V) of those rows
+ *            (it reads nd at 2-hop candidates, which are not in the row's own rank list, hence a second sweep);
+ *   qe and invert once, as in ctl_rerank;
+ *   sweep C, each block of query rows: D against the gallery rows, normalised -> Jaccard + blend -> the k smallest
+ *            (distance, gallery column) -> out_idx / out_dist [nq, k], ascending; with identities (q_pid != NULL) also
+ *            the collect / sort / count passes of ctl_eval_matrix_* on those rows (the caller completes them with
+ *            ctl_eval_finalize_packed).
+ * The GEMM runs one plan and k-order for every shape, so a distance depends only on its two rows; the row maximum is
+ * exact; the normalisation is the same IEEE division; the later kernels are ctl_rerank's.
+ * ctl_rerank_topk zeroes *status, pos_count, buckets and *overflow; no host synchronisation, no allocation (capturable
+ * in a CUDA graph).  ctl_rerank_topk_workspace_bytes is host-only: 0 for what ctl_rerank_plan rejects, and for d not a
+ * positive multiple of 8, k < 1, k > min(128, ng) or block_rows < 1. */
+size_t ctl_rerank_topk_workspace_bytes(int64_t nq, int64_t ng, int32_t d, int32_t k1, int32_t k2, int32_t k,
+                                       int64_t block_rows);
+int ctl_rerank_topk(const void* planes, int64_t nq, int64_t ng, int32_t d, int32_t flags, int32_t k1, int32_t k2,
+                    float lambda_value, int32_t k, int64_t block_rows, int64_t* out_idx, float* out_dist,
+                    const int32_t* q_pid, const int32_t* q_cam, const int32_t* g_pid, const uint64_t* g_cammask,
+                    int32_t max_pos, uint64_t* pos_keys, int32_t* pos_count, int32_t* buckets, int32_t* overflow,
+                    int32_t* status, void* workspace, size_t workspace_bytes, ctl_stream_t stream);
+/* The row-block stages ctl_rerank_topk composes.  Every table (rank [n, kr], rowmax [n], V, out_idx / out_dist
+ * [nq, k]) is the global one; a block covers rows [r0, r0 + rows) (queries [q0, q0 + rows) for jaccard) and its
+ * matrix argument holds just those rows:
+ *   dist_rows   : rows [r0, r0 + rows) of the planes (n rows) against rows [c0, c0 + cols) -> out [rows, ld_out];
+ *                 with rowmax != NULL divided by rowmax[r0 + i] as the rank stage does (nd);
+ *   rank_rows   : steps 2 + 3 of a [rows, n] block: nd in place, rank and rowmax of its rows, *status OR-ed;
+ *   expand_rows : step 4 of the block's rows (its nd [rows, n]), into the global V;
+ *   jaccard_rows: step 6 of the queries, nd [rows, ld_nd] holding the gallery columns only, out [rows, ld_out];
+ *   topk_rows   : the k <= min(128, n) smallest (value, column) of each row of a [rows, n] block, ascending. */
+int ctl_rerank_dist_rows(const void* planes, int64_t n, int32_t d, int32_t flags, int64_t r0, int64_t rows, int64_t c0,
+                         int64_t cols, const float* rowmax, float* out, int64_t ld_out, ctl_stream_t stream);
+int ctl_rerank_rank_rows(float* dist, int64_t r0, int64_t rows, int64_t n, int64_t ld, int32_t kr, int32_t* rank,
+                         float* rowmax, int32_t* status, ctl_stream_t stream);
+int ctl_rerank_expand_rows(const float* nd, int64_t r0, int64_t rows, int64_t n, int64_t ld, const int32_t* rank,
+                           int32_t k1, int32_t k2, int32_t* v_idx, float* v_val, int32_t* v_cnt, ctl_stream_t stream);
+int ctl_rerank_jaccard_rows(int64_t nq, int64_t ng, int64_t q0, int64_t rows, const int32_t* idx, const float* val,
+                            const int32_t* cnt, int32_t cap, const int32_t* col_ptr, const int32_t* inv_row,
+                            const float* inv_val, const float* nd, int64_t ld_nd, float lambda_value, float* out,
+                            int64_t ld_out, ctl_stream_t stream);
+int ctl_rerank_topk_rows(float* dist, int64_t r0, int64_t rows, int64_t n, int64_t ld, int32_t k, int64_t* out_idx,
+                         float* out_dist, ctl_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * Per-identity centroid mean (segmented reduction)
  * replaces: modelling/bases.py:92-95 (_calculate_centroids), the tensor part of
