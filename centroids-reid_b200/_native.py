@@ -174,6 +174,8 @@ SIGNATURES = {
     "ctl_upsample2_zero_nhwc_f16": (C.c_int, [_p, _i32, _i32, _i32, _i32, _p, _p, _p]),
     "ctl_stem_im2col_f16": (C.c_int, [_p, _i32, _i32, _i32, _p, _p]),
     "ctl_augment_batch_u8": (C.c_int, [_p, _i32, _i32, _i32, _i32, _p, _p, _p, _p, _p]),
+    "ctl_resize_bilinear_u8_workspace_bytes": (_sz, [_i64, _i32, _i32]),
+    "ctl_resize_bilinear_u8": (C.c_int, [_p, _i64, _p, _i64, _i32, _i32, _p, _p, _p, _sz, _p]),
     "ctl_adam_multi_step": (C.c_int, [_p, _i32, C.c_int64, _f, _f, _f, _f, _f, C.c_int64, _f, _p, _p]),
     "ctl_sgd_step": (C.c_int, [_p, _p, C.c_int64, _f, _f, _p, _p]),
     "ctl_loss_scale_update": (C.c_int, [_p, _p, _p, _p, _f, _f, _f, _i32, _p]),

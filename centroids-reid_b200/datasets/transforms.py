@@ -1,5 +1,7 @@
-"""Device-side training transforms: the arithmetic of ReidTransforms.build_transforms(is_train=True)
-(datasets/transforms/build.py:15-27) after `T.Resize`, for a whole batch in one kernel.
+"""Device-side transforms: the arithmetic of ReidTransforms.build_transforms (datasets/transforms/build.py:15-33) for a
+whole batch -- `T.Resize` of native-size images packed in a RaggedImages (pack_images -> resize_batch, bit for bit
+PIL's BILINEAR resize), then the training chain after it in one kernel (augment_batch) or the eval chain
+(normalize_batch, or TrunkEngine.forward_u8, which folds it into the stem).  This module alone knows the ragged layout.
 
 The reference draws its random numbers per image inside torchvision / `random` (flip: torch.rand(1) < p;
 crop: torch.randint; erasing: random.uniform / random.randint with up to 100 attempts, random_erasing.py:30-55).
@@ -78,3 +80,104 @@ def normalize_batch(images_u8: torch.Tensor, pixel_mean=(0.485, 0.456, 0.406), p
 
 
 _NEUTRAL = {}
+
+
+class RaggedImages:
+    """A batch of native-size HWC RGB uint8 images of any sizes, packed back to back (no padding, any byte alignment)
+    in one uint8 buffer `data`, with `table` int64 [n, 3] = {byte offset, h, w} per image (struct ctl_resize_entry);
+    h = w = 0 is a mock row (the A0 batch contract's padded rows), which resizes to zeros.  `rows` is the sum of the
+    real images' heights, the row count of resize_batch's intermediate.  Built by pack_images; `resize_batch` turns it
+    into the `T.Resize` output."""
+
+    def __init__(self, data: torch.Tensor, table: torch.Tensor, rows: int):
+        self.data, self.table, self.rows = data, table, int(rows)
+
+    def __len__(self):
+        return self.table.shape[0]
+
+    @property
+    def device(self):
+        return self.data.device
+
+    def to(self, device, non_blocking: bool = True) -> "RaggedImages":
+        """The same batch on `device`; from pinned host buffers the copies do not block the host."""
+        return RaggedImages(self.data.to(device, non_blocking=non_blocking),
+                            self.table.to(device, non_blocking=non_blocking), self.rows)
+
+
+def pack_images(images, pin: bool = True) -> RaggedImages:
+    """HWC uint8 arrays [h, w, 3] or PIL RGB images (the reference's loaders decode with `.convert("RGB")`,
+    datasets/bases.py:32-33), with `None` for a mock row -> one host RaggedImages (pinned when `pin`)."""
+    arrays = []
+    for i, im in enumerate(images):
+        if im is None:
+            arrays.append(None)
+            continue
+        if hasattr(im, "mode") and hasattr(im, "size"):  # PIL image
+            if im.mode != "RGB":
+                raise ValueError(f"image {i}: PIL mode {im.mode!r}, expected 'RGB'")
+            im = np.asarray(im)
+        a = np.asarray(im)
+        if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3 or a.shape[0] < 1 or a.shape[1] < 1:
+            raise ValueError(f"image {i}: expected uint8 [h >= 1, w >= 1, 3], got {a.dtype} {a.shape}")
+        arrays.append(np.ascontiguousarray(a))
+    if not arrays:
+        raise ValueError("pack_images: no images")
+    table = np.zeros((len(arrays), 3), dtype=np.int64)
+    off = 0
+    for i, a in enumerate(arrays):
+        if a is not None:
+            table[i] = off, a.shape[0], a.shape[1]
+            off += a.nbytes
+    data = torch.empty(max(off, 1), dtype=torch.uint8, pin_memory=pin)
+    flat = data.numpy()
+    for (o, _, _), a in zip(table, arrays):
+        if a is not None:
+            flat[o: o + a.nbytes] = a.reshape(-1)
+    t = torch.from_numpy(table)
+    return RaggedImages(data, t.pin_memory() if pin else t, int(table[:, 1].sum()))
+
+
+def _resize_size(size):
+    if isinstance(size, (int, np.integer)) or len(size) != 2:
+        raise ValueError(f"size must be (h, w) as in T.Resize((h, w)) / INPUT.SIZE_TEST, got {size!r}")
+    return int(size[0]), int(size[1])
+
+
+def resize_workspace_bytes(ragged: RaggedImages, size) -> int:
+    """Bytes of the uint8 intermediate [ragged.rows, w, 3] (ctl_resize_bilinear_u8_workspace_bytes)."""
+    h, w = _resize_size(size)
+    n = N.lib().ctl_resize_bilinear_u8_workspace_bytes(ragged.rows, h, w)
+    if n == 0:
+        raise ValueError(f"resize to {size!r}: unsupported output size")
+    return n
+
+
+def _resize_enqueue(ragged: RaggedImages, out: torch.Tensor, status: torch.Tensor, workspace: torch.Tensor):
+    """ctl_resize_bilinear_u8 (enqueue only, capturable in a CUDA graph); the caller reads `status` back."""
+    N.check(N.lib().ctl_resize_bilinear_u8(ragged.data.data_ptr(), ragged.data.numel(), ragged.table.data_ptr(),
+                                           len(ragged), out.shape[1], out.shape[2], out.data_ptr(), status.data_ptr(),
+                                           workspace.data_ptr(), workspace.numel(), N.stream_ptr()))
+
+
+def resize_batch(ragged: RaggedImages, size) -> torch.Tensor:
+    """`T.Resize((h, w))` (datasets/transforms/build.py:19,29: PIL `Image.resize((w, h), BILINEAR)`) of every image of a
+    device RaggedImages -> uint8 [B, h, w, 3] on the device, bit for bit PIL's output; mock rows are zeros.  The input
+    of augment_batch, normalize_batch and TrunkEngine.forward_u8.  Reads the device status word back (one
+    synchronisation) and raises ValueError when a table entry does not fit in the data buffer."""
+    N.require_cuda(ragged.data, ragged.table)
+    if ragged.data.dtype != torch.uint8 or ragged.table.dtype != torch.int64 or ragged.table.dim() != 2 \
+            or ragged.table.shape[1] != 3 or not ragged.table.is_contiguous():
+        raise ValueError("resize_batch: expected a RaggedImages from pack_images")
+    h, w = _resize_size(size)
+    dev = ragged.device
+    with torch.cuda.device(dev):
+        out = torch.empty(len(ragged), h, w, 3, dtype=torch.uint8, device=dev)
+        status = torch.zeros(1, dtype=torch.int32, device=dev)
+        ws = torch.empty(resize_workspace_bytes(ragged, (h, w)), dtype=torch.uint8, device=dev)
+        _resize_enqueue(ragged, out, status, ws)
+        st = int(status.item())
+    if st:
+        raise ValueError(f"resize_batch: status {st}: a table entry lies outside the image buffer"
+                         f"{' or the intermediate' if st & 2 else ''}; its output is zeros")
+    return out

@@ -12,7 +12,8 @@ the embeddings on the device and copies them to the host ONCE (the reference doe
 inference_utils.py:123-125), `calculate_centroids` is the segmented-mean kernel, and `get_similar` streams
 query x gallery distances into a per-query top-k without materialising the [Q, G] matrix or its argsort
 (get_similar.py:112-119); with `topk == 0` the full matrix path of the reference is kept.
-The image-folder datasets / PIL loading of the reference stay where they are (host JPEG decode is out of scope).
+The image-folder datasets / PIL loading of the reference stay where they are (host JPEG decode is out of scope); a
+loader that ships the decoded images at native size as a RaggedImages has `T.Resize` run on the device.
 """
 from __future__ import annotations
 
@@ -24,6 +25,7 @@ import numpy as np
 import torch
 
 from .. import retrieval as R
+from ..datasets.transforms import RaggedImages, resize_batch
 from ..modelling.baseline import embed
 from ..reduce import calculate_centroids  # noqa: F401  (re-export: inference_utils.py:147-159)
 from ..utils.reid_metric import get_dist_func
@@ -31,11 +33,23 @@ from ..utils.reid_metric import get_dist_func
 log = logging.getLogger(__name__)
 
 
-def _inference(model, batch, use_cuda=True, normalize_with_bn=True):
-    """inference_utils.py:104-113.  `model` exposes `.backbone` (ctl_b200 Baseline) and `.bn`."""
+def _inference(model, batch, use_cuda=True, normalize_with_bn=True, cfg=None):
+    """inference_utils.py:104-113.  `model` exposes `.backbone` (ctl_b200 Baseline) and `.bn`.  `batch[0]` is the
+    reference's float tensor [B, 3, H, W], or a RaggedImages of native-size images (datasets.transforms.pack_images):
+    those are resized on the device to cfg.INPUT.SIZE_TEST (`T.Resize`, bit for bit PIL's) and embedded from uint8
+    with cfg.INPUT.PIXEL_MEAN / PIXEL_STD (TrunkEngine.forward_u8), so the loader ships native-size bytes only."""
     if not use_cuda:
         raise RuntimeError("ctl_b200 has no CPU path (use_cuda=False); run the reference for CPU inference")
     data, _, filename = batch
+    if isinstance(data, RaggedImages):
+        if cfg is None:
+            raise ValueError("_inference: a RaggedImages batch needs cfg (INPUT.SIZE_TEST, PIXEL_MEAN, PIXEL_STD)")
+        with torch.no_grad():
+            u8 = resize_batch(data.to("cuda"), cfg.INPUT.SIZE_TEST)
+            eng = model.backbone.engine(bn_head=model.bn) if normalize_with_bn else model.backbone.engine()
+            out = eng.forward_u8(u8, want_emb=normalize_with_bn, pixel_mean=tuple(cfg.INPUT.PIXEL_MEAN),
+                                 pixel_std=tuple(cfg.INPUT.PIXEL_STD))
+        return out["emb" if normalize_with_bn else "global_feat"], filename
     data = data.cuda(non_blocking=True)
     with torch.no_grad():
         if normalize_with_bn:
@@ -46,12 +60,13 @@ def _inference(model, batch, use_cuda=True, normalize_with_bn=True):
 
 
 def run_inference(model, val_loader, cfg, print_freq, use_cuda=True):
-    """inference_utils.py:116-131 -> (embeddings float32 [N, D] numpy, paths numpy array)."""
+    """inference_utils.py:116-131 -> (embeddings float32 [N, D] numpy, paths numpy array).  The loader yields float
+    tensors as the reference's does, or RaggedImages of native-size images (resized on the device, see _inference)."""
     chunks, paths = [], []
     for pos, x in enumerate(val_loader):
         if pos % print_freq == 0:
             log.info(f"Number of processed images: {pos * cfg.TEST.IMS_PER_BATCH}")
-        embedding, path = _inference(model, x, use_cuda)
+        embedding, path = _inference(model, x, use_cuda, cfg=cfg)
         chunks.append(embedding)  # stays on the device; one D2H copy at the end
         paths.extend(list(path))
     if not chunks:

@@ -18,7 +18,8 @@ def _alias(name):
 
 
 for _sub in ("_native", "retrieval", "utils", "utils.reid_metric", "utils.eval_reid", "losses",
-             "losses.triplet_loss", "losses.center_loss", "reduce", "modelling", "inference"):
+             "losses.triplet_loss", "losses.center_loss", "reduce", "modelling", "inference", "datasets",
+             "datasets.transforms"):
     try:
         _alias(_sub)
     except ModuleNotFoundError:

@@ -675,6 +675,34 @@ int ctl_grad_check_multi(const void* table_device, int32_t n_tensors, int64_t n_
 int ctl_augment_batch_u8(const void* images_u8_nhwc, int32_t n, int32_t h, int32_t w, int32_t pad, const int32_t* params_device,
                          const float* mean3_host, const float* std3_host, float* out_nchw, ctl_stream_t stream);
 
+/* ---- T.Resize((out_h, out_w)) of native-size images (datasets/transforms/build.py:19,29) ----
+ * The reference resizes PIL RGB images (datasets/bases.py:32-33, inference/inference_utils.py:33-34), so T.Resize is
+ * Image.resize((out_w, out_h), BILINEAR).  This reproduces it bit for bit.  PIL resamples the width first, then the
+ * height of the width pass's output clipped to uint8; per axis (`in` -> `out` pixels), in IEEE double without FMA:
+ *   scale = in / out, support = max(scale, 1), ss = 1 / support, center = (o + 0.5) scale,
+ *   xmin = max((int)(center - support + 0.5), 0), taps = min((int)(center + support + 0.5), in) - xmin,
+ *   w[t] = tri((t + xmin - center + 0.5) ss) (tri(x) = max(1 - |x|, 0)), each divided by their sum taken in tap order,
+ *   k[t] = (int)(0.5 + w[t] 2^22), pixel = clamp((2^21 + sum_t src[xmin + t] k[t]) >> 22, 0, 255) per channel.
+ * src: HWC RGB uint8 images packed back to back in src_bytes bytes, any byte alignment; table_device: n entries
+ * struct ctl_resize_entry below.  out_u8_nhwc: uint8 [n][out_h][out_w][3].  An entry with h == 0 or w == 0 is a mock
+ * row (zeros).  An entry whose h * w * 3 bytes at `offset` do not fit in src_bytes (or with a negative or > 2^24 side)
+ * gives zeros and sets bit 0 of *status; nothing outside src_bytes is read.
+ * workspace: the uint8 intermediate [sum of the h of the real entries][out_w][3], planned by
+ * ctl_resize_bilinear_u8_workspace_bytes(total_rows = that sum, ...), which is host-only and 0 for a negative
+ * total_rows or an output size the call rejects.  An image whose rows do not fit in the workspace gives zeros and sets
+ * bit 1 of *status.  Two launches (width pass, height pass); the call zeroes *status first.  No host synchronisation,
+ * no allocation: capturable in a CUDA graph.  A null pointer, n < 1, an output side outside 1..16384, or a workspace
+ * shorter than one intermediate row is CTL_ERR_INVALID_ARGUMENT before any device work. */
+typedef struct ctl_resize_entry {
+  int64_t offset; /* first byte of the image in src */
+  int64_t h;
+  int64_t w;
+} ctl_resize_entry;
+size_t ctl_resize_bilinear_u8_workspace_bytes(int64_t total_rows, int32_t out_h, int32_t out_w);
+int ctl_resize_bilinear_u8(const void* src, int64_t src_bytes, const void* table_device, int64_t n, int32_t out_h,
+                           int32_t out_w, void* out_u8_nhwc, int32_t* status, void* workspace, size_t workspace_bytes,
+                           ctl_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
