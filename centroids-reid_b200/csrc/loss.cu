@@ -280,7 +280,8 @@ __global__ void __launch_bounds__(128) mine_single_kernel(const float* __restric
     const float x = dap - dan;
     // hinge: max(0, x + margin); soft margin: log(1 + exp(x)), slope sigmoid(x)
     const float h = soft ? (fmaxf(x, 0.f) + log1pf(expf(-fabsf(x)))) : fmaxf(x + margin, 0.f);
-    const float slope = soft ? 1.f / (1.f + expf(-x)) : ((x + margin > 0.f) ? 1.f : 0.f);
+    // a hinge of exactly 0 passes the gradient, like torch's clamp_min / MarginRankingLoss
+    const float slope = soft ? 1.f / (1.f + expf(-x)) : ((x + margin >= 0.f) ? 1.f : 0.f);
     o.a_row[a] = active ? a : -1;
     o.p_row[a] = pidx;
     o.n_row[a] = nidx;
@@ -417,7 +418,7 @@ __global__ void __launch_bounds__(128) mine_step_kernel(const float* __restrict_
     o.hinge[t] = ok ? fmaxf(h, 0.f) : 0.f;
     bool sp = true, sn = true;
     if (ok) { pair_dist(G, NT, sq, a_row, pidx, &sp); pair_dist(G, NT, sq, a_row, nidx, &sn); }
-    const bool on = ok && h > 0.f;
+    const bool on = ok && h >= 0.f;  // a hinge of exactly 0 passes the gradient (torch's clamp_min)
     o.cap[t] = (on && !sp) ? 1.f / dap : 0.f;
     o.can[t] = (on && !sn) ? 1.f / dan : 0.f;
   }
