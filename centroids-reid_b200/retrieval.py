@@ -1068,9 +1068,44 @@ def rerank_blocked_stages(q: torch.Tensor, g: torch.Tensor, k: int, k1: int = 20
     nq, ng = q.shape[0], g.shape[0]
     n = nq + ng
     k, R, _ = _rerank_topk_args(nq, ng, planes.d, k1, k2, k, block_rows)
-    pl = rerank_plan(nq, ng, k1, k2)
-    L = N.lib()
     dev = q.device
+    r = _rerank_tables(planes, nq, ng, k, k1, k2, lambda_value, R)
+    ev = None
+    if q_pids is not None:
+        ev = _eval_buffers(encode_ids(q_pids, g_pids, q_camids, g_camids, respect_camids, dev), nq, dev)
+
+    def mark(name):
+        if events is not None:
+            e = torch.cuda.Event(enable_timing=True)
+            e.record()
+            events.append((name, e))
+
+    with torch.cuda.device(dev):
+        blk = torch.empty(min(R, n) * n, dtype=torch.float32, device=dev)
+        mark("start")
+        _rerank_sweep_a(r, 0, n, blk)
+        mark("A")
+        _rerank_sweep_b(r, 0, n, blk, k1, k2)
+        mark("B")
+        _rerank_qe_invert(r, k1, k2)
+        mark("qe_invert")
+        del blk
+        _rerank_sweep_c(r, 0, nq, ev)
+        mark("C")
+        if ev is not None:
+            ranks, ap_h, first_h, cnt_h, ovf_h = _finalize_and_read_back(ev["buckets"], ev["pos_count"], nq,
+                                                                          ev["ids"].max_pos, ev["ovf"])
+            if ovf_h:
+                raise OverflowError("positives list overflowed (max_pos too small)")
+            r["eval"] = _aggregate(ranks, ap_h, cnt_h, np.asarray(q_pids), ng, max_rank, first=first_h)
+    return r
+
+
+def _rerank_tables(planes: Planes, nq: int, ng: int, k: int, k1: int, k2: int, lambda_value: float, R: int) -> dict:
+    """The global tables of the row-blocked stages, every one linear in N = nq + ng (see rerank_blocked_stages)."""
+    n = nq + ng
+    pl = rerank_plan(nq, ng, k1, k2)
+    dev = planes.buf.device
     i32, f32 = dict(dtype=torch.int32, device=dev), dict(dtype=torch.float32, device=dev)
     r = {"plan": pl, "planes": planes, "block_rows": R, "lambda": float(lambda_value), "rank": torch.empty(n, pl.kr, **i32),
          "rowmax": torch.empty(n, **f32), "status": torch.zeros(1, **i32), "v_idx": torch.full((n, pl.v_cap), -1, **i32),
@@ -1084,68 +1119,77 @@ def rerank_blocked_stages(q: torch.Tensor, g: torch.Tensor, k: int, k1: int = 20
     cap = r["q_idx"].shape[1]
     r.update(col_ptr=torch.empty(n + 1, **i32), inv_row=torch.full((ng * cap,), -1, **i32),
              inv_val=torch.zeros(ng * cap, **f32))
-    ev = None
-    if q_pids is not None:
-        ev = _eval_buffers(encode_ids(q_pids, g_pids, q_camids, g_camids, respect_camids, dev), nq, dev)
-    cursor = torch.empty(n, **i32)
-    blk = torch.empty(min(R, n) * n, **f32)
-
-    def mark(name):
-        if events is not None:
-            e = torch.cuda.Event(enable_timing=True)
-            e.record()
-            events.append((name, e))
-
-    with torch.cuda.device(dev):
-        s = N.stream_ptr()
-        mark("start")
-        for r0 in range(0, n, R):  # sweep A
-            rows = min(R, n - r0)
-            N.check(L.ctl_rerank_dist_rows(planes.ptr, n, planes.d, planes.flags, r0, rows, 0, n, None,
-                                           blk.data_ptr(), n, s))
-            N.check(L.ctl_rerank_rank_rows(blk.data_ptr(), r0, rows, n, n, pl.kr, r["rank"].data_ptr(),
-                                           r["rowmax"].data_ptr(), r["status"].data_ptr(), s))
-        mark("A")
-        for r0 in range(0, n, R):  # sweep B
-            rows = min(R, n - r0)
-            N.check(L.ctl_rerank_dist_rows(planes.ptr, n, planes.d, planes.flags, r0, rows, 0, n,
-                                           r["rowmax"].data_ptr(), blk.data_ptr(), n, s))
-            N.check(L.ctl_rerank_expand_rows(blk.data_ptr(), r0, rows, n, n, r["rank"].data_ptr(), k1, k2,
-                                             r["v_idx"].data_ptr(), r["v_val"].data_ptr(), r["v_cnt"].data_ptr(), s))
-        mark("B")
-        if k2 > 1:
-            N.check(L.ctl_rerank_qe(r["rank"].data_ptr(), n, k1, k2, r["v_idx"].data_ptr(), r["v_val"].data_ptr(),
-                                    r["v_cnt"].data_ptr(), r["q_idx"].data_ptr(), r["q_val"].data_ptr(),
-                                    r["q_cnt"].data_ptr(), s))
-        N.check(L.ctl_rerank_invert(nq, ng, r["q_idx"].data_ptr(), r["q_val"].data_ptr(), r["q_cnt"].data_ptr(), cap,
-                                    r["col_ptr"].data_ptr(), cursor.data_ptr(), r["inv_row"].data_ptr(),
-                                    r["inv_val"].data_ptr(), s))
-        mark("qe_invert")
-        del blk
-        Rq = min(R, nq)
-        fin = torch.empty(Rq, ng, **f32)
-        for q0 in range(0, nq, Rq):  # sweep C
-            rows = min(Rq, nq - q0)
-            out = rerank_final_rows(r, q0, rows, out=fin)
-            N.check(L.ctl_rerank_topk_rows(out.data_ptr(), q0, rows, ng, ng, k, r["idx"].data_ptr(),
-                                           r["dist"].data_ptr(), s))
-            if ev is not None:
-                ids, mp = ev["ids"], ev["ids"].max_pos
-                idp = (ids.q_pid.data_ptr() + 4 * q0, ids.q_cam.data_ptr() + 4 * q0, ids.g_pid.data_ptr(),
-                       ids.g_mask.data_ptr(), mp)
-                pk, pc = ev["pos_keys"][q0:].data_ptr(), ev["pos_count"][q0:].data_ptr()
-                N.check(L.ctl_eval_matrix_collect(out.data_ptr(), rows, ng, ng, *idp, pk, pc, ev["ovf"].data_ptr(), s))
-                N.check(L.ctl_sort_key_rows(pk, pc, rows, mp, s))
-                N.check(L.ctl_eval_matrix_count(out.data_ptr(), rows, ng, ng, *idp, pk, pc,
-                                                ev["buckets"][q0:].data_ptr(), s))
-        mark("C")
-        if ev is not None:
-            ranks, ap_h, first_h, cnt_h, ovf_h = _finalize_and_read_back(ev["buckets"], ev["pos_count"], nq,
-                                                                          ev["ids"].max_pos, ev["ovf"])
-            if ovf_h:
-                raise OverflowError("positives list overflowed (max_pos too small)")
-            r["eval"] = _aggregate(ranks, ap_h, cnt_h, np.asarray(q_pids), ng, max_rank, first=first_h)
     return r
+
+
+def _rerank_sweep_a(r: dict, lo: int, hi: int, blk: torch.Tensor):
+    """Sweep A over rows [lo, hi) in blocks of r["block_rows"]: rank and rowmax of those rows (status OR-ed).  `blk` holds
+    min(block_rows, hi - lo) rows of N floats."""
+    L = N.lib()
+    planes, R = r["planes"], r["block_rows"]
+    n, s = planes.n, N.stream_ptr()
+    for r0 in range(lo, hi, R):
+        rows = min(R, hi - r0)
+        N.check(L.ctl_rerank_dist_rows(planes.ptr, n, planes.d, planes.flags, r0, rows, 0, n, None, blk.data_ptr(), n, s))
+        N.check(L.ctl_rerank_rank_rows(blk.data_ptr(), r0, rows, n, n, r["plan"].kr, r["rank"].data_ptr(),
+                                       r["rowmax"].data_ptr(), r["status"].data_ptr(), s))
+
+
+def _rerank_sweep_b(r: dict, lo: int, hi: int, blk: torch.Tensor, k1: int, k2: int):
+    """Sweep B over rows [lo, hi): the expansion V of those rows.  Reads rowmax of those rows and the rank table of
+    every row (the reciprocity test), so both must be complete."""
+    L = N.lib()
+    planes, R = r["planes"], r["block_rows"]
+    n, s = planes.n, N.stream_ptr()
+    for r0 in range(lo, hi, R):
+        rows = min(R, hi - r0)
+        N.check(L.ctl_rerank_dist_rows(planes.ptr, n, planes.d, planes.flags, r0, rows, 0, n, r["rowmax"].data_ptr(),
+                                       blk.data_ptr(), n, s))
+        N.check(L.ctl_rerank_expand_rows(blk.data_ptr(), r0, rows, n, n, r["rank"].data_ptr(), k1, k2,
+                                         r["v_idx"].data_ptr(), r["v_val"].data_ptr(), r["v_cnt"].data_ptr(), s))
+
+
+def _rerank_qe_invert(r: dict, k1: int, k2: int):
+    """Query expansion (k2 > 1) and the inverted index of the gallery rows, over the whole V."""
+    L = N.lib()
+    n = r["planes"].n
+    nq = r["idx"].shape[0]
+    cap = r["q_idx"].shape[1]
+    s = N.stream_ptr()
+    if k2 > 1:
+        N.check(L.ctl_rerank_qe(r["rank"].data_ptr(), n, k1, k2, r["v_idx"].data_ptr(), r["v_val"].data_ptr(),
+                                r["v_cnt"].data_ptr(), r["q_idx"].data_ptr(), r["q_val"].data_ptr(),
+                                r["q_cnt"].data_ptr(), s))
+    cursor = torch.empty(n, dtype=torch.int32, device=r["rank"].device)
+    N.check(L.ctl_rerank_invert(nq, n - nq, r["q_idx"].data_ptr(), r["q_val"].data_ptr(), r["q_cnt"].data_ptr(), cap,
+                                r["col_ptr"].data_ptr(), cursor.data_ptr(), r["inv_row"].data_ptr(),
+                                r["inv_val"].data_ptr(), s))
+
+
+def _rerank_sweep_c(r: dict, lo: int, hi: int, ev: Optional[dict]):
+    """Sweep C over queries [lo, hi) against the whole gallery: their top-k rows of r["idx"] / r["dist"] and, with
+    `ev` (_eval_buffers over all queries), the collect / sort / count passes of those rows."""
+    if hi <= lo:
+        return
+    L = N.lib()
+    nq = r["idx"].shape[0]
+    ng = r["planes"].n - nq
+    k = r["idx"].shape[1]
+    s = N.stream_ptr()
+    Rq = min(r["block_rows"], hi - lo)
+    fin = torch.empty(Rq, ng, dtype=torch.float32, device=r["rank"].device)
+    for q0 in range(lo, hi, Rq):
+        rows = min(Rq, hi - q0)
+        out = rerank_final_rows(r, q0, rows, out=fin)
+        N.check(L.ctl_rerank_topk_rows(out.data_ptr(), q0, rows, ng, ng, k, r["idx"].data_ptr(), r["dist"].data_ptr(), s))
+        if ev is not None:
+            ids, mp = ev["ids"], ev["ids"].max_pos
+            idp = (ids.q_pid.data_ptr() + 4 * q0, ids.q_cam.data_ptr() + 4 * q0, ids.g_pid.data_ptr(),
+                   ids.g_mask.data_ptr(), mp)
+            pk, pc = ev["pos_keys"][q0:].data_ptr(), ev["pos_count"][q0:].data_ptr()
+            N.check(L.ctl_eval_matrix_collect(out.data_ptr(), rows, ng, ng, *idp, pk, pc, ev["ovf"].data_ptr(), s))
+            N.check(L.ctl_sort_key_rows(pk, pc, rows, mp, s))
+            N.check(L.ctl_eval_matrix_count(out.data_ptr(), rows, ng, ng, *idp, pk, pc, ev["buckets"][q0:].data_ptr(), s))
 
 
 def rerank_final_rows(r: dict, q0: int, rows: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -1170,3 +1214,190 @@ def rerank_final_rows(r: dict, q0: int, rows: int, out: Optional[torch.Tensor] =
                                           r["inv_row"].data_ptr(), r["inv_val"].data_ptr(), nd.data_ptr(), ng,
                                           r["lambda"], out.data_ptr(), ng, s))
     return out
+
+
+# ----------------------------------------------------------------------------------------
+# row-blocked re-ranking sharded over ranks
+# ----------------------------------------------------------------------------------------
+
+
+def row_shares(n: int, world: int) -> list:
+    """The contiguous share [lo, hi) of n rows that each of `world` ranks computes: sizes differ by at most one, and a
+    rank gets no rows when world > n."""
+    return [(j * int(n) // world, (j + 1) * int(n) // world) for j in range(world)]
+
+
+class ShardExchange:
+    """The exchanges of the sharded re-ranking, over the ranks of a torch.distributed group (None: one rank, nothing is
+    exchanged).  Every rank calls each method in the same order."""
+
+    def __init__(self, group=None):
+        import torch.distributed as dist
+
+        self.group = group
+        self.world = 1 if group is None else dist.get_world_size(group)
+        self.rank = 0 if group is None else dist.get_rank(group)
+
+    def objects(self, obj) -> list:
+        """Every rank's picklable `obj`, in rank order."""
+        import torch.distributed as dist
+
+        if self.group is None:
+            return [obj]
+        out = [None] * self.world
+        dist.all_gather_object(out, obj, group=self.group)
+        return out
+
+    def rows(self, t: torch.Tensor, counts: Sequence[int]) -> torch.Tensor:
+        """The concatenation over ranks of each rank's `t` (counts[j] rows on rank j): shards padded to the largest,
+        all-gathered, trimmed."""
+        import torch.distributed as dist
+
+        if self.group is None:
+            return t
+        m = max(counts)
+        pad = t.new_zeros((m,) + tuple(t.shape[1:]))
+        pad[: t.shape[0]] = t
+        out = t.new_empty((self.world * m,) + tuple(t.shape[1:]))
+        dist.all_gather_into_tensor(out, pad, group=self.group)
+        if all(c == m for c in counts):
+            return out
+        return torch.cat([out[j * m: j * m + c] for j, c in enumerate(counts)])
+
+    def max_(self, t: torch.Tensor) -> torch.Tensor:
+        """In place: the element-wise maximum over ranks."""
+        import torch.distributed as dist
+
+        if self.group is not None:
+            dist.all_reduce(t, op=dist.ReduceOp.MAX, group=self.group)
+        return t
+
+
+def _local_error(q_local, g_local, ids_args):
+    """What is wrong with this rank's own arguments, as (exception class, message), or None."""
+    try:
+        N.require_cuda(q_local, g_local)
+        if q_local.dim() != 2 or g_local.dim() != 2 or q_local.shape[1] != g_local.shape[1]:
+            raise ValueError(f"expected [Q_r, d] and [G_r, d] features, got {tuple(q_local.shape)} and "
+                             f"{tuple(g_local.shape)}")
+        if q_local.device != g_local.device:
+            raise ValueError("query and gallery shards are on different devices")
+        if ids_args is not None and len(ids_args[1]) != g_local.shape[0]:
+            raise ValueError(f"{len(ids_args[1])} gallery pids for {g_local.shape[0]} gallery rows")
+    except (RuntimeError, ValueError) as e:
+        return type(e), str(e)
+    return None
+
+
+def _rerank_sharded(ex, q_local: torch.Tensor, g_local: torch.Tensor, k: int, k1: int, k2: int, lambda_value: float,
+                    normalize: bool, block_rows: Optional[int], ids_args=None, max_rank: int = 50) -> dict:
+    """The sharded protocol of rerank_topk_sharded / rerank_topk_and_eval_sharded over the exchange `ex` (ShardExchange,
+    or a stand-in with its methods).  ids_args = (q_pids of all queries, this rank's g_pids, q_camids of all queries, this
+    rank's g_camids, respect_camids) adds the evaluation.  Returns the gathered tables of rerank_blocked_stages (rank,
+    rowmax, v_*, q_*, col_ptr, inv_*, idx, dist, status, plan, planes, block_rows; `eval` with identities), the same on
+    every rank."""
+    # 1. shard sizes, identities and local errors in ONE exchange; then every rank checks the same global arguments and
+    #    raises the same error before any data is exchanged
+    err = _local_error(q_local, g_local, ids_args)
+    ok = err is None
+    mine = {"nq": q_local.shape[0] if ok else 0, "ng": g_local.shape[0] if ok else 0, "d": q_local.shape[1] if ok else 0,
+            "err": err}
+    if ids_args is not None:
+        mine.update(nq_ids=len(ids_args[0]), g_pids=np.asarray(ids_args[1]),
+                    g_camids=list(ids_args[3])[: mine["ng"]])
+    meta = ex.objects(mine)
+    for j, m in enumerate(meta):
+        if m["err"] is not None:
+            raise m["err"][0](f"rank {j}: {m['err'][1]}")
+    nq_r, ng_r = [m["nq"] for m in meta], [m["ng"] for m in meta]
+    nq, ng = sum(nq_r), sum(ng_r)
+    if len({m["d"] for m in meta}) != 1:
+        raise ValueError(f"feature widths differ across ranks: {[m['d'] for m in meta]}")
+    d = meta[0]["d"]
+    k, R, _ = _rerank_topk_args(nq, ng, d, k1, k2, k, block_rows)
+    if ids_args is not None and any(m["nq_ids"] != nq for m in meta):
+        raise ValueError(f"q_pids must cover all {nq} queries; ranks give {[m['nq_ids'] for m in meta]}")
+
+    # 2. features of all N rows on every rank, in the order [queries by rank; gallery by rank]
+    dev = q_local.device
+    q = ex.rows(q_local.detach().float().contiguous(), nq_r)
+    g = ex.rows(g_local.detach().float().to(dev).contiguous(), ng_r)
+    planes = _rerank_inputs(q, g, normalize)
+    del q, g
+    r = _rerank_tables(planes, nq, ng, k, k1, k2, lambda_value, R)
+    ev = None
+    if ids_args is not None:
+        q_pids, _, q_camids, _, respect_camids = ids_args
+        g_pids = np.concatenate([m["g_pids"] for m in meta])
+        g_camids = [c for m in meta for c in m["g_camids"]]
+        ev = _eval_buffers(encode_ids(q_pids, g_pids, q_camids, g_camids, respect_camids, dev), nq, dev)
+    n = nq + ng
+    shares, q_shares = row_shares(n, ex.world), row_shares(nq, ex.world)
+    lo, hi = shares[ex.rank]
+    qlo, qhi = q_shares[ex.rank]
+    counts, q_counts = [b - a for a, b in shares], [b - a for a, b in q_shares]
+    with torch.cuda.device(dev):
+        # 3. sweep A on this rank's rows -> the whole rank table and row maxima
+        blk = torch.empty(min(R, hi - lo) * n, dtype=torch.float32, device=dev)
+        _rerank_sweep_a(r, lo, hi, blk)
+        r["rank"] = ex.rows(r["rank"][lo:hi], counts)
+        r["rowmax"] = ex.rows(r["rowmax"][lo:hi], counts)
+        ex.max_(r["status"])
+        # 4. sweep B on the same rows -> the whole V
+        _rerank_sweep_b(r, lo, hi, blk, k1, k2)
+        del blk
+        for key in ("v_idx", "v_val", "v_cnt"):
+            r[key] = ex.rows(r[key][lo:hi], counts)
+        if k2 == 1:
+            r.update(q_idx=r["v_idx"], q_val=r["v_val"], q_cnt=r["v_cnt"])
+        # 5. query expansion and the inverted index, whole, on every rank
+        _rerank_qe_invert(r, k1, k2)
+        # 6. sweep C on this rank's queries against the whole gallery, then the per-query results of every rank
+        _rerank_sweep_c(r, qlo, qhi, ev)
+        r["idx"] = ex.rows(r["idx"][qlo:qhi], q_counts)
+        r["dist"] = ex.rows(r["dist"][qlo:qhi], q_counts)
+        if ev is not None:
+            mp = ev["ids"].max_pos
+            ex.max_(ev["ovf"])
+            if qhi > qlo:
+                ranks, pack = _finalize(ev["buckets"][qlo:qhi], ev["pos_count"][qlo:qhi], qhi - qlo, mp, ev["ovf"])
+            else:
+                ranks = torch.empty(0, mp, dtype=torch.int32, device=dev)
+                pack = torch.empty(1, 3, dtype=torch.float64, device=dev)
+            ranks = ex.rows(ranks, q_counts)
+            pack = torch.cat([ex.rows(pack[: qhi - qlo], q_counts), ev["ovf"].double().expand(1, 3)])
+            h = pack.cpu().numpy()
+        st = int(r["status"].item())
+    if st:
+        raise ValueError("re-ranking: a row of the distance matrix has no positive maximum (N = 1 or identical features)")
+    if ev is not None:
+        ap_h, first_h, cnt_h, ovf_h = _unpack(h, nq)
+        if ovf_h:
+            raise OverflowError("positives list overflowed (max_pos too small)")
+        r["eval"] = _aggregate(ranks, ap_h, cnt_h, np.asarray(q_pids), ng, max_rank, first=first_h)
+    return r
+
+
+def rerank_topk_sharded(q_local: torch.Tensor, g_local: torch.Tensor, k: int, k1: int = 20, k2: int = 6,
+                        lambda_value: float = 0.3, normalize: bool = False, block_rows: Optional[int] = None, group=None):
+    """rerank_topk with the queries and the gallery sharded over the ranks of `group` (torch.distributed; None: one
+    rank).  Rank j holds q_local [Q_j, d] and g_local [G_j, d]; the problem is queries [all q_local in rank order] against
+    gallery [all g_local in rank order], and returned gallery indices are positions in that concatenation.  Every rank
+    returns the full (idx [Q, k] int64, dist [Q, k] float32), bit-identical to rerank_topk on the concatenated features.
+    The N = Q + G rows of sweeps A and B and the Q queries of sweep C are split in contiguous shares (row_shares); the
+    rank table, the row maxima, V and the results are all-gathered between the sweeps (DESIGN.md §5)."""
+    r = _rerank_sharded(ShardExchange(group), q_local, g_local, k, k1, k2, lambda_value, normalize, block_rows)
+    return r["idx"], r["dist"]
+
+
+def rerank_topk_and_eval_sharded(q_local: torch.Tensor, g_local: torch.Tensor, k: int, q_pids, g_pids_local, q_camids,
+                                 g_camids_local, k1: int = 20, k2: int = 6, lambda_value: float = 0.3,
+                                 normalize: bool = False, max_rank: int = 50, respect_camids: bool = False,
+                                 block_rows: Optional[int] = None, group=None):
+    """rerank_topk_and_eval with the queries and the gallery sharded over the ranks of `group`, as rerank_topk_sharded.
+    q_pids / q_camids cover ALL queries (as in topk_and_eval_sharded); g_pids_local / g_camids_local this rank's gallery
+    rows.  Every rank returns (idx, dist, EvalResult), bit-identical to rerank_topk_and_eval on the concatenation."""
+    ids_args = (q_pids, g_pids_local, q_camids, g_camids_local, respect_camids)
+    r = _rerank_sharded(ShardExchange(group), q_local, g_local, k, k1, k2, lambda_value, normalize, block_rows, ids_args,
+                        max_rank)
+    return r["idx"], r["dist"], r["eval"]

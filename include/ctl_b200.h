@@ -253,7 +253,14 @@ int ctl_rerank_topk(const void* planes, int64_t nq, int64_t ng, int32_t d, int32
  *   rank_rows   : steps 2 + 3 of a [rows, n] block: nd in place, rank and rowmax of its rows, *status OR-ed;
  *   expand_rows : step 4 of the block's rows (its nd [rows, n]), into the global V;
  *   jaccard_rows: step 6 of the queries, nd [rows, ld_nd] holding the gallery columns only, out [rows, ld_out];
- *   topk_rows   : the k <= min(128, n) smallest (value, column) of each row of a [rows, n] block, ascending. */
+ *   topk_rows   : the k <= min(128, n) smallest (value, column) of each row of a [rows, n] block, ascending.
+ * With the rows sharded over ranks (each holding the planes of all N rows): sweep A on the rank's contiguous rows,
+ * all-gather rank and rowmax, OR (MAX) the status words; sweep B on the same rows (expand_rows reads the rank lists of
+ * other rows), all-gather V; qe and invert on every rank over the whole V; sweep C on the rank's contiguous queries
+ * against all ng gallery rows, then the collect / sort / count passes and ctl_eval_finalize_packed on those queries
+ * alone, and all-gather idx / dist, ranks and the packed rows.  Each stage writes only its own rows of the global
+ * tables, so the gathered tables and results equal the one-rank run's bit for bit; the entry points above need no
+ * offset beyond r0 / q0. */
 int ctl_rerank_dist_rows(const void* planes, int64_t n, int32_t d, int32_t flags, int64_t r0, int64_t rows, int64_t c0,
                          int64_t cols, const float* rowmax, float* out, int64_t ld_out, ctl_stream_t stream);
 int ctl_rerank_rank_rows(float* dist, int64_t r0, int64_t rows, int64_t n, int64_t ld, int32_t kr, int32_t* rank,
