@@ -7,7 +7,7 @@ include/ctl_b200.h.  torch is used for device memory, streams and torch.distribu
 """
 from __future__ import annotations
 
-from dataclasses import dataclass
+from dataclasses import dataclass, replace
 from typing import Optional, Sequence
 
 import numpy as np
@@ -318,16 +318,26 @@ def _finalize(buckets, count, nq, max_pos, ovf):
     return ranks, pack
 
 
-def _unpack(h: np.ndarray, nq: int):
-    """host view of `pack`: (ap, first-hit rank, #positives, overflow flag) -- float64 is exact for these integers."""
-    return h[:nq, 0], h[:nq, 1].astype(np.int64), h[:nq, 2].astype(np.int32), int(h[nq, 0])
+_OVF_POS = "positives list overflowed (max_pos too small)"
+_OVF_TOPK = "a device-side list overflowed (exact ties at the k-th distance, or max_pos)"
 
 
-def _finalize_and_read_back(buckets, count, nq, max_pos, ovf):
-    """_finalize + ONE device->host copy.  Returns (ranks on the device, ap, first, count, overflow) -- the last four on
-    the host."""
-    ranks, pack = _finalize(buckets, count, nq, max_pos, ovf)
-    return (ranks,) + _unpack(pack.cpu().numpy(), nq)
+def _eval_result(ranks, pack, q_pids, num_g: int, max_rank: int, msg: str = _OVF_POS, qp: Optional[Planes] = None,
+                 rows=()) -> tuple:
+    """The host end of every evaluation, from _finalize's (ranks, pack): ONE device->host copy of `pack` (unless it is
+    already a host array), the overflow check, the caller's query order (when `qp` stores its rows in another order;
+    `ranks` and the device tensors `rows` are re-ordered) and eval_func's final reductions.  Returns rows + (EvalResult,).
+    float64 is exact for the packed integers."""
+    h = pack if isinstance(pack, np.ndarray) else pack.cpu().numpy()
+    nq = h.shape[0] - 1
+    ap, first, cnt = h[:nq, 0], h[:nq, 1].astype(np.int64), h[:nq, 2].astype(np.int32)
+    if h[nq, 0]:
+        raise OverflowError(msg)
+    inv_d, inv_h = _query_inverse(qp) if qp is not None else (None, None)
+    if inv_h is not None:  # back to the caller's query order
+        rows = tuple(t.index_select(0, inv_d) for t in rows)
+        ranks, ap, first, cnt = ranks.index_select(0, inv_d), ap[inv_h], first[inv_h], cnt[inv_h]
+    return tuple(rows) + (_aggregate(ranks, ap, cnt, np.asarray(q_pids), num_g, max_rank, first=first),)
 
 
 def _tile_lists_enabled(qp: Planes, gp: Planes) -> bool:
@@ -386,58 +396,24 @@ def evaluate_streamed(
     """eval_func semantics (utils/eval_reid.py:25-92) straight from the features: two tensor-
     core passes (collect the positives' distances; count kept rows before each positive),
     no distance matrix, no argsort.  With `group` (torch.distributed), `gp` is this rank's
-    gallery shard and g_* its identities; keys are all-gathered, buckets all-reduced.
+    gallery shard and g_* its identities, and the passes exchange as topk_and_eval_sharded's do.  The merged threshold
+    list then holds world x (the largest per-shard max_pos of any rank, MAX-reduced here even when `ids` is given), so
+    the `ranks` matrix may carry more -1 padding columns than an unsharded run's; every column up to a query's positive
+    count is the same.
     Identities are given in the caller's row order even when the planes were built with `order=`; a precomputed `ids`
     must have been encoded with the planes' orders (encode_ids(q_order=, g_order=))."""
-    import ctypes as C
-
-    import torch.distributed as dist
-
-    L = N.lib()
+    ex = ShardExchange(group)
     dev = qp.buf.device
-    nq, ng = qp.n, gp.n
-    world = dist.get_world_size(group) if group is not None else 1
     if ids is None:
-        if world > 1 and not np.issubdtype(np.asarray(q_pids).dtype, np.integer):
+        if ex.world > 1 and not np.issubdtype(np.asarray(q_pids).dtype, np.integer):
             raise ValueError("sharded evaluation needs integer pids")
         # sharded: dense re-labelling must agree across ranks -> identity map instead of np.unique
-        ids = encode_ids(q_pids, g_pids, q_camids, g_camids, respect_camids, dev, global_labels=world > 1,
+        ids = encode_ids(q_pids, g_pids, q_camids, g_camids, respect_camids, dev, global_labels=ex.world > 1,
                          q_order=qp.order_host, g_order=gp.order_host)
-    d_qpid, d_qcam, d_gpid, d_gmask, max_pos_local = ids.q_pid, ids.q_cam, ids.g_pid, ids.g_mask, ids.max_pos
-    max_pos = max_pos_local
-    if world > 1:
-        mp = torch.tensor([max_pos_local], device=dev, dtype=torch.int64)
-        dist.all_reduce(mp, op=dist.ReduceOp.SUM, group=group)  # positives of a pid may spread over shards
-        max_pos = int(mp.item())
-    pos_keys = torch.zeros(nq, max_pos, dtype=torch.int64, device=dev)
-    pos_count = torch.zeros(nq, dtype=torch.int32, device=dev)
-    ovf = torch.zeros(1, dtype=torch.int32, device=dev)
-    s = N.stream_ptr
-    gmap = _g_index_map(gp, g_index_offset)
-    idp = dict(q_pid=d_qpid.data_ptr(), q_cam=d_qcam.data_ptr(), g_pid=d_gpid.data_ptr(), g_cammask=d_gmask.data_ptr(),
-               max_pos=max_pos, overflow=ovf.data_ptr(), g_index_offset=g_index_offset, g_index_map=N.ptr(gmap))
-    with torch.cuda.device(dev):
-        # pass 1 (collect) only wants the positives: tiles whose identity ranges are disjoint are not run -- with both
-        # operands stored in pid order (build_planes(order=pid_order(..))) that is ~95 % of a Market-sized problem
-        work = _tile_list(qp, gp, ids, 0) if _tile_lists_enabled(qp, gp) else None
-        p1 = N.PassDesc(pos_keys=pos_keys.data_ptr(), pos_count=pos_count.data_ptr(), tile_list=N.ptr(work), **idp)
-        N.check(L.ctl_dist_pass(qp.ptr, nq, gp.ptr, ng, qp.d, qp.flags, C.byref(p1), s()))
-        if world > 1:
-            pos_keys, pos_count = _allgather_keys(pos_keys, pos_count, max_pos, group)
-        N.check(L.ctl_sort_key_rows(pos_keys.data_ptr(), pos_count.data_ptr(), nq, max_pos, s()))
-        buckets = torch.zeros(nq, max_pos + 1, dtype=torch.int32, device=dev)
-        p2 = N.PassDesc(thr_keys=pos_keys.data_ptr(), thr_count=pos_count.data_ptr(), buckets=buckets.data_ptr(), **idp)
-        N.check(L.ctl_dist_pass(qp.ptr, nq, gp.ptr, ng, qp.d, qp.flags, C.byref(p2), s()))
-        if world > 1:
-            dist.all_reduce(buckets, op=dist.ReduceOp.SUM, group=group)
-        ranks, ap_h, first_h, cnt_h, ovf_h = _finalize_and_read_back(buckets, pos_count, nq, max_pos, ovf)
-    if ovf_h:
-        raise OverflowError("positives list overflowed (max_pos too small)")
-    inv_d, inv_h = _query_inverse(qp)
-    if inv_h is not None:  # back to the caller's query order
-        ranks, ap_h, first_h, cnt_h = ranks.index_select(0, inv_d), ap_h[inv_h], first_h[inv_h], cnt_h[inv_h]
-    num_g = total_gallery if total_gallery is not None else ng
-    return _aggregate(ranks, ap_h, cnt_h, np.asarray(q_pids), num_g, max_rank, first=first_h)
+    if ex.world > 1:
+        ids = replace(ids, max_pos=_max_over_ranks(ex, ids.max_pos, dev))
+    num_g = total_gallery if total_gallery is not None else gp.n
+    return _streamed(ex, qp, gp, ids, None, q_pids, num_g, max_rank, g_index_offset)[0]
 
 
 def _encode_identities_global(q_pids, g_pids, q_camids, g_camids):
@@ -450,28 +426,6 @@ def _encode_identities_global(q_pids, g_pids, q_camids, g_camids):
     g_mask = (np.uint64(1) << g_cam.astype(np.uint64)).astype(np.uint64)
     max_pos = int(np.bincount(g_pid - g_pid.min()).max()) if len(g_pid) else 1
     return q_pid, q_cam, g_pid, g_mask, max(1, max_pos)
-
-
-def _allgather_keys(pos_keys, pos_count, max_pos, group):
-    """Concatenates every rank's positives per query (ragged, packed to the left)."""
-    import torch.distributed as dist
-
-    world = dist.get_world_size(group)
-    keys_all = [torch.empty_like(pos_keys) for _ in range(world)]
-    cnt_all = [torch.empty_like(pos_count) for _ in range(world)]
-    dist.all_gather(keys_all, pos_keys, group=group)
-    dist.all_gather(cnt_all, pos_count, group=group)
-    nq = pos_keys.shape[0]
-    out = torch.zeros_like(pos_keys)
-    total = torch.zeros_like(pos_count)
-    col = torch.arange(max_pos, device=pos_keys.device)[None, :]
-    for kr, cr in zip(keys_all, cnt_all):
-        valid = col < cr[:, None]
-        dest = (total[:, None] + col).clamp(max=max_pos - 1)
-        rows = torch.arange(nq, device=pos_keys.device)[:, None].expand_as(dest)
-        out[rows[valid], dest[valid].long()] = kr[valid]
-        total = total + cr
-    return out, total
 
 
 def merge_topk(idx_list: Sequence[torch.Tensor], dist_list: Sequence[torch.Tensor], k: int):
@@ -552,89 +506,188 @@ def topk_and_eval(qp: Planes, gp: Planes, k: int, q_pids, g_pids, q_camids, g_ca
     Identities are given in the caller's row order; a precomputed `ids` must carry the planes' orders
     (encode_ids(q_order=qp.order_host, g_order=gp.order_host)).
     Returns (idx [nq,k] int64, dist [nq,k] float32 on the device, EvalResult), all in the caller's indexing."""
-    dev = qp.buf.device
     if ids is None:
-        ids = encode_ids(q_pids, g_pids, q_camids, g_camids, respect_camids, dev, q_order=qp.order_host,
+        ids = encode_ids(q_pids, g_pids, q_camids, g_camids, respect_camids, qp.buf.device, q_order=qp.order_host,
                          g_order=gp.order_host)
-    if tile_lists is None:
-        tile_lists = _tile_lists_enabled(qp, gp)
-    with torch.cuda.device(dev):
-        out = _topk_and_eval_enqueue(qp, gp, k, ids, tile_lists)
-        h = out["pack"].cpu().numpy()
-    return _topk_and_eval_finish(out, h, qp, gp, k, q_pids, g_pids, q_camids, g_camids, max_rank, respect_camids, ids)
+    return _streamed(ShardExchange(None), qp, gp, ids, k, q_pids, gp.n, max_rank, 0, tile_lists)
 
 
-def _topk_and_eval_enqueue(qp: Planes, gp: Planes, k: int, ids: "EncodedIds", tile_lists: bool):
-    """The launch sequence of topk_and_eval, no host synchronisation (capturable in a CUDA graph): returns the device
-    tensors {idx, dst, ranks, pack} in the planes' row order and whether pass 1 ran a threshold subset."""
+class ShardExchange:
+    """The exchanges of the sharded paths (the streamed passes of evaluate_streamed / topk_and_eval_sharded and the
+    row-blocked re-ranking), over the ranks of a torch.distributed group (None: one rank, nothing is exchanged).  Every
+    rank calls each method in the same order.  Tests substitute stand-ins with the same methods."""
+
+    def __init__(self, group=None):
+        import torch.distributed as dist
+
+        self.dist, self.group = dist, group
+        self.world = 1 if group is None else dist.get_world_size(group)
+        self.rank = 0 if group is None else dist.get_rank(group)
+
+    def objects(self, obj) -> list:
+        """Every rank's picklable `obj`, in rank order."""
+        if self.group is None:
+            return [obj]
+        out = [None] * self.world
+        self.dist.all_gather_object(out, obj, group=self.group)
+        return out
+
+    def rows(self, t: torch.Tensor, counts: Sequence[int]) -> torch.Tensor:
+        """The concatenation over ranks of each rank's `t` (counts[j] rows on rank j): one all-gather, of shards padded
+        to the largest when the counts differ, then trimmed."""
+        if self.group is None:
+            return t
+        m = max(counts)
+        even = all(c == m for c in counts)
+        part = t.contiguous()
+        if not even:
+            part = t.new_zeros((m,) + tuple(t.shape[1:]))
+            part[: t.shape[0]] = t
+        out = t.new_empty((self.world * m,) + tuple(t.shape[1:]))
+        self.dist.all_gather_into_tensor(out, part, group=self.group)
+        if even:
+            return out
+        return torch.cat([out[j * m: j * m + c] for j, c in enumerate(counts)])
+
+    def max_(self, t: torch.Tensor) -> torch.Tensor:
+        """In place: the element-wise maximum over ranks."""
+        if self.group is not None:
+            self.dist.all_reduce(t, op=self.dist.ReduceOp.MAX, group=self.group)
+        return t
+
+    def sum_(self, t: torch.Tensor) -> torch.Tensor:
+        """In place: the element-wise sum over ranks."""
+        if self.group is not None:
+            self.dist.all_reduce(t, op=self.dist.ReduceOp.SUM, group=self.group)
+        return t
+
+
+def _max_over_ranks(ex, v: int, device) -> int:
+    return int(ex.max_(torch.tensor([v], device=device, dtype=torch.int64)).item())
+
+
+def _gather_keys(ex, pos_keys: torch.Tensor, pos_count: torch.Tensor):
+    """Exchange 1 of the sharded passes, up to the row sort: every rank's positives' keys of a query side by side in rank
+    order, [nq, world * max_pos], with unused slots set to the largest key so that ONE sort of the whole row packs and
+    orders them (ctl_sort_key_rows); and the total count per query."""
+    nq, mp_l = pos_keys.shape
+    col = torch.arange(mp_l, device=pos_keys.device)[None, :]
+    masked = torch.where(col < pos_count[:, None].clamp(max=mp_l), pos_keys, torch.full_like(pos_keys, -1))
+    keys = ex.rows(masked, [nq] * ex.world).view(ex.world, nq, mp_l).permute(1, 0, 2).reshape(nq, ex.world * mp_l)
+    count = ex.rows(pos_count.contiguous(), [nq] * ex.world).view(ex.world, nq).sum(0, dtype=torch.int32)
+    return keys, count
+
+
+def _streamed_enqueue(ex, qp: Planes, gp: Planes, ids: "EncodedIds", k: Optional[int], tile_lists: bool,
+                      g_index_offset: int = 0) -> dict:
+    """The launch sequence of the streamed passes over this rank's gallery `gp` (the whole gallery at world 1), with the
+    exchanges of `ex` (ShardExchange or a stand-in) between them:
+      pass 1: the positives' keys (+ the 16-column group minima -> tau)
+      exchange 1 (world > 1): every rank's positives (_gather_keys); then one row sort gives the threshold list
+      pass 2: kept rows before each positive (+ the candidates <= tau, sorted)
+      exchange 2 (world > 1): sum of the bucket counts, MAX of the overflow flag, every rank's k best keys merged by
+                              integer key order; at world 1 the top-k is emitted from the candidates
+      finalize
+    k=None evaluates only: no minima, threshold or candidates.  `tile_lists`: pass 1 runs a tile list (topk_and_eval).
+    At world 1 nothing is exchanged and nothing waits for the host (capturable in a CUDA graph).  Returns the device
+    tensors {rows: (idx, dst) or (), ranks, pack} in the planes' query order."""
     import ctypes as C
 
     L = N.lib()
     dev = qp.buf.device
-    nq, ng = qp.n, gp.n
-    k = int(min(k, ng))
-    emit_all, n_groups, merge, cap = C.c_int32(), C.c_int32(), C.c_int32(), C.c_int32()
-    N.check(L.ctl_topk_plan(ng, k, C.byref(emit_all), C.byref(n_groups), C.byref(merge), C.byref(cap)))
-    d_qpid, d_qcam, d_gpid, d_gmask, max_pos = ids.q_pid, ids.q_cam, ids.g_pid, ids.g_mask, ids.max_pos
-    gmin = torch.empty(nq, n_groups.value, dtype=torch.float32, device=dev)
-    tau = torch.empty(nq, dtype=torch.float32, device=dev)
-    cand = torch.empty(nq, cap.value, dtype=torch.int64, device=dev)
-    zeros = torch.zeros(2 * nq + 1, dtype=torch.int32, device=dev)
-    cand_count, pos_count, ovf = zeros[:nq], zeros[nq: 2 * nq], zeros[2 * nq:]
-    pos_keys = torch.empty(nq, max_pos, dtype=torch.int64, device=dev)
-    buckets = torch.zeros(nq, max_pos + 1, dtype=torch.int32, device=dev)
-    idx = torch.empty(nq, k, dtype=torch.int64, device=dev)
-    dst = torch.empty(nq, k, dtype=torch.float32, device=dev)
+    nq, ng, world = qp.n, gp.n, ex.world
+    mp_l = ids.max_pos  # capacity of one rank's positives (the same on every rank)
+    mp = mp_l * world   # capacity of the merged threshold list
+    i32 = dict(dtype=torch.int32, device=dev)
     s = N.stream_ptr
-    gmap = _g_index_map(gp, 0)
-    idp = dict(q_pid=d_qpid.data_ptr(), q_cam=d_qcam.data_ptr(), g_pid=d_gpid.data_ptr(),
-               g_cammask=d_gmask.data_ptr(), max_pos=max_pos, overflow=ovf.data_ptr(), g_index_map=N.ptr(gmap))
-    p1 = N.PassDesc(pos_keys=pos_keys.data_ptr(), pos_count=pos_count.data_ptr(), **idp)
-    if not emit_all.value:
+    keep = []
+    if k is None:
+        emit_all = True
+        pos_keys = torch.zeros(nq, mp_l, dtype=torch.int64, device=dev)
+        pos_count, ovf = torch.zeros(nq, **i32), torch.zeros(1, **i32)
+        buckets = None
+    else:
+        k_loc = int(min(k, ng))
+        plan = [C.c_int32() for _ in range(4)]
+        N.check(L.ctl_topk_plan(ng, k_loc, *[C.byref(x) for x in plan]))
+        emit_all, n_groups, merge, cap = [x.value for x in plan]
+        gmin = torch.empty(nq, n_groups, dtype=torch.float32, device=dev)
+        tau = torch.empty(nq, dtype=torch.float32, device=dev)
+        cand = torch.empty(nq, cap, dtype=torch.int64, device=dev)
+        zeros = torch.zeros(2 * nq + 1, **i32)
+        cand_count, pos_count, ovf = zeros[:nq], zeros[nq: 2 * nq], zeros[2 * nq:]
+        pos_keys = torch.empty(nq, mp_l, dtype=torch.int64, device=dev)
+        buckets = torch.zeros(nq, mp + 1, **i32)
+        keep += [gmin, tau, cand, zeros]
+    gmap = _g_index_map(gp, g_index_offset)  # keys carry the caller's gallery row (sharded: the GLOBAL row)
+    idp = dict(q_pid=ids.q_pid.data_ptr(), q_cam=ids.q_cam.data_ptr(), g_pid=ids.g_pid.data_ptr(),
+               g_cammask=ids.g_mask.data_ptr(), overflow=ovf.data_ptr(), g_index_offset=g_index_offset,
+               g_index_map=N.ptr(gmap))
+    p1 = N.PassDesc(pos_keys=pos_keys.data_ptr(), pos_count=pos_count.data_ptr(), max_pos=mp_l, **idp)
+    if not emit_all:
         p1.gmin = gmin.data_ptr()
     work = None
-    if tile_lists:
-        # (small gallery, tau = +inf: pass 1 only collects -> stride 0, just the tiles that can hold a positive)
-        stride = 0 if emit_all.value else L.ctl_dist_subset_stride(ng, k)
-        if emit_all.value or stride > 1:
+    if tile_lists:  # (no threshold, or tau = +inf for a small gallery: stride 0, just the tiles that can hold a positive)
+        stride = 0 if emit_all else L.ctl_dist_subset_stride(ng, k_loc)
+        if emit_all or stride > 1:
             work = _tile_list(qp, gp, ids, stride)
     if work is not None:
         p1.tile_list = work.data_ptr()
-        if not emit_all.value:
+        if not emit_all:
             N.check(L.ctl_fill_f32(gmin.data_ptr(), gmin.numel(), float("inf"), s()))  # groups of tiles not run
     N.check(L.ctl_dist_pass(qp.ptr, nq, gp.ptr, ng, qp.d, qp.flags, C.byref(p1), s()))
-    if emit_all.value:
+    if k is not None and emit_all:
         N.check(L.ctl_fill_f32(tau.data_ptr(), nq, float("inf"), s()))
-    else:
-        N.check(L.ctl_select_tau(gmin.data_ptr(), nq, n_groups.value, merge.value, k, tau.data_ptr(), s()))
-    N.check(L.ctl_sort_key_rows(pos_keys.data_ptr(), pos_count.data_ptr(), nq, max_pos, s()))
-    p2 = N.PassDesc(tau=tau.data_ptr(), cand_keys=cand.data_ptr(), cand_count=cand_count.data_ptr(),
-                    cand_cap=cap.value, thr_keys=pos_keys.data_ptr(), thr_count=pos_count.data_ptr(),
-                    buckets=buckets.data_ptr(), **idp)
+    elif k is not None:
+        N.check(L.ctl_select_tau(gmin.data_ptr(), nq, n_groups, merge, k_loc, tau.data_ptr(), s()))
+    thr, thr_count, sort_count = pos_keys, pos_count, pos_count
+    if world > 1:
+        thr, thr_count = _gather_keys(ex, pos_keys, pos_count)
+        sort_count = torch.full((nq,), mp, **i32)
+    N.check(L.ctl_sort_key_rows(thr.data_ptr(), sort_count.data_ptr(), nq, mp, s()))
+    if buckets is None:
+        buckets = torch.zeros(nq, mp + 1, **i32)
+    p2 = N.PassDesc(thr_keys=thr.data_ptr(), thr_count=thr_count.data_ptr(), buckets=buckets.data_ptr(), max_pos=mp,
+                    **idp)
+    if k is not None:
+        p2.tau, p2.cand_keys, p2.cand_count, p2.cand_cap = tau.data_ptr(), cand.data_ptr(), cand_count.data_ptr(), cap
     N.check(L.ctl_dist_pass(qp.ptr, nq, gp.ptr, ng, qp.d, qp.flags, C.byref(p2), s()))
-    N.check(L.ctl_sort_key_rows(cand.data_ptr(), cand_count.data_ptr(), nq, cap.value, s()))
-    N.check(L.ctl_topk_emit(cand.data_ptr(), cand_count.data_ptr(), nq, cap.value, k, idx.data_ptr(),
-                            dst.data_ptr(), ovf.data_ptr(), s()))
-    ranks, pack = _finalize(buckets, pos_count, nq, max_pos, ovf)
-    return {"idx": idx, "dst": dst, "ranks": ranks, "pack": pack, "subset": work is not None and not emit_all.value,
-            "keep": (gmin, tau, cand, zeros, pos_keys, buckets, work, gmap)}
+    rows = ()
+    if k is not None:
+        N.check(L.ctl_sort_key_rows(cand.data_ptr(), cand_count.data_ptr(), nq, cap, s()))
+    if world > 1:
+        ex.sum_(buckets)
+        ex.max_(ovf)
+        if k is not None:
+            best = ex.rows(cand[:, :k_loc].contiguous(), [nq] * world)
+            rows = merge_topk_keys(best.view(world, nq, k_loc).permute(1, 0, 2).reshape(nq, world * k_loc),
+                                   int(min(k, world * k_loc)))
+    elif k is not None:
+        idx = torch.empty(nq, k_loc, dtype=torch.int64, device=dev)
+        dst = torch.empty(nq, k_loc, dtype=torch.float32, device=dev)
+        N.check(L.ctl_topk_emit(cand.data_ptr(), cand_count.data_ptr(), nq, cap, k_loc, idx.data_ptr(), dst.data_ptr(),
+                                ovf.data_ptr(), s()))
+        rows = (idx, dst)
+    ranks, pack = _finalize(buckets, thr_count, nq, mp, ovf)
+    return {"rows": rows, "ranks": ranks, "pack": pack, "keep": keep + [pos_keys, thr, sort_count, buckets, work, gmap]}
 
 
-def _topk_and_eval_finish(out, h, qp, gp, k, q_pids, g_pids, q_camids, g_camids, max_rank, respect_camids, ids):
-    """host half of topk_and_eval: overflow handling, back to the caller's query order, eval_func's final reductions."""
-    nq, ng = qp.n, gp.n
-    idx, dst, ranks = out["idx"], out["dst"], out["ranks"]
-    ap_h, first_h, cnt_h, ovf_h = _unpack(h, nq)
-    if ovf_h and out["subset"]:
-        # the looser threshold let more rows through than the candidate list holds: threshold from every tile
-        return topk_and_eval(qp, gp, k, q_pids, g_pids, q_camids, g_camids, max_rank, respect_camids, ids, tile_lists=False)
-    if ovf_h:
-        raise OverflowError("a device-side list overflowed (exact ties at the k-th distance, or max_pos)")
-    inv_d, inv_h = _query_inverse(qp)
-    if inv_h is not None:  # back to the caller's query order
-        idx, dst, ranks = idx.index_select(0, inv_d), dst.index_select(0, inv_d), ranks.index_select(0, inv_d)
-        ap_h, first_h, cnt_h = ap_h[inv_h], first_h[inv_h], cnt_h[inv_h]
-    return idx, dst, _aggregate(ranks, ap_h, cnt_h, np.asarray(q_pids), ng, max_rank, first=first_h)
+def _streamed(ex, qp: Planes, gp: Planes, ids: "EncodedIds", k: Optional[int], q_pids, num_g: int, max_rank: int,
+              g_index_offset: int = 0, tile_lists: Optional[bool] = None) -> tuple:
+    """_streamed_enqueue, ONE read-back and _eval_result: (idx, dist, EvalResult) in the caller's query order, or
+    (EvalResult,) when k is None.  `tile_lists` defaults to both planes being stored in identity order.  When the looser
+    threshold of a tile-list pass 1 lets more rows through than a candidate list holds, the call runs once more with the
+    threshold from every tile; the overflow flag is MAX-reduced and `tile_lists` is the caller's, so every rank retries
+    together."""
+    if tile_lists is None:
+        tile_lists = _tile_lists_enabled(qp, gp)
+    with torch.cuda.device(qp.buf.device):
+        out = _streamed_enqueue(ex, qp, gp, ids, k, tile_lists, g_index_offset)
+        h = out["pack"].cpu().numpy()
+        if h[qp.n, 0] and tile_lists and k is not None:
+            return _streamed(ex, qp, gp, ids, k, q_pids, num_g, max_rank, g_index_offset, tile_lists=False)
+        msg = (_OVF_POS if k is None else _OVF_TOPK) + (" on some rank" if ex.world > 1 else "")
+        return _eval_result(out["ranks"], h, q_pids, num_g, max_rank, msg, qp, out["rows"])
 
 
 class TopkEvalSession:
@@ -648,18 +701,17 @@ class TopkEvalSession:
                  respect_camids: bool = False, dist: str = "euclidean", normalize: bool = False):
         N.require_cuda(gallery)
         dev = gallery.device
-        self.dev, self.k, self.max_rank, self.respect = dev, int(k), max_rank, respect_camids
-        self.args = (q_pids, g_pids, q_camids, g_camids)
-        self.dist, self.normalize = dist, normalize
+        self.dev, self.k, self.max_rank, self.q_pids = dev, int(k), max_rank, q_pids
         self.gp = build_planes(gallery, dist, normalize)
         self.ids = encode_ids(q_pids, g_pids, q_camids, g_camids, respect_camids, dev)
         self.q = torch.empty(num_query, gallery.shape[1], dtype=torch.float32, device=dev)  # static input of the graph
         self.host = torch.empty(num_query + 1, 3, dtype=torch.float64).pin_memory()
         self.done = torch.cuda.Event()
+        one = ShardExchange(None)
 
         def enqueue():
             qp = build_planes(self.q, dist, normalize)
-            out = _topk_and_eval_enqueue(qp, self.gp, self.k, self.ids, False)
+            out = _streamed_enqueue(one, qp, self.gp, self.ids, self.k, False)
             self.host.copy_(out["pack"], non_blocking=True)
             out["qp"] = qp
             return out
@@ -688,8 +740,8 @@ class TopkEvalSession:
             self.done.record()
             self.done.synchronize()
         out = self.out
-        return _topk_and_eval_finish(out, self.host.numpy(), out["qp"], self.gp, self.k, *self.args, self.max_rank,
-                                     self.respect, self.ids)
+        return _eval_result(out["ranks"], self.host.numpy(), self.q_pids, self.gp.n, self.max_rank, _OVF_TOPK, out["qp"],
+                            out["rows"])
 
 
 def encode_ids_sharded(q_pids, g_pids_local, q_camids, g_camids_local, device, group, q_order=None,
@@ -697,104 +749,25 @@ def encode_ids_sharded(q_pids, g_pids_local, q_camids, g_camids_local, device, g
     """Identity arrays of (all queries, THIS rank's gallery shard) for topk_and_eval_sharded: raw integer pids (every
     rank must agree on the labelling, so no np.unique), camera ids in [0, 64); `max_pos` = the largest number of
     same-pid rows of any shard (one MAX all-reduce, done once per validation set)."""
-    import torch.distributed as dist
-
     ids = encode_ids(q_pids, g_pids_local, q_camids, g_camids_local, False, device, global_labels=True, q_order=q_order,
                      g_order=g_order)
-    mp = torch.tensor([ids.max_pos], device=device, dtype=torch.int64)
-    dist.all_reduce(mp, op=dist.ReduceOp.MAX, group=group)
-    ids.max_pos = int(mp.item())
+    ids.max_pos = _max_over_ranks(ShardExchange(group), ids.max_pos, device)
     return ids
 
 
 def topk_and_eval_sharded(qp: Planes, gp_local: Planes, k: int, ids: EncodedIds, q_pids, g_index_offset: int,
                           total_gallery: int, group, max_rank: int = 50, tile_lists: Optional[bool] = None):
     """BASELINE config 5: topk_and_eval with the GALLERY AXIS SHARDED over the ranks of `group` (queries replicated:
-    all-gather them once before building `qp`).  Every rank runs the two tensor-core passes over its own shard; the
-    exchange steps are (utils/reid_metric.py:112-136 + utils/eval_reid.py:25-92 semantics, bit-identical to one GPU):
+    all-gather them once before building `qp`).  Every rank runs the two tensor-core passes over its own shard, with
+    the exchanges of _streamed_enqueue between them (utils/reid_metric.py:112-136 + utils/eval_reid.py:25-92 semantics,
+    bit-identical to one GPU):
       after pass 1: all-gather of the positives' (distance, index) keys [nq, max_pos] -> one sorted threshold list
       after pass 2: all-reduce(sum) of the integer bucket counts; all-gather of each rank's k best packed keys and a
                     k-way merge by integer key order (world-size independent).
+    `ids` comes from encode_ids_sharded, so max_pos is the same on every rank; every shard must hold at least k rows.
     Returns (idx [nq, k] global gallery rows, dist [nq, k], EvalResult) on every rank."""
-    import ctypes as C
-
-    import torch.distributed as dist
-
-    L = N.lib()
-    dev = qp.buf.device
-    world = dist.get_world_size(group)
-    nq, ng = qp.n, gp_local.n
-    k_loc = int(min(k, ng))
-    emit_all, n_groups, merge, cap = C.c_int32(), C.c_int32(), C.c_int32(), C.c_int32()
-    N.check(L.ctl_topk_plan(ng, k_loc, C.byref(emit_all), C.byref(n_groups), C.byref(merge), C.byref(cap)))
-    mp_l = ids.max_pos            # per-shard capacity (same on every rank)
-    mp = mp_l * world             # capacity of the merged threshold list
-    gmin = torch.empty(nq, n_groups.value, dtype=torch.float32, device=dev)
-    tau = torch.empty(nq, dtype=torch.float32, device=dev)
-    cand = torch.empty(nq, cap.value, dtype=torch.int64, device=dev)
-    zeros = torch.zeros(2 * nq + 1, dtype=torch.int32, device=dev)
-    cand_count, pos_count, ovf = zeros[:nq], zeros[nq: 2 * nq], zeros[2 * nq:]
-    pos_keys = torch.empty(nq, mp_l, dtype=torch.int64, device=dev)
-    buckets = torch.zeros(nq, mp + 1, dtype=torch.int32, device=dev)
-    s = N.stream_ptr
-    if tile_lists is None:
-        tile_lists = _tile_lists_enabled(qp, gp_local)
-    gmap = _g_index_map(gp_local, g_index_offset)  # pid-sorted shard: keys carry the GLOBAL gallery row
-    idp = dict(q_pid=ids.q_pid.data_ptr(), q_cam=ids.q_cam.data_ptr(), g_pid=ids.g_pid.data_ptr(),
-               g_cammask=ids.g_mask.data_ptr(), overflow=ovf.data_ptr(), g_index_offset=g_index_offset,
-               g_index_map=N.ptr(gmap))
-    with torch.cuda.device(dev):
-        p1 = N.PassDesc(pos_keys=pos_keys.data_ptr(), pos_count=pos_count.data_ptr(), max_pos=mp_l, **idp)
-        if not emit_all.value:
-            p1.gmin = gmin.data_ptr()
-        work = None
-        if tile_lists:  # pid-sorted shard: pass 1 runs the tiles that can hold a positive + a subset for tau (topk_and_eval)
-            stride = 0 if emit_all.value else L.ctl_dist_subset_stride(ng, k_loc)
-            if emit_all.value or stride > 1:
-                work = _tile_list(qp, gp_local, ids, stride)
-        if work is not None:
-            p1.tile_list = work.data_ptr()
-            if not emit_all.value:
-                N.check(L.ctl_fill_f32(gmin.data_ptr(), gmin.numel(), float("inf"), s()))
-        N.check(L.ctl_dist_pass(qp.ptr, nq, gp_local.ptr, ng, qp.d, qp.flags, C.byref(p1), s()))
-        if emit_all.value:
-            N.check(L.ctl_fill_f32(tau.data_ptr(), nq, float("inf"), s()))
-        else:
-            N.check(L.ctl_select_tau(gmin.data_ptr(), nq, n_groups.value, merge.value, k_loc, tau.data_ptr(), s()))
-        # exchange 1: every rank's positives, unused slots = the largest key, so ONE row sort packs and orders them
-        col = torch.arange(mp_l, device=dev)[None, :]
-        masked = torch.where(col < pos_count[:, None].clamp(max=mp_l), pos_keys, torch.full_like(pos_keys, -1))
-        g_keys = torch.empty(world, nq, mp_l, dtype=torch.int64, device=dev)
-        g_cnt = torch.empty(world, nq, dtype=torch.int32, device=dev)
-        dist.all_gather_into_tensor(g_keys, masked, group=group)
-        dist.all_gather_into_tensor(g_cnt, pos_count.contiguous(), group=group)
-        thr = g_keys.permute(1, 0, 2).reshape(nq, mp).contiguous()
-        thr_count = g_cnt.sum(0, dtype=torch.int32)
-        full = torch.full((nq,), mp, dtype=torch.int32, device=dev)
-        N.check(L.ctl_sort_key_rows(thr.data_ptr(), full.data_ptr(), nq, mp, s()))
-        p2 = N.PassDesc(tau=tau.data_ptr(), cand_keys=cand.data_ptr(), cand_count=cand_count.data_ptr(),
-                        cand_cap=cap.value, thr_keys=thr.data_ptr(), thr_count=thr_count.data_ptr(),
-                        buckets=buckets.data_ptr(), max_pos=mp, **idp)
-        N.check(L.ctl_dist_pass(qp.ptr, nq, gp_local.ptr, ng, qp.d, qp.flags, C.byref(p2), s()))
-        N.check(L.ctl_sort_key_rows(cand.data_ptr(), cand_count.data_ptr(), nq, cap.value, s()))
-        # exchange 2: bucket counts (integers) and the k best keys of every shard
-        dist.all_reduce(buckets, op=dist.ReduceOp.SUM, group=group)
-        best = cand[:, :k_loc].contiguous()
-        g_best = torch.empty(world, nq, k_loc, dtype=torch.int64, device=dev)
-        dist.all_gather_into_tensor(g_best, best, group=group)
-        dist.all_reduce(ovf, op=dist.ReduceOp.MAX, group=group)
-        idx, dst = merge_topk_keys(g_best.permute(1, 0, 2).reshape(nq, world * k_loc), int(min(k, world * k_loc)))
-        ranks, ap_h, first_h, cnt_h, ovf_h = _finalize_and_read_back(buckets, thr_count, nq, mp, ovf)
-        if ovf_h and tile_lists and not emit_all.value:  # (the flag is MAX-reduced: every rank takes this branch together)
-            return topk_and_eval_sharded(qp, gp_local, k, ids, q_pids, g_index_offset, total_gallery, group, max_rank,
-                                         tile_lists=False)
-        inv_d, inv_h = _query_inverse(qp)
-        if inv_h is not None:  # back to the caller's query order
-            idx, dst, ranks = idx.index_select(0, inv_d), dst.index_select(0, inv_d), ranks.index_select(0, inv_d)
-            ap_h, first_h, cnt_h = ap_h[inv_h], first_h[inv_h], cnt_h[inv_h]
-    if ovf_h:
-        raise OverflowError("a device-side list overflowed on some rank (exact ties at the k-th distance, or max_pos)")
-    return idx, dst, _aggregate(ranks, ap_h, cnt_h, np.asarray(q_pids), total_gallery, max_rank, first=first_h)
+    return _streamed(ShardExchange(group), qp, gp_local, ids, k, q_pids, total_gallery, max_rank, g_index_offset,
+                     tile_lists)
 
 
 # ----------------------------------------------------------------------------------------
@@ -811,28 +784,35 @@ def evaluate_matrix(distmat: torch.Tensor, q_pids, g_pids, q_camids, g_camids, m
     N.require_cuda(distmat)
     if distmat.dim() != 2 or distmat.dtype != torch.float32 or distmat.stride(1) != 1:
         raise ValueError("expected a [nq, ng] float32 matrix with unit column stride")
-    L = N.lib()
     dev = distmat.device
     nq, ng = distmat.shape
-    ld = distmat.stride(0)
-    ids = encode_ids(q_pids, g_pids, q_camids, g_camids, respect_camids, dev)
-    max_pos = ids.max_pos
-    pos_keys = torch.zeros(nq, max_pos, dtype=torch.int64, device=dev)
-    zeros = torch.zeros(nq + 1, dtype=torch.int32, device=dev)
-    pos_count, ovf = zeros[:nq], zeros[nq:]
-    buckets = torch.zeros(nq, max_pos + 1, dtype=torch.int32, device=dev)
-    idp = (ids.q_pid.data_ptr(), ids.q_cam.data_ptr(), ids.g_pid.data_ptr(), ids.g_mask.data_ptr(), max_pos)
+    ev = _eval_buffers(encode_ids(q_pids, g_pids, q_camids, g_camids, respect_camids, dev), nq, dev)
     with torch.cuda.device(dev):
-        s = N.stream_ptr()
-        N.check(L.ctl_eval_matrix_collect(distmat.data_ptr(), nq, ng, ld, *idp, pos_keys.data_ptr(), pos_count.data_ptr(),
-                                          ovf.data_ptr(), s))
-        N.check(L.ctl_sort_key_rows(pos_keys.data_ptr(), pos_count.data_ptr(), nq, max_pos, s))
-        N.check(L.ctl_eval_matrix_count(distmat.data_ptr(), nq, ng, ld, *idp, pos_keys.data_ptr(), pos_count.data_ptr(),
-                                        buckets.data_ptr(), s))
-        ranks, ap_h, first_h, cnt_h, ovf_h = _finalize_and_read_back(buckets, pos_count, nq, max_pos, ovf)
-    if ovf_h:
-        raise OverflowError("positives list overflowed (max_pos too small)")
-    return _aggregate(ranks, ap_h, cnt_h, np.asarray(q_pids), ng, max_rank, first=first_h)
+        _eval_matrix_rows(distmat, 0, nq, ng, distmat.stride(0), ev)
+        ranks, pack = _finalize(ev["buckets"], ev["pos_count"], nq, ev["ids"].max_pos, ev["ovf"])
+        return _eval_result(ranks, pack, q_pids, ng, max_rank)[0]
+
+
+def _eval_buffers(ids: "EncodedIds", nq: int, dev) -> dict:
+    """The zeroed buffers of the collect / sort / count steps over a materialised matrix (_eval_matrix_rows,
+    ctl_rerank_topk)."""
+    pos_keys = torch.zeros(nq, ids.max_pos, dtype=torch.int64, device=dev)
+    zeros = torch.zeros(nq + 1, dtype=torch.int32, device=dev)
+    return {"ids": ids, "pos_keys": pos_keys, "pos_count": zeros[:nq], "ovf": zeros[nq:],
+            "buckets": torch.zeros(nq, ids.max_pos + 1, dtype=torch.int32, device=dev)}
+
+
+def _eval_matrix_rows(d: torch.Tensor, q0: int, rows: int, ng: int, ld: int, ev: dict):
+    """The collect, row sort and count of eval_func over the distances `d` ([rows, ng], row stride ld) of queries
+    [q0, q0 + rows), into the rows of `ev` (_eval_buffers over all queries)."""
+    L = N.lib()
+    s = N.stream_ptr()
+    ids, mp = ev["ids"], ev["ids"].max_pos
+    idp = (ids.q_pid.data_ptr() + 4 * q0, ids.q_cam.data_ptr() + 4 * q0, ids.g_pid.data_ptr(), ids.g_mask.data_ptr(), mp)
+    pk, pc = ev["pos_keys"][q0:].data_ptr(), ev["pos_count"][q0:].data_ptr()
+    N.check(L.ctl_eval_matrix_collect(d.data_ptr(), rows, ng, ld, *idp, pk, pc, ev["ovf"].data_ptr(), s))
+    N.check(L.ctl_sort_key_rows(pk, pc, rows, mp, s))
+    N.check(L.ctl_eval_matrix_count(d.data_ptr(), rows, ng, ld, *idp, pk, pc, ev["buckets"][q0:].data_ptr(), s))
 
 
 @dataclass
@@ -890,10 +870,13 @@ def rerank(q: torch.Tensor, g: torch.Tensor, k1: int = 20, k2: int = 6, lambda_v
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
     with torch.cuda.device(dev):
         _rerank_enqueue(planes, nq, ng, k1, k2, lambda_value, out, status, ws)
-        st = int(status.item())
-    if st:
-        raise ValueError("re-ranking: a row of the distance matrix has no positive maximum (N = 1 or identical features)")
+        _check_status(status)
     return out
+
+
+def _check_status(status: torch.Tensor):
+    if int(status.item()):
+        raise ValueError("re-ranking: a row of the distance matrix has no positive maximum (N = 1 or identical features)")
 
 
 def rerank_stages(q: torch.Tensor, g: torch.Tensor, k1: int = 20, k2: int = 6, lambda_value: float = 0.3,
@@ -997,13 +980,6 @@ def _rerank_topk_enqueue(planes: Planes, nq: int, ng: int, k1: int, k2: int, lam
                                     ws.data_ptr(), ws.numel(), N.stream_ptr()))
 
 
-def _eval_buffers(ids: "EncodedIds", nq: int, dev) -> dict:
-    return {"ids": ids, "pos_keys": torch.zeros(nq, ids.max_pos, dtype=torch.int64, device=dev),
-            "pos_count": torch.zeros(nq, dtype=torch.int32, device=dev),
-            "buckets": torch.zeros(nq, ids.max_pos + 1, dtype=torch.int32, device=dev),
-            "ovf": torch.zeros(1, dtype=torch.int32, device=dev)}
-
-
 def _rerank_topk_run(q, g, k, k1, k2, lambda_value, normalize, block_rows, ids_args=None, max_rank=50):
     """ctl_rerank_topk from features; ids_args = (q_pids, g_pids, q_camids, g_camids, respect_camids) adds the
     evaluation."""
@@ -1023,15 +999,10 @@ def _rerank_topk_run(q, g, k, k1, k2, lambda_value, normalize, block_rows, ids_a
         del ws
         if ev is not None:
             ranks, pack = _finalize(ev["buckets"], ev["pos_count"], nq, ev["ids"].max_pos, ev["ovf"])
-        st = int(status.item())
-    if st:
-        raise ValueError("re-ranking: a row of the distance matrix has no positive maximum (N = 1 or identical features)")
-    if ev is None:
-        return idx, dst, None
-    ap_h, first_h, cnt_h, ovf_h = _unpack(pack.cpu().numpy(), nq)
-    if ovf_h:
-        raise OverflowError("positives list overflowed (max_pos too small)")
-    return idx, dst, _aggregate(ranks, ap_h, cnt_h, np.asarray(ids_args[0]), ng, max_rank, first=first_h)
+        _check_status(status)
+        if ev is None:
+            return idx, dst, None
+        return (idx, dst) + _eval_result(ranks, pack, ids_args[0], ng, max_rank)
 
 
 def rerank_topk(q: torch.Tensor, g: torch.Tensor, k: int, k1: int = 20, k2: int = 6, lambda_value: float = 0.3,
@@ -1063,16 +1034,10 @@ def rerank_blocked_stages(q: torch.Tensor, g: torch.Tensor, k: int, k1: int = 20
     invert, _jaccard_rows / _topk_rows), keeping every intermediate that is linear in N: {rank [N, kr], rowmax [N],
     v_idx / v_val / v_cnt, q_idx / q_val / q_cnt, col_ptr, inv_row, inv_val, idx / dist [Q, k], status, plan, planes,
     block_rows}, plus `eval` (the EvalResult) when identities are given.  For tests and inspection: `events`, a list,
-    receives (name, CUDA event) pairs recorded after each sweep ("A", "B", "qe_invert", "C")."""
-    planes = _rerank_inputs(q, g, normalize)
-    nq, ng = q.shape[0], g.shape[0]
-    n = nq + ng
-    k, R, _ = _rerank_topk_args(nq, ng, planes.d, k1, k2, k, block_rows)
-    dev = q.device
-    r = _rerank_tables(planes, nq, ng, k, k1, k2, lambda_value, R)
-    ev = None
-    if q_pids is not None:
-        ev = _eval_buffers(encode_ids(q_pids, g_pids, q_camids, g_camids, respect_camids, dev), nq, dev)
+    receives (name, CUDA event) pairs recorded before the sweeps ("start") and after each ("A", "B", "qe_invert", "C").
+    The one-rank case of the sharded protocol (_rerank_sharded); like rerank(), raises ValueError when a row of the
+    distance matrix has no positive maximum."""
+    ids_args = None if q_pids is None else (q_pids, g_pids, q_camids, g_camids, respect_camids)
 
     def mark(name):
         if events is not None:
@@ -1080,25 +1045,8 @@ def rerank_blocked_stages(q: torch.Tensor, g: torch.Tensor, k: int, k1: int = 20
             e.record()
             events.append((name, e))
 
-    with torch.cuda.device(dev):
-        blk = torch.empty(min(R, n) * n, dtype=torch.float32, device=dev)
-        mark("start")
-        _rerank_sweep_a(r, 0, n, blk)
-        mark("A")
-        _rerank_sweep_b(r, 0, n, blk, k1, k2)
-        mark("B")
-        _rerank_qe_invert(r, k1, k2)
-        mark("qe_invert")
-        del blk
-        _rerank_sweep_c(r, 0, nq, ev)
-        mark("C")
-        if ev is not None:
-            ranks, ap_h, first_h, cnt_h, ovf_h = _finalize_and_read_back(ev["buckets"], ev["pos_count"], nq,
-                                                                          ev["ids"].max_pos, ev["ovf"])
-            if ovf_h:
-                raise OverflowError("positives list overflowed (max_pos too small)")
-            r["eval"] = _aggregate(ranks, ap_h, cnt_h, np.asarray(q_pids), ng, max_rank, first=first_h)
-    return r
+    return _rerank_sharded(ShardExchange(None), q, g, k, k1, k2, lambda_value, normalize, block_rows, ids_args, max_rank,
+                           mark)
 
 
 def _rerank_tables(planes: Planes, nq: int, ng: int, k: int, k1: int, k2: int, lambda_value: float, R: int) -> dict:
@@ -1183,13 +1131,7 @@ def _rerank_sweep_c(r: dict, lo: int, hi: int, ev: Optional[dict]):
         out = rerank_final_rows(r, q0, rows, out=fin)
         N.check(L.ctl_rerank_topk_rows(out.data_ptr(), q0, rows, ng, ng, k, r["idx"].data_ptr(), r["dist"].data_ptr(), s))
         if ev is not None:
-            ids, mp = ev["ids"], ev["ids"].max_pos
-            idp = (ids.q_pid.data_ptr() + 4 * q0, ids.q_cam.data_ptr() + 4 * q0, ids.g_pid.data_ptr(),
-                   ids.g_mask.data_ptr(), mp)
-            pk, pc = ev["pos_keys"][q0:].data_ptr(), ev["pos_count"][q0:].data_ptr()
-            N.check(L.ctl_eval_matrix_collect(out.data_ptr(), rows, ng, ng, *idp, pk, pc, ev["ovf"].data_ptr(), s))
-            N.check(L.ctl_sort_key_rows(pk, pc, rows, mp, s))
-            N.check(L.ctl_eval_matrix_count(out.data_ptr(), rows, ng, ng, *idp, pk, pc, ev["buckets"][q0:].data_ptr(), s))
+            _eval_matrix_rows(out, q0, rows, ng, ng, ev)
 
 
 def rerank_final_rows(r: dict, q0: int, rows: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -1227,52 +1169,6 @@ def row_shares(n: int, world: int) -> list:
     return [(j * int(n) // world, (j + 1) * int(n) // world) for j in range(world)]
 
 
-class ShardExchange:
-    """The exchanges of the sharded re-ranking, over the ranks of a torch.distributed group (None: one rank, nothing is
-    exchanged).  Every rank calls each method in the same order."""
-
-    def __init__(self, group=None):
-        import torch.distributed as dist
-
-        self.group = group
-        self.world = 1 if group is None else dist.get_world_size(group)
-        self.rank = 0 if group is None else dist.get_rank(group)
-
-    def objects(self, obj) -> list:
-        """Every rank's picklable `obj`, in rank order."""
-        import torch.distributed as dist
-
-        if self.group is None:
-            return [obj]
-        out = [None] * self.world
-        dist.all_gather_object(out, obj, group=self.group)
-        return out
-
-    def rows(self, t: torch.Tensor, counts: Sequence[int]) -> torch.Tensor:
-        """The concatenation over ranks of each rank's `t` (counts[j] rows on rank j): shards padded to the largest,
-        all-gathered, trimmed."""
-        import torch.distributed as dist
-
-        if self.group is None:
-            return t
-        m = max(counts)
-        pad = t.new_zeros((m,) + tuple(t.shape[1:]))
-        pad[: t.shape[0]] = t
-        out = t.new_empty((self.world * m,) + tuple(t.shape[1:]))
-        dist.all_gather_into_tensor(out, pad, group=self.group)
-        if all(c == m for c in counts):
-            return out
-        return torch.cat([out[j * m: j * m + c] for j, c in enumerate(counts)])
-
-    def max_(self, t: torch.Tensor) -> torch.Tensor:
-        """In place: the element-wise maximum over ranks."""
-        import torch.distributed as dist
-
-        if self.group is not None:
-            dist.all_reduce(t, op=dist.ReduceOp.MAX, group=self.group)
-        return t
-
-
 def _local_error(q_local, g_local, ids_args):
     """What is wrong with this rank's own arguments, as (exception class, message), or None."""
     try:
@@ -1290,12 +1186,13 @@ def _local_error(q_local, g_local, ids_args):
 
 
 def _rerank_sharded(ex, q_local: torch.Tensor, g_local: torch.Tensor, k: int, k1: int, k2: int, lambda_value: float,
-                    normalize: bool, block_rows: Optional[int], ids_args=None, max_rank: int = 50) -> dict:
+                    normalize: bool, block_rows: Optional[int], ids_args=None, max_rank: int = 50, mark=None) -> dict:
     """The sharded protocol of rerank_topk_sharded / rerank_topk_and_eval_sharded over the exchange `ex` (ShardExchange,
-    or a stand-in with its methods).  ids_args = (q_pids of all queries, this rank's g_pids, q_camids of all queries, this
-    rank's g_camids, respect_camids) adds the evaluation.  Returns the gathered tables of rerank_blocked_stages (rank,
-    rowmax, v_*, q_*, col_ptr, inv_*, idx, dist, status, plan, planes, block_rows; `eval` with identities), the same on
-    every rank."""
+    or a stand-in with its methods); with ShardExchange(None), rerank_blocked_stages.  ids_args = (q_pids of all queries,
+    this rank's g_pids, q_camids of all queries, this rank's g_camids, respect_camids) adds the evaluation.  `mark(name)`,
+    if given, is called on the device's stream before the sweeps ("start") and after each ("A", "B", "qe_invert", "C").
+    Returns the gathered tables of rerank_blocked_stages (rank, rowmax, v_*, q_*, col_ptr, inv_*, idx, dist, status,
+    plan, planes, block_rows; `eval` with identities), the same on every rank."""
     # 1. shard sizes, identities and local errors in ONE exchange; then every rank checks the same global arguments and
     #    raises the same error before any data is exchanged
     err = _local_error(q_local, g_local, ids_args)
@@ -1336,15 +1233,19 @@ def _rerank_sharded(ex, q_local: torch.Tensor, g_local: torch.Tensor, k: int, k1
     lo, hi = shares[ex.rank]
     qlo, qhi = q_shares[ex.rank]
     counts, q_counts = [b - a for a, b in shares], [b - a for a, b in q_shares]
+    mark = mark or (lambda name: None)
     with torch.cuda.device(dev):
         # 3. sweep A on this rank's rows -> the whole rank table and row maxima
         blk = torch.empty(min(R, hi - lo) * n, dtype=torch.float32, device=dev)
+        mark("start")
         _rerank_sweep_a(r, lo, hi, blk)
+        mark("A")
         r["rank"] = ex.rows(r["rank"][lo:hi], counts)
         r["rowmax"] = ex.rows(r["rowmax"][lo:hi], counts)
         ex.max_(r["status"])
         # 4. sweep B on the same rows -> the whole V
         _rerank_sweep_b(r, lo, hi, blk, k1, k2)
+        mark("B")
         del blk
         for key in ("v_idx", "v_val", "v_cnt"):
             r[key] = ex.rows(r[key][lo:hi], counts)
@@ -1352,8 +1253,10 @@ def _rerank_sharded(ex, q_local: torch.Tensor, g_local: torch.Tensor, k: int, k1
             r.update(q_idx=r["v_idx"], q_val=r["v_val"], q_cnt=r["v_cnt"])
         # 5. query expansion and the inverted index, whole, on every rank
         _rerank_qe_invert(r, k1, k2)
+        mark("qe_invert")
         # 6. sweep C on this rank's queries against the whole gallery, then the per-query results of every rank
         _rerank_sweep_c(r, qlo, qhi, ev)
+        mark("C")
         r["idx"] = ex.rows(r["idx"][qlo:qhi], q_counts)
         r["dist"] = ex.rows(r["dist"][qlo:qhi], q_counts)
         if ev is not None:
@@ -1366,15 +1269,9 @@ def _rerank_sharded(ex, q_local: torch.Tensor, g_local: torch.Tensor, k: int, k1
                 pack = torch.empty(1, 3, dtype=torch.float64, device=dev)
             ranks = ex.rows(ranks, q_counts)
             pack = torch.cat([ex.rows(pack[: qhi - qlo], q_counts), ev["ovf"].double().expand(1, 3)])
-            h = pack.cpu().numpy()
-        st = int(r["status"].item())
-    if st:
-        raise ValueError("re-ranking: a row of the distance matrix has no positive maximum (N = 1 or identical features)")
-    if ev is not None:
-        ap_h, first_h, cnt_h, ovf_h = _unpack(h, nq)
-        if ovf_h:
-            raise OverflowError("positives list overflowed (max_pos too small)")
-        r["eval"] = _aggregate(ranks, ap_h, cnt_h, np.asarray(q_pids), ng, max_rank, first=first_h)
+        _check_status(r["status"])
+        if ev is not None:
+            r["eval"] = _eval_result(ranks, pack, q_pids, ng, max_rank)[0]
     return r
 
 

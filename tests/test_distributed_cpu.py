@@ -1,7 +1,8 @@
 """CPU, world_size 2, gloo: the host-side logic of the sharded (N > 1) retrieval path --
-per-shard top-k merge under the canonical (distance, index) order, all-gather of the
-positives' keys, all-reduce of the integer bucket counts -- with the device kernels emulated
-in numpy from the oracle's distance matrix."""
+per-shard top-k merge under the canonical (distance, index) order, exchange 1 of the streamed
+passes (retrieval._gather_keys over ShardExchange: every rank's positives' keys, unused slots
+masked), the all-reduce of the integer bucket counts (ShardExchange.sum_) -- with the device
+kernels (and the row sort) emulated in numpy from the oracle's distance matrix."""
 import os
 import socket
 
@@ -57,13 +58,15 @@ def _worker(rank, world, port, out_q):
     junk = same & (gc[None, :] == cams[:nq, None])
     pos = same & ~junk
     max_pos = int(np.bincount(pids[nq:]).max())
-    keys = np.zeros((nq, max_pos), dtype=np.uint64)
+    keys = np.full((nq, max_pos), 12345, dtype=np.uint64)  # unused slots: whatever the collect left there
     cnt = pos.sum(1).astype(np.int32)
     allk = _key(Dl, np.broadcast_to(shard[None, :], Dl.shape))
     for q in range(nq):
         keys[q, : cnt[q]] = allk[q][pos[q]]
-    gk, gcnt = R._allgather_keys(torch.from_numpy(keys.view(np.int64)), torch.from_numpy(cnt), max_pos, None)
-    gk = gk.numpy().view(np.uint64)
+    ex = R.ShardExchange(dist.group.WORLD)
+    gk, gcnt = R._gather_keys(ex, torch.from_numpy(keys.view(np.int64)), torch.from_numpy(cnt))
+    ok_shape = tuple(gk.shape) == (nq, world * max_pos)
+    gk = np.sort(gk.numpy().view(np.uint64), axis=1)  # ctl_sort_key_rows over the whole row: unused slots sort last
     gcnt = gcnt.numpy()
     buckets = np.zeros((nq, max_pos + 1), dtype=np.int32)
     for q in range(nq):
@@ -72,9 +75,7 @@ def _worker(rank, world, port, out_q):
         kept = allk[q][~junk[q]]
         j = np.searchsorted(thr, kept, side="right")
         np.add.at(buckets[q], j[j < gcnt[q]], 1)
-    tb = torch.from_numpy(buckets)
-    dist.all_reduce(tb)
-    buckets = tb.numpy()
+    buckets = ex.sum_(torch.from_numpy(buckets)).numpy()
     ranks = np.full((nq, max_pos), -1, dtype=np.int32)
     ap = np.full(nq, np.nan)
     for q in range(nq):
@@ -86,12 +87,13 @@ def _worker(rank, world, port, out_q):
     res = R._aggregate(ranks, ap, gcnt, pids[:nq], ng, 50)
     cmc, mAP, topk, single = O.eval_func(O.rank_indices(D), pids[:nq], pids[nq:], cams[:nq], cams[nq:], 50)
     ok_eval = np.array_equal(res.cmc, cmc) and abs(res.mAP - mAP) < 1e-12 and np.allclose(res.all_topk, topk)
+    ok_eval = ok_eval and ok_shape
     if rank == 0:
         out_q.put((ok_topk, ok_eval))
     dist.destroy_process_group()
 
 
-def test_sharded_merge_world2_gloo():
+def test_sharded_merge_and_key_exchange_world2_gloo():
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
     port = _free_port()

@@ -62,6 +62,8 @@ def _exchange_worker(rank, world, port, out_q):
     out["objects"] = ex.objects({"r": rank})
     m = torch.tensor([rank, 1 - rank], dtype=torch.int32)
     out["max"] = ex.max_(m).numpy()
+    t = torch.tensor([[rank + 1, 10 * rank], [-3, 7]], dtype=torch.int32)
+    out["sum"] = ex.sum_(t).numpy()
     out_q.put((rank, out))
     dist.destroy_process_group()
 
@@ -75,6 +77,7 @@ def test_padded_all_gather_of_uneven_shards_world2_gloo():
         assert np.array_equal(out["even"], np.concatenate([np.arange(4), 2 * np.arange(4)]))
         assert out["objects"] == [{"r": 0}, {"r": 1}]
         assert np.array_equal(out["max"], [1, 1])
+        assert np.array_equal(out["sum"], [[3, 10], [-6, 14]])
 
 
 class _Spy(R.ShardExchange):
@@ -89,6 +92,10 @@ class _Spy(R.ShardExchange):
     def max_(self, t):
         self.data_calls += 1
         return super().max_(t)
+
+    def sum_(self, t):
+        self.data_calls += 1
+        return super().sum_(t)
 
 
 def _reject_worker(rank, world, port, out_q):

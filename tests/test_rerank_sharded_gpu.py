@@ -2,16 +2,16 @@
 rerank_topk_and_eval_sharded) against the one-GPU path on the same device, with torch.equal throughout.
 
 W ranks are emulated on one device: each runs the protocol in a thread of its own, one at a time, and the exchange
-stand-in hands the parts over (`_Shards`).  The query and gallery features are split unevenly over the ranks, some ranks
-holding none; the row shares of the sweeps put boundaries inside the queries and, at W = 2 with Q = G, exactly at the
-query / gallery boundary.
+stand-in hands the parts over (shard_exchange.Shards).  The query and gallery features are split unevenly over the
+ranks, some ranks holding none; the row shares of the sweeps put boundaries inside the queries and, at W = 2 with
+Q = G, exactly at the query / gallery boundary.
 """
 import socket
-import threading
 
 import numpy as np
 import pytest
 import torch
+from shard_exchange import Shards
 
 from ctl_b200 import retrieval as R
 from oracle import ctl_oracle as O
@@ -19,76 +19,6 @@ from oracle import ctl_oracle as O
 pytestmark = pytest.mark.gpu
 
 K1, K2, LAM = 20, 6, 0.3
-_EMPTY = object()
-
-
-class _Shards:
-    """W ranks of the protocol on one device, in W threads that run one at a time: a rank runs until its next exchange,
-    leaves its part there and hands over to the next rank; the exchange returns once every rank's part is in."""
-
-    def __init__(self, world):
-        self.world = world
-        self.cv = threading.Condition()
-        self.turn = 0
-        self.slots = []
-
-    def run(self, fn):
-        """fn(exchange) on every rank; returns the per-rank results, re-raising the first rank's error."""
-        out, errs = [None] * self.world, [None] * self.world
-
-        def worker(rank):
-            with self.cv:
-                self.cv.wait_for(lambda: self.turn == rank)
-            try:
-                out[rank] = fn(_Exchange(self, rank))
-            except BaseException as e:  # noqa: BLE001 -- re-raised below
-                errs[rank] = e
-            finally:
-                with self.cv:
-                    self.turn = (rank + 1) % self.world
-                    self.cv.notify_all()
-
-        threads = [threading.Thread(target=worker, args=(r,)) for r in range(self.world)]
-        for t in threads:
-            t.start()
-        for t in threads:
-            t.join()
-        self.errors = errs
-        for e in errs:
-            if e is not None:
-                raise e
-        return out
-
-
-class _Exchange:
-    def __init__(self, shards, rank):
-        self.s, self.rank, self.world, self.calls = shards, rank, shards.world, 0
-
-    def _all(self, part):
-        s = self.s
-        with s.cv:
-            if len(s.slots) <= self.calls:
-                s.slots.append([_EMPTY] * self.world)
-            slot = s.slots[self.calls]
-            slot[self.rank] = part
-            self.calls += 1
-            s.turn = (self.rank + 1) % self.world
-            s.cv.notify_all()
-            if not s.cv.wait_for(lambda: s.turn == self.rank and all(p is not _EMPTY for p in slot), timeout=600):
-                raise RuntimeError(f"rank {self.rank}: exchange {self.calls - 1} never completed")
-            return list(slot)
-
-    def objects(self, obj):
-        return self._all(obj)
-
-    def rows(self, t, counts):
-        parts = self._all(t)
-        assert [p.shape[0] for p in parts] == list(counts)
-        return torch.cat(parts)
-
-    def max_(self, t):
-        parts = self._all(t.clone())
-        return t.copy_(torch.stack(parts).amax(0))
 
 
 def _cuts(n, world, seed):
@@ -110,7 +40,7 @@ def _sharded(world, q, g, k, ids=None, respect=False, k1=K1, k2=K2, lam=LAM, nor
         return R._rerank_sharded(ex, q[qc[j]: qc[j + 1]], g[gc[j]: gc[j + 1]], k, k1, k2, lam, normalize, block_rows,
                                  ids_args)
 
-    return _Shards(world).run(fn)
+    return Shards(world).run(fn)
 
 
 def _assert_eval_equal(a, b):
@@ -255,7 +185,7 @@ def test_status_error_raises_on_every_rank():
     """Identical features: every row maximum is 0."""
     q = torch.ones(20, 64, device="cuda")
     g = torch.ones(50, 64, device="cuda")
-    shards = _Shards(3)
+    shards = Shards(3)
     with pytest.raises(ValueError, match="no positive maximum"):
         shards.run(lambda ex: R._rerank_sharded(ex, q[ex.rank * 5: ex.rank * 5 + 5 + 5 * (ex.rank == 2)],
                                                  g[ex.rank * 10: ex.rank * 10 + 10 + 20 * (ex.rank == 2)],
@@ -297,6 +227,11 @@ class _Recorder:
         self.log.append(t.cpu())
         return t
 
+    def sum_(self, t):
+        self.ex.sum_(t)
+        self.log.append(t.cpu())
+        return t
+
 
 class _Replay:
     """One rank alone: every exchange returns what the recorded run got."""
@@ -315,6 +250,9 @@ class _Replay:
         return self._next().to(t.device)
 
     def max_(self, t):
+        return t.copy_(self._next())
+
+    def sum_(self, t):
         return t.copy_(self._next())
 
 
@@ -348,7 +286,7 @@ def test_peak_allocation_per_rank():
             ex = rec["ex"] = _Recorder(ex)
         return R._rerank_sharded(ex, *shard_args(ex.rank))["idx"]
 
-    full = _Shards(world).run(fn)[0]
+    full = Shards(world).run(fn)[0]
     torch.cuda.synchronize()
     torch.cuda.empty_cache()
     base = torch.cuda.memory_allocated()

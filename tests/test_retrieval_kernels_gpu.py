@@ -10,13 +10,15 @@ comparison.  Here every kernel of csrc/retrieval.cu meets a numpy float64 / inte
                               rows, CTL_DIST_SQRT at identical rows and CTL_FLAG_NORMALIZE;
   C. the merged-group plan    galleries above 131 072 rows (ctl_topk_plan: merge > 1);
   D. select_tau / sort_key_rows / topk_emit / eval_finalize / dist_worklist, each against numpy;
-  E. the gallery-sharded protocol of include/ctl_b200.h on ONE device (g_index_offset != 0, g_index_map + offset).
+  E. the gallery-sharded protocol of include/ctl_b200.h on ONE device (g_index_offset != 0, g_index_map + offset),
+     by hand and through retrieval's sharded streamed passes with W = 2, 3 ranks emulated (shard_exchange.Shards).
 """
 import ctypes as C
 
 import numpy as np
 import pytest
 import torch
+from shard_exchange import Shards
 
 from oracle import ctl_oracle as O
 
@@ -516,13 +518,15 @@ def sharded_problem(R):
     return q, gal, pids, cams, k, qp, base
 
 
-def _same_as_unsharded(R, base, idx, dst, ranks, ap, cnt, q_pids, ng):
+def _same_as_unsharded(base, idx, dst, res):
+    """idx / dst (None: not computed) and the EvalResult equal the unsharded run's; the merged threshold list may be
+    wider than the unsharded one, so `ranks` may have more columns, all -1."""
     b_idx, b_dst, b_res = base
-    assert torch.equal(idx, b_idx) and torch.equal(dst, b_dst)
-    ranks = ranks.cpu().numpy()
+    if idx is not None:
+        assert torch.equal(idx, b_idx) and torch.equal(dst, b_dst)
+    ranks = res.ranks
     w = b_res.ranks.shape[1]
     assert ranks.shape[1] >= w and np.array_equal(ranks[:, :w], b_res.ranks) and (ranks[:, w:] == -1).all()
-    res = R._aggregate(ranks, ap, cnt, q_pids, ng, 50)
     assert np.array_equal(res.cmc, b_res.cmc) and res.mAP == b_res.mAP and np.array_equal(res.all_topk, b_res.all_topk)
     assert np.array_equal(res.single_performance, b_res.single_performance)
 
@@ -597,7 +601,36 @@ def test_sharded_protocol_on_one_device(R, N, sharded_problem, pid_sorted):
     ap = torch.empty(nq, dtype=torch.float64, device="cuda")
     N.check(L.ctl_eval_finalize(total.data_ptr(), thr_count.data_ptr(), nq, mp, ranks.data_ptr(), ap.data_ptr(), s()))
     idx, dst = R.merge_topk(idx_l, dst_l, k)
-    _same_as_unsharded(R, base, idx, dst, ranks, ap.cpu().numpy(), thr_count.cpu().numpy(), pids[:nq], ng)
+    _same_as_unsharded(base, idx, dst, R._aggregate(ranks.cpu().numpy(), ap.cpu().numpy(), thr_count.cpu().numpy(),
+                                                    pids[:nq], ng, 50))
+
+
+@pytest.mark.parametrize("topk", [True, False])
+@pytest.mark.parametrize("pid_sorted", [False, True])
+@pytest.mark.parametrize("world", [2, 3])
+def test_sharded_streamed_passes_under_a_stand_in_exchange(R, sharded_problem, world, pid_sorted, topk):
+    """retrieval._streamed -- the code of topk_and_eval_sharded (top-k + evaluation) and evaluate_streamed(group=)
+    (evaluation only) -- with W ranks emulated on one device (shard_exchange.Shards) over uneven gallery shards of at
+    least k rows, in the caller's order or in identity order: bit-identical to the unsharded run on every rank."""
+    q, gal, pids, cams, k, qp, base = sharded_problem
+    nq, ng = q.shape[0], gal.shape[0]
+    cuts = {2: (0, 4270, ng), 3: tuple(np.concatenate([[0], np.cumsum(SHARDS)]))}[world]
+    qo = R.pid_order(pids[:nq]) if pid_sorted else None
+    qps = R.build_planes(q, order=qo)
+
+    def rank(ex):
+        lo, hi = int(cuts[ex.rank]), int(cuts[ex.rank + 1])
+        g_pid, g_cam = pids[nq + lo: nq + hi], cams[nq + lo: nq + hi]
+        go = R.pid_order(g_pid) if pid_sorted else None
+        ids = R.encode_ids(pids[:nq], g_pid, cams[:nq], g_cam, False, "cuda", global_labels=True, q_order=qo, g_order=go)
+        ids.max_pos = R._max_over_ranks(ex, ids.max_pos, "cuda")  # encode_ids_sharded
+        return R._streamed(ex, qps, R.build_planes(gal[lo:hi], order=go), ids, k if topk else None, pids[:nq], ng, 50, lo)
+
+    for out in Shards(world).run(rank):
+        if topk:
+            _same_as_unsharded(base, *out)
+        else:
+            _same_as_unsharded(base, None, None, out[0])
 
 
 def test_topk_and_eval_sharded_in_a_group_of_one(R, sharded_problem, tmp_path):
