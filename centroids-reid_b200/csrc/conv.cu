@@ -82,9 +82,16 @@ struct ConvCfg {
   static_assert(SMEM <= 227 * 1024, "conv_gemm_kernel shared memory");
 };
 
-// Tile order: n fastest, then pixel tiles row-major inside an image, then images.  Each CTA owns a
-// CONTIGUOUS range of tiles so that coordinates advance by carries (no integer division in the loop)
-// and consecutive tiles of a CTA reuse the same activation tile from L2.
+// Tile order: n fastest, then pixel tiles row-major inside an image, then images.  An unchained launch of more than
+// one n-tile deals the tiles round-robin: CTA c takes tiles c, c + grid, c + 2 grid, ...  So the CTAs running at any
+// moment hold every n-tile of a few consecutive m-tiles, and the n_tiles reads of one activation tile fall within one
+// tile's runtime: the first brings its lines into L2 and the others hit them.  A contiguous range per CTA instead
+// spaces those reads one tile apart per CTA while all other CTAs stream their own activation tiles through L2; where
+// those add up to more than L2 (layer4 at the bench shape: 132 x 512 KB), each n-tile re-reads its activation tile
+// from HBM.  A launch of one n-tile has no such re-read and keeps a contiguous range per CTA: the order in which it
+// reads its input then matches what the launch before it left in L2.  A chained launch (N2 > 0) owns a contiguous
+// range of whole m-tiles.  In a contiguous range the coordinates advance by carries; a round-robin step recomputes
+// them from the tile index (a few integer divisions per tile).
 struct TileIter {
   int nt, tw, th, img;
   __device__ __forceinline__ void init(int tile, const ConvKernelParams& p) {
@@ -107,6 +114,13 @@ struct TileIter {
         }
       }
     }
+  }
+  // to `tile`, `step` tiles after the current one
+  __device__ __forceinline__ void advance(int tile, int step, const ConvKernelParams& p) {
+    if (step == 1)
+      next(p);
+    else
+      init(tile, p);
   }
 };
 
@@ -165,14 +179,14 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid
   const int warp = threadIdx.x >> 5;
   const int num_tiles = p.m_tiles * p.n_tiles;
   const int conv_kblocks = p.k_blocks;
-  // contiguous, balanced tile range of this CTA (chained: of whole m-tiles)
-  const int units = N2 > 0 ? p.m_tiles : num_tiles;
-  const int per = units / (int)gridDim.x, rem = units - per * (int)gridDim.x;
-  int t_begin = (int)blockIdx.x * per + min((int)blockIdx.x, rem);
-  int t_end = t_begin + per + ((int)blockIdx.x < rem ? 1 : 0);
-  if constexpr (N2 > 0) {
-    t_begin *= p.n_tiles;
-    t_end *= p.n_tiles;
+  // this CTA's tiles: t_begin, t_begin + t_step, ... < t_end (see "Tile order"); the producer and both consumer
+  // warpgroups walk the same sequence
+  int t_begin = (int)blockIdx.x, t_end = num_tiles, t_step = (int)gridDim.x;
+  if (N2 > 0 || p.n_tiles == 1) {  // a contiguous, balanced range of whole m-tiles
+    const int per = p.m_tiles / (int)gridDim.x, rem = p.m_tiles - per * (int)gridDim.x;
+    t_begin = ((int)blockIdx.x * per + min((int)blockIdx.x, rem)) * p.n_tiles;
+    t_end = t_begin + (per + ((int)blockIdx.x < rem ? 1 : 0)) * p.n_tiles;
+    t_step = 1;
   }
 
   if (threadIdx.x == 0) {
@@ -202,12 +216,12 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid
   if (warp < 4) {
     // ===================== TMA producer =====================
     setmaxnreg_dec<PRODUCER_REGS>();
-    if (threadIdx.x == 0 && t_begin < t_end) {
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       TileIter it;
       it.init(t_begin, p);
-      for (int tile = t_begin; tile < t_end; ++tile, it.next(p)) {
+      for (int tile = t_begin; tile < t_end; tile += t_step, it.advance(tile, t_step, p)) {
         const int h0 = it.th * p.TH, w0 = it.tw * p.TW;
         for (int t = 0; t < p.n_taps; ++t) {
           const ConvTap tap = t < 9 ? p.taps[t] : p.tap9;
@@ -269,8 +283,8 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid
     uint32_t phase = 0;
     uint32_t g = 0;  // running sub-tile counter -> staging slab
     TileIter it;
-    if (t_begin < t_end) it.init(t_begin, p);
-    for (int tile = t_begin; tile < t_end; ++tile, it.next(p)) {
+    it.init(t_begin, p);
+    for (int tile = t_begin; tile < t_end; tile += t_step, it.advance(tile, t_step, p)) {
       const int h0 = it.th * p.TH, w0 = it.tw * p.TW;
       int held = -1;  // ring slot still read by the wgmma group in flight
       for (int kb = 0; kb < conv_kblocks; ++kb) {
