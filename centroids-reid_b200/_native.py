@@ -135,8 +135,7 @@ SIGNATURES = {
     "ctl_conv1x1_chain_supported": (_i32, [_i32, _i32]),
     "ctl_conv1x1_chain_nhwc_f16": (C.c_int, [_p, _i32, _p, _i32, _i32, _i32, _i32, _i32, _p, _p, _p, _p, _i32, _p, _p,
                                              _i32, _i32, _p, _p]),
-    "ctl_trunk_create": (C.c_int, [C.POINTER(_p), _i32, _i32, C.POINTER(_i32)]),
-    "ctl_trunk_create_ex": (C.c_int, [C.POINTER(_p), _i32, _i32, _i32, C.POINTER(_i32)]),
+    "ctl_trunk_create": (C.c_int, [C.POINTER(_p), _i32, _i32, _i32, C.POINTER(_i32)]),
     "ctl_trunk_feature_dim": (_i32, [_p]),
     "ctl_trunk_destroy": (None, [_p]),
     "ctl_weights_pack": (C.c_int, [_p, C.POINTER(NamedTensor), _i32, _p]),
@@ -146,8 +145,7 @@ SIGNATURES = {
     "ctl_embed_blocks": (C.c_int, [_p, _p, _i32, _i32, _i32, _p, _p, _sz, _p]),
     "ctl_embed_head": (C.c_int, [_p, _p, _i32, _i32, _p, _p, _p]),
     "ctl_embed_launches": (_i32, [_p]),
-    "ctl_trainer_create": (C.c_int, [C.POINTER(_p), _i32, _i32, C.c_float, C.POINTER(_i32)]),
-    "ctl_trainer_create_ex": (C.c_int, [C.POINTER(_p), _i32, _i32, _i32, C.c_float, C.POINTER(_i32)]),
+    "ctl_trainer_create": (C.c_int, [C.POINTER(_p), _i32, _i32, _i32, C.c_float, C.POINTER(_i32)]),
     "ctl_trainer_feature_dim": (_i32, [_p]),
     "ctl_trainer_destroy": (None, [_p]),
     "ctl_trainer_bind": (C.c_int, [_p, C.POINTER(NamedTensor), _i32, C.POINTER(NamedTensor), _i32]),

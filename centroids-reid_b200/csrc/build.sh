@@ -12,7 +12,7 @@ pids=()
 for src in "${HERE}"/*.cu; do
   obj="${HERE}/obj/$(basename "${src%.cu}").o"
   if [[ ! -f "$obj" || "$src" -nt "$obj" || "${HERE}/wgmma.cuh" -nt "$obj" || "${HERE}/common.h" -nt "$obj" \
-        || "${HERE}/../../include/ctl_b200.h" -nt "$obj" ]]; then
+        || "${HERE}/resnet.h" -nt "$obj" || "${HERE}/../../include/ctl_b200.h" -nt "$obj" ]]; then
     ( "$NVCC" "${FLAGS[@]}" -c "$src" -o "$obj" > "${obj%.o}.log" 2>&1 || { cat "${obj%.o}.log"; exit 1; } ) &
     pids+=($!)
   fi

@@ -260,7 +260,6 @@ struct PackEntry {
   int cout, cin, k, pad_;
   long long chunk_begin;
 };
-static constexpr int PACK_CHUNK = 8192;
 
 __global__ void __launch_bounds__(256) train_pack_kernel(const PackEntry* __restrict__ table, int n_tensors, long long n_chunks) {
   pdl_launch_dependents();
@@ -274,8 +273,8 @@ __global__ void __launch_bounds__(256) train_pack_kernel(const PackEntry* __rest
     const PackEntry e = table[lo];
     const int kk = e.k * e.k;
     const long long numel = (long long)e.cout * e.cin * kk;
-    const long long base = (chunk - e.chunk_begin) * PACK_CHUNK;
-    const long long end = min(numel, base + PACK_CHUNK);
+    const long long base = (chunk - e.chunk_begin) * CTL_PACK_CHUNK;
+    const long long end = min(numel, base + CTL_PACK_CHUNK);
     for (long long i = base + threadIdx.x; i < end; i += blockDim.x) {
       const int rs = (int)(i % kk);
       const long long t = i / kk;

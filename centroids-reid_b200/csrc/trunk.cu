@@ -16,15 +16,13 @@
 #include <array>
 #include <map>
 #include <string>
-#include <unordered_map>
 #include <vector>
 
 #include "common.h"
+#include "resnet.h"
 #include "wgmma.cuh"
 
 namespace ctl {
-
-static constexpr float TRUNK_BN_EPS = 1e-5f;
 
 // w [cout][cin][k][k] fp32 (+ BatchNorm gamma/beta/mean/var of `nbn` channels starting at channel c0; nullptr = no fold)
 //   -> out [cout][k][k][cin] fp16 rows of pitch `pitch` elements at column offset `col0`;
@@ -37,7 +35,7 @@ __global__ void fold_pack_kernel(const float* __restrict__ w, int cout, int cin,
   float scale = 1.f, b = 0.f;
   if (gamma != nullptr && co >= c0) {
     const int j = co - c0;
-    scale = __fdiv_rn(gamma[j], __fsqrt_rn(__fadd_rn(var[j], TRUNK_BN_EPS)));
+    scale = __fdiv_rn(gamma[j], __fsqrt_rn(__fadd_rn(var[j], BN_EPS)));
     b = __fsub_rn(beta[j], __fmul_rn(mean[j], scale));
   }
   const int kk = k * k;
@@ -49,14 +47,17 @@ __global__ void fold_pack_kernel(const float* __restrict__ w, int cout, int cin,
   if (threadIdx.x == 0 && bias != nullptr) bias[co] = accumulate ? __fadd_rn(bias[co], b) : b;
 }
 
-// stem layouts from the folded [64][3][7][7] weights (ctl_stem_conv7x7_tc: [64][192], k = (c*7 + r)*8 + s, s = 7 and
-// k >= 168 zero;  ctl_stem_pool_fused: [28][64][8], chunk = r*4 + s/2, element = (s%2)*4 + ch, ch == 3 and s == 7 zero)
+// stem layouts (ctl_stem_conv7x7_tc: [64][192], k = (c*7 + r)*8 + s, s = 7 and k >= 168 zero;  ctl_stem_pool_fused:
+// [28][64][8], chunk = r*4 + s/2, element = (s%2)*4 + ch, ch == 3 and s == 7 zero) -- see stem_pack
 __global__ void stem_pack_kernel(const float* __restrict__ w, const float* __restrict__ gamma, const float* __restrict__ beta,
                                  const float* __restrict__ mean, const float* __restrict__ var, __half* __restrict__ w192,
                                  __half* __restrict__ w3, float* __restrict__ bias) {
   const int o = blockIdx.x;
-  const float scale = __fdiv_rn(gamma[o], __fsqrt_rn(__fadd_rn(var[o], TRUNK_BN_EPS)));
-  if (threadIdx.x == 0) bias[o] = __fsub_rn(beta[o], __fmul_rn(mean[o], scale));
+  float scale = 1.f;
+  if (gamma != nullptr) {
+    scale = __fdiv_rn(gamma[o], __fsqrt_rn(__fadd_rn(var[o], BN_EPS)));
+    if (threadIdx.x == 0) bias[o] = __fsub_rn(beta[o], __fmul_rn(mean[o], scale));
+  }
   for (int i = threadIdx.x; i < 192; i += blockDim.x) {
     float v = 0.f;
     if (i < 168) {
@@ -65,6 +66,7 @@ __global__ void stem_pack_kernel(const float* __restrict__ w, const float* __res
     }
     w192[(size_t)o * 192 + i] = __float2half_rn(v);
   }
+  if (w3 == nullptr) return;
   for (int i = threadIdx.x; i < 28 * 8; i += blockDim.x) {
     const int chunk = i / 8, e = i % 8, r = chunk / 4, s = (chunk % 4) * 2 + e / 4, ch = e % 4;
     float v = 0.f;
@@ -73,26 +75,29 @@ __global__ void stem_pack_kernel(const float* __restrict__ w, const float* __res
   }
 }
 
+int stem_pack(const float* w, const float* gamma, const float* beta, const float* mean, const float* var, __half* w192,
+              __half* w3, float* bias, cudaStream_t st) {
+  stem_pack_kernel<<<64, 128, 0, st>>>(w, gamma, beta, mean, var, w192, w3, bias);
+  CTL_LAUNCH_CHECK();
+  return 0;
+}
+
 __global__ void head_pack_kernel(const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ mean,
                                  const float* __restrict__ var, int n, float* __restrict__ scale, float* __restrict__ shift) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const float s = __fdiv_rn(gamma[i], __fsqrt_rn(__fadd_rn(var[i], TRUNK_BN_EPS)));
+  const float s = __fdiv_rn(gamma[i], __fsqrt_rn(__fadd_rn(var[i], BN_EPS)));
   scale[i] = s;
   shift[i] = __fsub_rn(beta[i], __fmul_rn(mean[i], s));
 }
 
-struct PackedConv {
+// a convolution of the layout and its packed operands: folded fp16 weights w, fp32 biases b
+struct PackedConv : ConvLayout {
   __half* w = nullptr;
   float* b = nullptr;
-  int cin = 0, cout = 0, k = 1, stride = 1, relu = 1, relu_from = 0;
 };
-struct TrunkBlock {
-  std::string prefix;  // "layer<stage>.<block>" of the state_dict names
-  PackedConv c1, c2, c3, down;  // a BasicBlock has no c3: c1 and c2 are its two 3x3 convolutions
-  bool has_down = false, has_in = false;
-  int in_half = 0;
-  float *in_gamma = nullptr, *in_beta = nullptr;
+struct TrunkBlock : BlockLayout<PackedConv> {
+  float *in_gamma = nullptr, *in_beta = nullptr;  // c1's InstanceNorm (IBN-a)
   __half* dual_w = nullptr;
   float* dual_b = nullptr;
 };
@@ -101,7 +106,7 @@ struct TrunkBlock {
 
 struct ctl_trunk {
   int block = CTL_BLOCK_BOTTLENECK, feature_dim = 2048;
-  int ibn = 0, last_stride = 1;
+  int ibn = 0;
   bool packed = false, has_head = false;
   std::vector<ctl::TrunkBlock> blocks;
   __half *stem_w192 = nullptr, *stem_w3 = nullptr;
@@ -116,72 +121,35 @@ struct ctl_trunk {
 
 namespace ctl {
 
-template <typename T>
-static T* dev_alloc(ctl_trunk* h, size_t count) {
-  void* p = nullptr;
-  if (cudaMalloc(&p, count * sizeof(T)) != cudaSuccess) return nullptr;
-  h->owned.push_back(p);
-  return static_cast<T*>(p);
-}
-
-struct TensorRef {
-  const float* data;
-  long long numel;
-};
-using TensorMap = std::unordered_map<std::string, TensorRef>;
-
-static const float* need(const TensorMap& m, const std::string& name, long long numel, int* rc) {
-  auto it = m.find(name);
-  if (it == m.end() || it->second.data == nullptr) {
-    set_error("ctl_weights_pack: tensor '%s' is missing", name.c_str());
-    *rc = CTL_ERR_INVALID_ARGUMENT;
-    return nullptr;
-  }
-  if (it->second.numel != numel) {
-    set_error("ctl_weights_pack: tensor '%s' has %lld elements, expected %lld", name.c_str(), it->second.numel, numel);
-    *rc = CTL_ERR_INVALID_ARGUMENT;
-    return nullptr;
-  }
-  return it->second.data;
-}
-
-// packs conv `conv` with BatchNorm `bn` (bn empty: raw weights); ibn_half > 0: BN folds channels [ibn_half, cout) only
-static int pack_conv(ctl_trunk* h, const TensorMap& m, const std::string& conv, const std::string& bn, int cout, int cin, int k,
-                     int ibn_half, PackedConv* out, cudaStream_t st) {
+// packs `c` with its BatchNorm folded in (IBN-a: channels [in_half, cout) only)
+static int pack_conv(ctl_trunk* h, const NamedMap& m, PackedConv& c, cudaStream_t st) {
   int rc = 0;
-  const float* w = need(m, conv + ".weight", (long long)cout * cin * k * k, &rc);
+  const float* w = lookup(m, c.conv + ".weight", (long long)c.cout * c.cin * c.k * c.k, &rc);
   if (rc) return rc;
-  const int nbn = cout - ibn_half;
-  const float *g = need(m, bn + ".weight", nbn, &rc), *b = need(m, bn + ".bias", nbn, &rc),
-              *mu = need(m, bn + ".running_mean", nbn, &rc), *va = need(m, bn + ".running_var", nbn, &rc);
+  const int nbn = c.cout - c.in_half;
+  const float *g = lookup(m, c.bn + ".weight", nbn, &rc), *b = lookup(m, c.bn + ".bias", nbn, &rc),
+              *mu = lookup(m, c.bn + ".running_mean", nbn, &rc), *va = lookup(m, c.bn + ".running_var", nbn, &rc);
   if (rc) return rc;
-  if (!out->w) out->w = dev_alloc<__half>(h, (size_t)cout * cin * k * k);
-  if (!out->b) out->b = dev_alloc<float>(h, cout);
-  if (!out->w || !out->b) {
+  if (!c.w) c.w = dev_alloc<__half>(h, (size_t)c.cout * c.cin * c.k * c.k);
+  if (!c.b) c.b = dev_alloc<float>(h, c.cout);
+  if (!c.w || !c.b) {
     set_error("ctl_weights_pack: out of device memory");
     return (int)cudaErrorMemoryAllocation;
   }
-  out->cin = cin;
-  out->cout = cout;
-  out->k = k;
-  fold_pack_kernel<<<cout, 256, 0, st>>>(w, cout, cin, k, g, b, mu, va, ibn_half, out->w, (long long)cin * k * k, 0, out->b, 0);
+  fold_pack_kernel<<<c.cout, 256, 0, st>>>(w, c.cout, c.cin, c.k, g, b, mu, va, c.in_half, c.w, (long long)c.cin * c.k * c.k, 0,
+                                           c.b, 0);
   CTL_LAUNCH_CHECK();
   return 0;
 }
 
-
-// The downsample of `blk` and the single-GEMM form of its block's last convolution `last` (conv3 of a bottleneck,
-// conv2 of a BasicBlock) + shortcut: [W_last | Wd] with bias_last + bias_d (ctl_conv1x1_dual_nhwc_f16 /
-// ctl_conv3x3_dual_nhwc_f16).  `last` must be packed already.
-static int pack_down_dual(ctl_trunk* h, const TensorMap& m, TrunkBlock& blk, const PackedConv& last, cudaStream_t st) {
+// The single-GEMM form of the last convolution `last` of `blk` (conv3 of a bottleneck, conv2 of a BasicBlock) + its
+// downsample: [W_last | Wd] with bias_last + bias_d (ctl_conv1x1_dual_nhwc_f16 / ctl_conv3x3_dual_nhwc_f16).  `last` and
+// the downsample must be packed already.
+static int pack_dual(ctl_trunk* h, const NamedMap& m, TrunkBlock& blk, const PackedConv& last, cudaStream_t st) {
   int rc = 0;
-  const std::string& p = blk.prefix;
-  const int sd = blk.down.stride;
-  if ((rc = pack_conv(h, m, p + ".downsample.0", p + ".downsample.1", blk.down.cout, blk.down.cin, 1, 0, &blk.down, st))) return rc;
-  blk.down.stride = sd;
-  blk.down.relu = 0;
+  const PackedConv& d = blk.down;
   const int km = last.k * last.k * last.cin;  // row length of the packed [cout][k][k][cin] weights
-  const int kt = km + blk.down.cin;
+  const int kt = km + d.cin;
   if (!blk.dual_w) {
     blk.dual_w = dev_alloc<__half>(h, (size_t)last.cout * kt);
     blk.dual_b = dev_alloc<float>(h, last.cout);
@@ -192,15 +160,14 @@ static int pack_down_dual(ctl_trunk* h, const TensorMap& m, TrunkBlock& blk, con
   }
   CTL_CUDA(cudaMemcpy2DAsync(blk.dual_w, (size_t)kt * 2, last.w, (size_t)km * 2, (size_t)km * 2, last.cout,
                              cudaMemcpyDeviceToDevice, st));
-  CTL_CUDA(cudaMemcpy2DAsync(blk.dual_w + km, (size_t)kt * 2, blk.down.w, (size_t)blk.down.cin * 2,
-                             (size_t)blk.down.cin * 2, last.cout, cudaMemcpyDeviceToDevice, st));
+  CTL_CUDA(cudaMemcpy2DAsync(blk.dual_w + km, (size_t)kt * 2, d.w, (size_t)d.cin * 2, (size_t)d.cin * 2, last.cout,
+                             cudaMemcpyDeviceToDevice, st));
   // bias_last + bias_d, one fp32 add per channel
   CTL_CUDA(cudaMemcpyAsync(blk.dual_b, last.b, last.cout * sizeof(float), cudaMemcpyDeviceToDevice, st));
-  const std::string d = p + ".downsample.1";
-  fold_pack_kernel<<<last.cout, 32, 0, st>>>(need(m, p + ".downsample.0.weight", (long long)blk.down.cout * blk.down.cin, &rc), blk.down.cout, 0, 1,
-                                             need(m, d + ".weight", blk.down.cout, &rc), need(m, d + ".bias", blk.down.cout, &rc),
-                                             need(m, d + ".running_mean", blk.down.cout, &rc),
-                                             need(m, d + ".running_var", blk.down.cout, &rc), 0, blk.down.w, 0, 0, blk.dual_b, 1);
+  fold_pack_kernel<<<last.cout, 32, 0, st>>>(lookup(m, d.conv + ".weight", (long long)d.cout * d.cin, &rc), d.cout, 0, 1,
+                                             lookup(m, d.bn + ".weight", d.cout, &rc), lookup(m, d.bn + ".bias", d.cout, &rc),
+                                             lookup(m, d.bn + ".running_mean", d.cout, &rc),
+                                             lookup(m, d.bn + ".running_var", d.cout, &rc), 0, d.w, 0, 0, blk.dual_b, 1);
   CTL_LAUNCH_CHECK();
   return rc;
 }
@@ -211,74 +178,15 @@ using namespace ctl;
 
 extern "C" {
 
-int ctl_trunk_create(ctl_trunk** out, int32_t ibn, int32_t last_stride, const int32_t stage_blocks[4]) {
-  return ctl_trunk_create_ex(out, CTL_BLOCK_BOTTLENECK, ibn, last_stride, stage_blocks);
-}
-
-int ctl_trunk_create_ex(ctl_trunk** out, int32_t block, int32_t ibn, int32_t last_stride, const int32_t stage_blocks[4]) {
-  CTL_CHECK_ARG(out != nullptr && stage_blocks != nullptr, "null pointer");
-  CTL_CHECK_ARG(block == CTL_BLOCK_BOTTLENECK || block == CTL_BLOCK_BASIC,
-                "block = %d: expected CTL_BLOCK_BOTTLENECK (0) or CTL_BLOCK_BASIC (1)", block);
-  CTL_CHECK_ARG(block == CTL_BLOCK_BOTTLENECK || !ibn, "IBN-a is defined for bottleneck blocks only (resnet_ibn_a.py)");
-  CTL_CHECK_ARG(last_stride == 1 || last_stride == 2, "last_stride must be 1 or 2 (config/defaults.py:24)");
-  for (int li = 0; li < 4; ++li)
-    CTL_CHECK_ARG(stage_blocks[li] >= 1, "stage_blocks[%d] = %d: every stage needs at least one block", li, stage_blocks[li]);
+int ctl_trunk_create(ctl_trunk** out, int32_t block, int32_t ibn, int32_t last_stride, const int32_t stage_blocks[4]) {
+  CTL_CHECK_ARG(out != nullptr, "null pointer");
   ctl_trunk* h = new ctl_trunk();
+  if (int rc = resnet_layout(block, ibn, last_stride, stage_blocks, &h->feature_dim, &h->blocks)) {
+    delete h;
+    return rc;
+  }
   h->block = block;
   h->ibn = ibn ? 1 : 0;
-  h->last_stride = last_stride;
-  const int planes[4] = {64, 128, 256, 512};
-  int inplanes = 64;
-  if (block == CTL_BLOCK_BASIC) {
-    h->feature_dim = 512;
-    // resnet.py:19-48,105-112: conv1 3x3 / stride, conv2 3x3; a downsample where stride != 1 or inplanes != planes,
-    // i.e. on the first block of layers 2-4
-    for (int li = 0; li < 4; ++li)
-      for (int bi = 0; bi < stage_blocks[li]; ++bi) {
-        TrunkBlock blk;
-        blk.prefix = "layer" + std::to_string(li + 1) + "." + std::to_string(bi);
-        const int stride = bi == 0 ? (li == 0 ? 1 : (li == 3 ? last_stride : 2)) : 1;
-        blk.c1.cin = inplanes;
-        blk.c1.cout = blk.c2.cin = blk.c2.cout = planes[li];
-        blk.c1.k = blk.c2.k = 3;
-        blk.c1.stride = stride;
-        blk.has_down = stride != 1 || inplanes != planes[li];
-        if (blk.has_down) {
-          blk.down.cin = inplanes;
-          blk.down.cout = planes[li];
-          blk.down.stride = stride;
-          blk.down.relu = 0;
-        }
-        inplanes = planes[li];
-        h->blocks.push_back(blk);
-      }
-    *out = h;
-    return 0;
-  }
-  for (int li = 0; li < 4; ++li)
-    for (int bi = 0; bi < stage_blocks[li]; ++bi) {
-      TrunkBlock blk;
-      blk.prefix = "layer" + std::to_string(li + 1) + "." + std::to_string(bi);
-      const int stride0 = li == 0 ? 1 : (li == 3 ? last_stride : 2);
-      blk.c1.cin = inplanes;
-      blk.c1.cout = planes[li];
-      blk.c2.cin = blk.c2.cout = planes[li];
-      blk.c2.k = 3;
-      blk.c2.stride = bi == 0 ? stride0 : 1;
-      blk.c3.cin = planes[li];
-      blk.c3.cout = planes[li] * 4;
-      blk.has_down = bi == 0;
-      if (blk.has_down) {
-        blk.down.cin = inplanes;
-        blk.down.cout = planes[li] * 4;
-        blk.down.stride = blk.c2.stride;
-        blk.down.relu = 0;
-        inplanes = planes[li] * 4;
-      }
-      blk.has_in = h->ibn && planes[li] != 512;  // resnet_ibn_a.py:116-119
-      blk.in_half = blk.has_in ? planes[li] / 2 : 0;
-      h->blocks.push_back(blk);
-    }
   *out = h;
   return 0;
 }
@@ -296,16 +204,13 @@ int ctl_weights_pack(ctl_trunk* h, const ctl_named_tensor* tensors, int32_t n_te
   int rc = ctl_device_check();
   if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  TensorMap m;
-  for (int i = 0; i < n_tensors; ++i) {
-    CTL_CHECK_ARG(tensors[i].name != nullptr, "tensor %d has no name", i);
-    m[tensors[i].name] = TensorRef{tensors[i].data, (long long)tensors[i].numel};
-  }
+  NamedMap m;
+  if ((rc = index_named(tensors, n_tensors, "ctl_weights_pack", "tensor", &m))) return rc;
   // ---- stem ----
   {
-    const float* w = need(m, "conv1.weight", 64 * 147, &rc);
-    const float *g = need(m, "bn1.weight", 64, &rc), *b = need(m, "bn1.bias", 64, &rc), *mu = need(m, "bn1.running_mean", 64, &rc),
-                *va = need(m, "bn1.running_var", 64, &rc);
+    const float* w = lookup(m, "conv1.weight", 64 * 147, &rc);
+    const float *g = lookup(m, "bn1.weight", 64, &rc), *b = lookup(m, "bn1.bias", 64, &rc),
+                *mu = lookup(m, "bn1.running_mean", 64, &rc), *va = lookup(m, "bn1.running_var", 64, &rc);
     if (rc) return rc;
     if (!h->stem_w192) {
       h->stem_w192 = dev_alloc<__half>(h, 64 * 192);
@@ -316,46 +221,32 @@ int ctl_weights_pack(ctl_trunk* h, const ctl_named_tensor* tensors, int32_t n_te
       set_error("ctl_weights_pack: out of device memory");
       return (int)cudaErrorMemoryAllocation;
     }
-    stem_pack_kernel<<<64, 128, 0, st>>>(w, g, b, mu, va, h->stem_w192, h->stem_w3, h->stem_b);
-    CTL_LAUNCH_CHECK();
+    if ((rc = stem_pack(w, g, b, mu, va, h->stem_w192, h->stem_w3, h->stem_b, st))) return rc;
   }
-  // ---- bottlenecks ----
+  // ---- blocks ----
   for (TrunkBlock& blk : h->blocks) {
-    const std::string& p = blk.prefix;
-    if (h->block == CTL_BLOCK_BASIC) {
-      if ((rc = pack_conv(h, m, p + ".conv1", p + ".bn1", blk.c1.cout, blk.c1.cin, 3, 0, &blk.c1, st))) return rc;
-      if ((rc = pack_conv(h, m, p + ".conv2", p + ".bn2", blk.c2.cout, blk.c2.cin, 3, 0, &blk.c2, st))) return rc;
-      if (blk.has_down && (rc = pack_down_dual(h, m, blk, blk.c2, st))) return rc;
-      continue;
-    }
-    if (blk.has_in) {
-      // IBN: channels [0, half) keep the raw convolution (InstanceNorm + ReLU follow as their own kernel), the
-      // BatchNorm half is folded; ReLU in the conv epilogue only from channel `half` on
-      if ((rc = pack_conv(h, m, p + ".conv1", p + ".bn1.BN", blk.c1.cout, blk.c1.cin, 1, blk.in_half, &blk.c1, st))) return rc;
-      blk.c1.relu_from = blk.in_half;
-      const float *ig = need(m, p + ".bn1.IN.weight", blk.in_half, &rc), *ib = need(m, p + ".bn1.IN.bias", blk.in_half, &rc);
+    for (PackedConv* c : blk.state_dict_order()) {
+      if (!c) continue;
+      if ((rc = pack_conv(h, m, *c, st))) return rc;
+      if (!c->in_half) continue;
+      // IBN: channels [0, half) keep the raw convolution, and InstanceNorm + ReLU follow as their own kernel
+      const float *ig = lookup(m, c->in + ".weight", c->in_half, &rc), *ib = lookup(m, c->in + ".bias", c->in_half, &rc);
       if (rc) return rc;
       if (!blk.in_gamma) {
-        blk.in_gamma = dev_alloc<float>(h, blk.in_half);
-        blk.in_beta = dev_alloc<float>(h, blk.in_half);
+        blk.in_gamma = dev_alloc<float>(h, c->in_half);
+        blk.in_beta = dev_alloc<float>(h, c->in_half);
       }
-      CTL_CUDA(cudaMemcpyAsync(blk.in_gamma, ig, blk.in_half * sizeof(float), cudaMemcpyDeviceToDevice, st));
-      CTL_CUDA(cudaMemcpyAsync(blk.in_beta, ib, blk.in_half * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    } else {
-      if ((rc = pack_conv(h, m, p + ".conv1", p + ".bn1", blk.c1.cout, blk.c1.cin, 1, 0, &blk.c1, st))) return rc;
+      CTL_CUDA(cudaMemcpyAsync(blk.in_gamma, ig, c->in_half * sizeof(float), cudaMemcpyDeviceToDevice, st));
+      CTL_CUDA(cudaMemcpyAsync(blk.in_beta, ib, c->in_half * sizeof(float), cudaMemcpyDeviceToDevice, st));
     }
-    const int s2 = blk.c2.stride;
-    if ((rc = pack_conv(h, m, p + ".conv2", p + ".bn2", blk.c2.cout, blk.c2.cin, 3, 0, &blk.c2, st))) return rc;
-    blk.c2.stride = s2;
-    if ((rc = pack_conv(h, m, p + ".conv3", p + ".bn3", blk.c3.cout, blk.c3.cin, 1, 0, &blk.c3, st))) return rc;
-    if (blk.has_down && (rc = pack_down_dual(h, m, blk, blk.c3, st))) return rc;
+    if (blk.has_down && (rc = pack_dual(h, m, blk, blk.bottleneck ? blk.c3 : blk.c2, st))) return rc;
   }
   // ---- optional BatchNorm1d head (ModelBase.bn, modelling/bases.py:83) ----
-  h->has_head = m.count("bn_head.weight") != 0;
+  h->has_head = m.refs.count("bn_head.weight") != 0;
   if (h->has_head) {
     const int fd = h->feature_dim;
-    const float *g = need(m, "bn_head.weight", fd, &rc), *b = need(m, "bn_head.bias", fd, &rc),
-                *mu = need(m, "bn_head.running_mean", fd, &rc), *va = need(m, "bn_head.running_var", fd, &rc);
+    const float *g = lookup(m, "bn_head.weight", fd, &rc), *b = lookup(m, "bn_head.bias", fd, &rc),
+                *mu = lookup(m, "bn_head.running_mean", fd, &rc), *va = lookup(m, "bn_head.running_var", fd, &rc);
     if (rc) return rc;
     if (!h->head_scale) {
       h->head_scale = dev_alloc<float>(h, fd);
@@ -373,8 +264,6 @@ int ctl_weights_pack(ctl_trunk* h, const ctl_named_tensor* tensors, int32_t n_te
 namespace ctl {
 
 static size_t round256(size_t b) { return (b + 255) & ~(size_t)255; }
-static int stem_side(int s) { return (s + 6 - 7) / 2 + 1; }  // conv1 7x7 / 2, pad 3
-static int pool_side(int s) { return (s + 2 - 3) / 2 + 1; }  // maxpool 3x3 / 2, pad 1
 static bool fused_stem_fits(int hgt, int wid) { return hgt % 4 == 0 && wid % 2 == 0 && wid <= 128; }
 
 // One of the activation slots of the block walk on a [n, hp, wp, 64] stem output: layer1's output is the largest tensor
@@ -447,7 +336,7 @@ static int run_stem(ctl_trunk* h, const void* x, const float* mean3, const float
 static int run_conv(ctl_trunk* h, const PackedConv& c, const void* x, int n, int hh, int ww, const void* residual, void* out,
                     cudaStream_t st) {
   ++h->launches;
-  return ctl_conv2d_nhwc_f16(x, n, hh, ww, c.cin, c.w, c.b, residual, out, c.cout, c.k, c.stride, c.relu, c.relu_from, st);
+  return ctl_conv2d_nhwc_f16(x, n, hh, ww, c.cin, c.w, c.b, residual, out, c.cout, c.k, c.stride, c.relu, c.in_half, st);
 }
 
 // The bottleneck walk on x [n, hh, ww, 64].  Intermediates rotate through five workspace slots of `slot` bytes; x is
@@ -474,9 +363,9 @@ static int run_blocks(ctl_trunk* h, const void* x, int x_slot, int n, int* hh, i
     void* dst = out && bi + 1 == h->blocks.size() ? out : buf[role[3]];
     const int h1 = *hh, w1 = *ww;
     if (o1_ready < 0 && (rc = run_conv(h, blk.c1, a, n, h1, w1, nullptr, o1, st))) return rc;
-    if (blk.has_in) {
+    if (blk.c1.in_half) {
       ++h->launches;
-      if ((rc = ctl_instnorm_relu_nhwc_f16(o1, n, h1 * w1, blk.c1.cout, blk.in_half, blk.in_gamma, blk.in_beta, TRUNK_BN_EPS, st)))
+      if ((rc = ctl_instnorm_relu_nhwc_f16(o1, n, h1 * w1, blk.c1.cout, blk.c1.in_half, blk.in_gamma, blk.in_beta, BN_EPS, st)))
         return rc;
     }
     const int s = blk.c2.stride;
@@ -495,10 +384,10 @@ static int run_blocks(ctl_trunk* h, const void* x, int x_slot, int n, int* hh, i
     if (chain) {
       if (dual)
         rc = ctl_conv1x1_chain_nhwc_f16(o2, blk.c3.cin, a, h1, w1, blk.down.cin, s, n, blk.dual_w, blk.dual_b, nullptr, dst,
-                                        blk.c3.cout, nx->w, nx->b, nx->cout, nx->relu_from, o1, st);
+                                        blk.c3.cout, nx->w, nx->b, nx->cout, nx->in_half, o1, st);
       else
         rc = ctl_conv1x1_chain_nhwc_f16(o2, blk.c3.cin, nullptr, h2, w2, 0, 1, n, blk.c3.w, blk.c3.b, r, dst, blk.c3.cout,
-                                        nx->w, nx->b, nx->cout, nx->relu_from, o1, st);
+                                        nx->w, nx->b, nx->cout, nx->in_half, o1, st);
     } else if (dual) {
       rc = ctl_conv1x1_dual_nhwc_f16(o2, blk.c3.cin, a, h1, w1, blk.down.cin, s, n, blk.dual_w, blk.dual_b, dst, blk.c3.cout, 1, st);
     } else {

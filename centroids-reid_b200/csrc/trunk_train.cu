@@ -18,26 +18,13 @@
 
 #include <algorithm>
 #include <string>
-#include <unordered_map>
 #include <vector>
 
 #include "common.h"
+#include "resnet.h"
 #include "wgmma.cuh"
 
 namespace ctl {
-
-static constexpr float TT_BN_EPS = 1e-5f;
-static constexpr int TT_PACK_CHUNK = 8192;  // == PACK_CHUNK of train.cu
-
-// conv1.weight [64][3][7][7] fp32 -> the tensor-core stem's operand [64][192] fp16, k = (c*7 + r)*8 + s (s = 7, k >= 168 zero)
-__global__ void stem_train_pack_kernel(const float* __restrict__ w, __half* __restrict__ w192) {
-  const int o = blockIdx.x;
-  for (int i = threadIdx.x; i < 192; i += blockDim.x) {
-    float v = 0.f;
-    if (i < 168 && (i & 7) < 7) v = w[(size_t)o * 147 + (i >> 3) * 7 + (i & 7)];
-    w192[(size_t)o * 192 + i] = __float2half_rn(v);
-  }
-}
 
 // dw [64][192] fp32 (im2col GEMM order) -> conv1.weight's gradient [64][3][7][7], times 1 / loss-scale
 __global__ void stem_train_unpack_kernel(const float* __restrict__ dw192, float inv_scale, float* __restrict__ dw) {
@@ -72,9 +59,7 @@ struct Bump {
   }
 };
 
-struct ConvSpec {
-  std::string conv, bn;
-  int cin = 0, cout = 0, k = 1, stride = 1, relu = 1, in_half = 0;  // in_half > 0: IBN (InstanceNorm on [0, half))
+struct ConvSpec : ConvLayout {
   // bound parameters / gradients (device pointers into the host framework's tensors)
   const float *w = nullptr, *gamma = nullptr, *beta = nullptr, *in_gamma = nullptr, *in_beta = nullptr;
   float *rmean = nullptr, *rvar = nullptr;
@@ -87,16 +72,13 @@ struct ConvSpec {
   int n = 0, h = 0, w_in = 0, ho = 0, wo = 0;
 };
 
-struct TrainBlock {
-  ConvSpec c1, c2, c3, down;  // a BasicBlock has no c3: c1 and c2 are its two 3x3 convolutions
-  bool has_down = false;
-};
+using TrainBlock = BlockLayout<ConvSpec>;
 
 }  // namespace ctl
 
 struct ctl_trainer {
   int block = CTL_BLOCK_BOTTLENECK, feature_dim = 2048;
-  int ibn = 0, last_stride = 1;
+  int ibn = 0;
   float momentum = 0.1f;
   bool bound = false, forwarded = false, saved = false;  // saved: the last forward completed (ctl_train_saved)
   std::vector<ctl::TrainBlock> blocks;
@@ -124,49 +106,25 @@ struct ctl_trainer {
 
 namespace ctl {
 
-struct Ref {
-  float* data;
-  long long numel;
-};
-using RefMap = std::unordered_map<std::string, Ref>;
-
-static float* lookup(const RefMap& m, const std::string& name, long long numel, bool required, const char* what, int* rc) {
-  auto it = m.find(name);
-  if (it == m.end() || it->second.data == nullptr) {
-    if (required) {
-      set_error("ctl_trainer_bind: %s '%s' is missing", what, name.c_str());
-      *rc = CTL_ERR_INVALID_ARGUMENT;
-    }
-    return nullptr;
-  }
-  if (it->second.numel != numel) {
-    set_error("ctl_trainer_bind: %s '%s' has %lld elements, expected %lld", what, name.c_str(), it->second.numel, numel);
-    *rc = CTL_ERR_INVALID_ARGUMENT;
-    return nullptr;
-  }
-  return it->second.data;
-}
-
-static int bind_conv(ConvSpec& c, const RefMap& p, const RefMap& g) {
+static int bind_conv(ConvSpec& c, const NamedMap& p, const NamedMap& g) {
   int rc = 0;
-  c.w = lookup(p, c.conv + ".weight", (long long)c.cout * c.cin * c.k * c.k, true, "parameter", &rc);
-  c.dw = lookup(g, c.conv + ".weight", (long long)c.cout * c.cin * c.k * c.k, true, "gradient", &rc);
+  c.w = lookup(p, c.conv + ".weight", (long long)c.cout * c.cin * c.k * c.k, &rc, "parameter");
+  c.dw = lookup(g, c.conv + ".weight", (long long)c.cout * c.cin * c.k * c.k, &rc, "gradient");
   const int nbn = c.cout - c.in_half;
-  const std::string bn = c.in_half ? c.bn + ".BN" : c.bn;
-  c.gamma = lookup(p, bn + ".weight", nbn, true, "parameter", &rc);
-  c.beta = lookup(p, bn + ".bias", nbn, true, "parameter", &rc);
-  c.rmean = lookup(p, bn + ".running_mean", nbn, false, "buffer", &rc);
-  c.rvar = lookup(p, bn + ".running_var", nbn, false, "buffer", &rc);
-  c.dgamma = lookup(g, bn + ".weight", nbn, true, "gradient", &rc);
-  c.dbeta = lookup(g, bn + ".bias", nbn, true, "gradient", &rc);
+  c.gamma = lookup(p, c.bn + ".weight", nbn, &rc, "parameter");
+  c.beta = lookup(p, c.bn + ".bias", nbn, &rc, "parameter");
+  c.rmean = lookup(p, c.bn + ".running_mean", nbn, &rc, "buffer", false);
+  c.rvar = lookup(p, c.bn + ".running_var", nbn, &rc, "buffer", false);
+  c.dgamma = lookup(g, c.bn + ".weight", nbn, &rc, "gradient");
+  c.dbeta = lookup(g, c.bn + ".bias", nbn, &rc, "gradient");
   if (c.in_half) {
-    c.in_gamma = lookup(p, c.bn + ".IN.weight", c.in_half, true, "parameter", &rc);
-    c.in_beta = lookup(p, c.bn + ".IN.bias", c.in_half, true, "parameter", &rc);
-    c.din_gamma = lookup(g, c.bn + ".IN.weight", c.in_half, true, "gradient", &rc);
-    c.din_beta = lookup(g, c.bn + ".IN.bias", c.in_half, true, "gradient", &rc);
+    c.in_gamma = lookup(p, c.in + ".weight", c.in_half, &rc, "parameter");
+    c.in_beta = lookup(p, c.in + ".bias", c.in_half, &rc, "parameter");
+    c.din_gamma = lookup(g, c.in + ".weight", c.in_half, &rc, "gradient");
+    c.din_beta = lookup(g, c.in + ".bias", c.in_half, &rc, "gradient");
   }
   if (!rc && (c.rmean == nullptr) != (c.rvar == nullptr)) {
-    set_error("ctl_trainer_bind: '%s' needs running_mean and running_var together (or neither)", bn.c_str());
+    set_error("ctl_trainer_bind: '%s' needs running_mean and running_var together (or neither)", c.bn.c_str());
     rc = CTL_ERR_INVALID_ARGUMENT;
   }
   return rc;
@@ -198,13 +156,13 @@ static int conv_bn_forward(ctl_trainer* t, ConvSpec& c, Bump& ws, void* bn_ws, s
   int rc = ctl_conv2d_nhwc_f16(a, n, h, w, c.cin, c.wf, t->zero_bias, nullptr, c.y, c.cout, c.k, c.stride, 0, 0, st);
   if (rc) return rc;
   if (!c.in_half)
-    return ctl_bn_train_forward_nhwc_f16(c.y, rows, c.cout, c.cout, c.gamma, c.beta, TT_BN_EPS, t->momentum, c.rmean, c.rvar, residual,
+    return ctl_bn_train_forward_nhwc_f16(c.y, rows, c.cout, c.cout, c.gamma, c.beta, BN_EPS, t->momentum, c.rmean, c.rvar, residual,
                                          c.relu, bn_ws, bn_ws_bytes, c.mean, c.invstd, c.z, st);
   // IBN (resnet_ibn_a.py:18-32): InstanceNorm on channels [0, half), batch-statistics BatchNorm on [half, C); ReLU
-  rc = ctl_instnorm_train_forward_nhwc_f16(c.y, n, c.ho * c.wo, c.cout, c.in_half, c.in_gamma, c.in_beta, TT_BN_EPS, c.in_mean,
+  rc = ctl_instnorm_train_forward_nhwc_f16(c.y, n, c.ho * c.wo, c.cout, c.in_half, c.in_gamma, c.in_beta, BN_EPS, c.in_mean,
                                            c.in_invstd, c.z, st);
   if (rc) return rc;
-  return ctl_bn_train_forward_nhwc_f16(static_cast<const __half*>(c.y) + c.in_half, rows, nbn, c.cout, c.gamma, c.beta, TT_BN_EPS,
+  return ctl_bn_train_forward_nhwc_f16(static_cast<const __half*>(c.y) + c.in_half, rows, nbn, c.cout, c.gamma, c.beta, BN_EPS,
                                        t->momentum, c.rmean, c.rvar, nullptr, 1, bn_ws, bn_ws_bytes, c.mean, c.invstd,
                                        static_cast<__half*>(c.z) + c.in_half, st);
 }
@@ -279,8 +237,8 @@ struct Plan {
 static int forward_walk(ctl_trainer* t, Bump& ws, Plan& plan, void* bn_ws, size_t bn_ws_bytes, const float* x, int n, int H, int W,
                         float* out_feat, cudaStream_t st) {
   int rc = 0;
-  const int h = (H + 6 - 7) / 2 + 1, w = (W + 6 - 7) / 2 + 1;
-  const int hp = (h + 2 - 3) / 2 + 1, wp = (w + 2 - 3) / 2 + 1;
+  const int h = stem_side(H), w = stem_side(W);
+  const int hp = pool_side(h), wp = pool_side(w);
   const long long rows0 = (long long)n * h * w;
   t->y0 = ws.take((size_t)rows0 * 64 * 2);
   t->z0 = ws.take((size_t)rows0 * 64 * 2);
@@ -291,10 +249,9 @@ static int forward_walk(ctl_trainer* t, Bump& ws, Plan& plan, void* bn_ws, size_
   plan.bn_need = std::max(plan.bn_need, ctl_bn_workspace_bytes(rows0, 64));
   if (!ws.dry) {
     // stem: raw 7x7/2 conv -> BatchNorm (ReLU only in the IBN-a variant, resnet.py:125 / resnet_ibn_a.py:129) -> max-pool
-    stem_train_pack_kernel<<<64, 192, 0, st>>>(t->w0, t->stem_w192);
-    CTL_LAUNCH_CHECK();
+    if ((rc = stem_pack(t->w0, nullptr, nullptr, nullptr, nullptr, t->stem_w192, nullptr, nullptr, st))) return rc;
     if ((rc = ctl_stem_conv7x7_tc(x, n, H, W, t->stem_w192, t->zero_bias, 0, t->y0, st))) return rc;
-    if ((rc = ctl_bn_train_forward_nhwc_f16(t->y0, rows0, 64, 64, t->g0, t->b0, TT_BN_EPS, t->momentum, t->rm0, t->rv0, nullptr, t->ibn,
+    if ((rc = ctl_bn_train_forward_nhwc_f16(t->y0, rows0, 64, 64, t->g0, t->b0, BN_EPS, t->momentum, t->rm0, t->rv0, nullptr, t->ibn,
                                             bn_ws, bn_ws_bytes, t->m0, t->i0, t->z0, st)))
       return rc;
     if ((rc = ctl_maxpool3x3s2_argmax_nhwc_f16(t->z0, n, h, w, 64, t->pool0, t->arg0, st))) return rc;
@@ -370,7 +327,7 @@ static int backward_walk(ctl_trainer* t, Bump& ws, Plan& plan, void* bn_ws, size
   }
   ws.off = mark;
   // stem: max-pool -> BatchNorm (ReLU mask only for IBN-a) -> 7x7 weight gradient through the im2col GEMM
-  const int h = (t->H + 6 - 7) / 2 + 1, w = (t->W + 6 - 7) / 2 + 1;
+  const int h = stem_side(t->H), w = stem_side(t->W);
   const long long rows0 = (long long)n * h * w;
   void* dz0 = ws.take((size_t)rows0 * 64 * 2);
   void* dy0 = ws.take((size_t)rows0 * 64 * 2);
@@ -412,105 +369,24 @@ static int plan_layout(const ctl_trainer* t, int n, int H, int W, Layout* out) {
   return 0;
 }
 
-template <typename T>
-static T* t_alloc(ctl_trainer* h, size_t count) {
-  void* p = nullptr;
-  if (cudaMalloc(&p, count * sizeof(T)) != cudaSuccess) return nullptr;
-  h->owned.push_back(p);
-  return static_cast<T*>(p);
-}
-
 }  // namespace ctl
 
 using namespace ctl;
 
 extern "C" {
 
-int ctl_trainer_create(ctl_trainer** out, int32_t ibn, int32_t last_stride, float momentum, const int32_t stage_blocks[4]) {
-  return ctl_trainer_create_ex(out, CTL_BLOCK_BOTTLENECK, ibn, last_stride, momentum, stage_blocks);
-}
-
-int ctl_trainer_create_ex(ctl_trainer** out, int32_t block, int32_t ibn, int32_t last_stride, float momentum,
-                          const int32_t stage_blocks[4]) {
-  CTL_CHECK_ARG(out != nullptr && stage_blocks != nullptr, "null pointer");
-  CTL_CHECK_ARG(block == CTL_BLOCK_BOTTLENECK || block == CTL_BLOCK_BASIC,
-                "block = %d: expected CTL_BLOCK_BOTTLENECK (0) or CTL_BLOCK_BASIC (1)", block);
-  CTL_CHECK_ARG(block == CTL_BLOCK_BOTTLENECK || !ibn, "IBN-a is defined for bottleneck blocks only (resnet_ibn_a.py)");
-  CTL_CHECK_ARG(last_stride == 1 || last_stride == 2, "last_stride must be 1 or 2 (config/defaults.py:24)");
+int ctl_trainer_create(ctl_trainer** out, int32_t block, int32_t ibn, int32_t last_stride, float momentum,
+                       const int32_t stage_blocks[4]) {
+  CTL_CHECK_ARG(out != nullptr, "null pointer");
   CTL_CHECK_ARG(momentum > 0.f && momentum <= 1.f, "momentum must be in (0, 1]");
-  for (int li = 0; li < 4; ++li)
-    CTL_CHECK_ARG(stage_blocks[li] >= 1, "stage_blocks[%d] = %d: every stage needs at least one block", li, stage_blocks[li]);
   ctl_trainer* t = new ctl_trainer();
+  if (int rc = resnet_layout(block, ibn, last_stride, stage_blocks, &t->feature_dim, &t->blocks)) {
+    delete t;
+    return rc;
+  }
   t->block = block;
   t->ibn = ibn ? 1 : 0;
-  t->last_stride = last_stride;
   t->momentum = momentum;
-  const int planes[4] = {64, 128, 256, 512};
-  int inplanes = 64;
-  if (block == CTL_BLOCK_BASIC) {
-    t->feature_dim = 512;
-    // resnet.py:19-48,105-112: conv1 3x3 / stride, conv2 3x3; a downsample on the first block of layers 2-4
-    for (int li = 0; li < 4; ++li)
-      for (int bi = 0; bi < stage_blocks[li]; ++bi) {
-        TrainBlock b;
-        const std::string p = "layer" + std::to_string(li + 1) + "." + std::to_string(bi);
-        const int stride = bi == 0 ? (li == 0 ? 1 : (li == 3 ? last_stride : 2)) : 1;
-        b.c1.conv = p + ".conv1";
-        b.c1.bn = p + ".bn1";
-        b.c1.cin = inplanes;
-        b.c1.cout = planes[li];
-        b.c1.k = 3;
-        b.c1.stride = stride;
-        b.c2.conv = p + ".conv2";
-        b.c2.bn = p + ".bn2";
-        b.c2.cin = b.c2.cout = planes[li];
-        b.c2.k = 3;
-        b.has_down = stride != 1 || inplanes != planes[li];
-        if (b.has_down) {
-          b.down.conv = p + ".downsample.0";
-          b.down.bn = p + ".downsample.1";
-          b.down.cin = inplanes;
-          b.down.cout = planes[li];
-          b.down.stride = stride;
-          b.down.relu = 0;
-        }
-        inplanes = planes[li];
-        t->blocks.push_back(b);
-      }
-    *out = t;
-    return 0;
-  }
-  for (int li = 0; li < 4; ++li)
-    for (int bi = 0; bi < stage_blocks[li]; ++bi) {
-      TrainBlock b;
-      const std::string p = "layer" + std::to_string(li + 1) + "." + std::to_string(bi);
-      const int stride0 = li == 0 ? 1 : (li == 3 ? last_stride : 2);
-      b.c1.conv = p + ".conv1";
-      b.c1.bn = p + ".bn1";
-      b.c1.cin = inplanes;
-      b.c1.cout = planes[li];
-      b.c1.in_half = (t->ibn && planes[li] != 512) ? planes[li] / 2 : 0;  // resnet_ibn_a.py:116-119
-      b.c2.conv = p + ".conv2";
-      b.c2.bn = p + ".bn2";
-      b.c2.cin = b.c2.cout = planes[li];
-      b.c2.k = 3;
-      b.c2.stride = bi == 0 ? stride0 : 1;
-      b.c3.conv = p + ".conv3";
-      b.c3.bn = p + ".bn3";
-      b.c3.cin = planes[li];
-      b.c3.cout = planes[li] * 4;
-      b.has_down = bi == 0;
-      if (b.has_down) {
-        b.down.conv = p + ".downsample.0";
-        b.down.bn = p + ".downsample.1";
-        b.down.cin = inplanes;
-        b.down.cout = planes[li] * 4;
-        b.down.stride = b.c2.stride;
-        b.down.relu = 0;
-      }
-      inplanes = planes[li] * 4;
-      t->blocks.push_back(b);
-    }
   *out = t;
   return 0;
 }
@@ -527,33 +403,26 @@ int ctl_trainer_bind(ctl_trainer* t, const ctl_named_tensor* params, int32_t n_p
   CTL_CHECK_ARG(t && params && grads && n_params > 0 && n_grads > 0, "bad arguments");
   int rc = ctl_device_check();
   if (rc) return rc;
-  RefMap p, g;
-  for (int i = 0; i < n_params; ++i) {
-    CTL_CHECK_ARG(params[i].name != nullptr, "parameter %d has no name", i);
-    p[params[i].name] = Ref{const_cast<float*>(params[i].data), (long long)params[i].numel};
-  }
-  for (int i = 0; i < n_grads; ++i) {
-    CTL_CHECK_ARG(grads[i].name != nullptr, "gradient %d has no name", i);
-    g[grads[i].name] = Ref{grads[i].data, (long long)grads[i].numel};
-  }
+  NamedMap p, g;
+  if ((rc = index_named(params, n_params, "ctl_trainer_bind", "parameter", &p)) ||
+      (rc = index_named(grads, n_grads, "ctl_trainer_bind", "gradient", &g)))
+    return rc;
   t->bound = false;
   t->forwarded = false;
-  t->w0 = lookup(p, "conv1.weight", 64 * 147, true, "parameter", &rc);
-  t->g0 = lookup(p, "bn1.weight", 64, true, "parameter", &rc);
-  t->b0 = lookup(p, "bn1.bias", 64, true, "parameter", &rc);
-  t->rm0 = lookup(p, "bn1.running_mean", 64, false, "buffer", &rc);
-  t->rv0 = lookup(p, "bn1.running_var", 64, false, "buffer", &rc);
-  t->dw0 = lookup(g, "conv1.weight", 64 * 147, true, "gradient", &rc);
-  t->dg0 = lookup(g, "bn1.weight", 64, true, "gradient", &rc);
-  t->db0 = lookup(g, "bn1.bias", 64, true, "gradient", &rc);
+  t->w0 = lookup(p, "conv1.weight", 64 * 147, &rc, "parameter");
+  t->g0 = lookup(p, "bn1.weight", 64, &rc, "parameter");
+  t->b0 = lookup(p, "bn1.bias", 64, &rc, "parameter");
+  t->rm0 = lookup(p, "bn1.running_mean", 64, &rc, "buffer", false);
+  t->rv0 = lookup(p, "bn1.running_var", 64, &rc, "buffer", false);
+  t->dw0 = lookup(g, "conv1.weight", 64 * 147, &rc, "gradient");
+  t->dg0 = lookup(g, "bn1.weight", 64, &rc, "gradient");
+  t->db0 = lookup(g, "bn1.bias", 64, &rc, "gradient");
   if (rc) return rc;
   CTL_CHECK_ARG((t->rm0 == nullptr) == (t->rv0 == nullptr), "bn1 needs running_mean and running_var together (or neither)");
   size_t total = 0;
   int n_convs = 0;
-  const bool basic = t->block == CTL_BLOCK_BASIC;
   for (TrainBlock& b : t->blocks) {
-    ConvSpec* cs[4] = {&b.c1, &b.c2, basic ? nullptr : &b.c3, b.has_down ? &b.down : nullptr};
-    for (ConvSpec* c : cs) {
+    for (ConvSpec* c : b.state_dict_order()) {
       if (!c) continue;
       if ((rc = bind_conv(*c, p, g))) return rc;
       total += (size_t)c->cout * c->cin * c->k * c->k;
@@ -562,10 +431,10 @@ int ctl_trainer_bind(ctl_trainer* t, const ctl_named_tensor* params, int32_t n_p
   }
   // packed fp16 operands: [forward arena | data-gradient arena], refreshed by ctl_train_pack_weights every forward
   if (!t->arena) {
-    t->arena = t_alloc<__half>(t, 2 * total);
-    t->table = t_alloc<long long>(t, (size_t)n_convs * 6);
-    t->stem_w192 = t_alloc<__half>(t, 64 * 192);
-    t->zero_bias = t_alloc<float>(t, 2048);
+    t->arena = dev_alloc<__half>(t, 2 * total);
+    t->table = dev_alloc<long long>(t, (size_t)n_convs * 6);
+    t->stem_w192 = dev_alloc<__half>(t, 64 * 192);
+    t->zero_bias = dev_alloc<float>(t, 2048);
     if (!t->arena || !t->table || !t->stem_w192 || !t->zero_bias) {
       set_error("ctl_trainer_bind: out of device memory");
       return (int)cudaErrorMemoryAllocation;
@@ -577,9 +446,7 @@ int ctl_trainer_bind(ctl_trainer* t, const ctl_named_tensor* params, int32_t n_p
   size_t off = 0;
   long long chunks = 0;
   for (TrainBlock& b : t->blocks) {
-    // table order: state_dict order (conv1, conv2, [conv3], downsample.0)
-    ConvSpec* cs[4] = {&b.c1, &b.c2, basic ? nullptr : &b.c3, b.has_down ? &b.down : nullptr};
-    for (ConvSpec* c : cs) {
+    for (ConvSpec* c : b.state_dict_order()) {  // the table's order
       if (!c) continue;
       const size_t numel = (size_t)c->cout * c->cin * c->k * c->k;
       c->wf = t->arena + off;
@@ -590,7 +457,7 @@ int ctl_trainer_bind(ctl_trainer* t, const ctl_named_tensor* params, int32_t n_p
       rows.push_back((long long)c->cout | ((long long)c->cin << 32));
       rows.push_back((long long)c->k);
       rows.push_back(chunks);
-      chunks += (long long)((numel + TT_PACK_CHUNK - 1) / TT_PACK_CHUNK);
+      chunks += (long long)((numel + CTL_PACK_CHUNK - 1) / CTL_PACK_CHUNK);
       off += numel;
     }
   }
@@ -650,16 +517,13 @@ int ctl_train_saved(const ctl_trainer* t, int32_t index, const void** y, const v
   if (index == 0) {
     *y = t->y0;
     *z = t->z0;
-    const int32_t s[4] = {t->n, (t->H + 6 - 7) / 2 + 1, (t->W + 6 - 7) / 2 + 1, 64};
+    const int32_t s[4] = {t->n, stem_side(t->H), stem_side(t->W), 64};
     memcpy(nhwc, s, sizeof(s));
     return 0;
   }
   int32_t i = 1;
-  const bool basic = t->block == CTL_BLOCK_BASIC;
   for (const TrainBlock& b : t->blocks) {
-    // forward order
-    const ConvSpec* cs[4] = {&b.c1, basic ? nullptr : &b.c2, b.has_down ? &b.down : nullptr, basic ? &b.c2 : &b.c3};
-    for (const ConvSpec* c : cs) {
+    for (const ConvSpec* c : b.forward_order()) {
       if (!c || i++ != index) continue;
       *y = c->y;
       *z = c->z;

@@ -44,8 +44,8 @@ class TrunkEngine:
         self.ibn, self.last_stride, self.block = ibn, last_stride, block
         self.launches_per_forward = 0  # kernels launched by the last forward / forward_u8
         self._h = C.c_void_p()
-        N.check(N.lib().ctl_trunk_create_ex(C.byref(self._h), BLOCKS[block], int(ibn), int(last_stride),
-                                            (C.c_int32 * 4)(*layers)))
+        N.check(N.lib().ctl_trunk_create(C.byref(self._h), BLOCKS[block], int(ibn), int(last_stride),
+                                         (C.c_int32 * 4)(*layers)))
         self.feature_dim = N.lib().ctl_trunk_feature_dim(self._h)
         self.pack(state, bn_head)
 

@@ -21,9 +21,7 @@ from typing import Dict, List, Tuple
 import torch
 
 from ... import _native as N
-from .engine import BLOCKS
-
-R50_LAYERS = (3, 4, 6, 3)
+from .engine import BLOCKS, R50_LAYERS
 
 
 def _named(tensors: Dict[str, torch.Tensor]):
@@ -47,8 +45,8 @@ class TrunkTrainer:
         self.block = block
         self.last_stride, self.layers, self.grad_scale, self.momentum = last_stride, tuple(layers), float(grad_scale), momentum
         self._h = C.c_void_p()
-        N.check(N.lib().ctl_trainer_create_ex(C.byref(self._h), BLOCKS[block], int(ibn), int(last_stride), float(momentum),
-                                              (C.c_int32 * 4)(*self.layers)))
+        N.check(N.lib().ctl_trainer_create(C.byref(self._h), BLOCKS[block], int(ibn), int(last_stride), float(momentum),
+                                           (C.c_int32 * 4)(*self.layers)))
         self.feature_dim = N.lib().ctl_trainer_feature_dim(self._h)
         self._bound = None  # (name, data_ptr) of the bound parameters
         self._ws = None

@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define CTL_ABI_VERSION 3
+#define CTL_ABI_VERSION 4
 
 #define CTL_OK 0
 #define CTL_ERR_INVALID_ARGUMENT (-1)
@@ -458,12 +458,11 @@ int ctl_instnorm_relu_nhwc_f16(void* x, int32_t n, int32_t hw, int32_t c, int32_
  * Baseline.forward's pooling (modelling/baseline.py:91-96), ModelBase.validation_step / inference_utils._inference
  * (modelling/bases.py:169-177, inference/inference_utils.py:104-113).  This is the eval trunk's only driver;
  * modelling/backbones/engine.py::TrunkEngine is its ctypes form.
- *   ctl_trunk_create_ex: ResNet of `block` = CTL_BLOCK_BOTTLENECK (resnet.py:51-87) or CTL_BLOCK_BASIC (resnet.py:19-48)
+ *   ctl_trunk_create   : ResNet of `block` = CTL_BLOCK_BOTTLENECK (resnet.py:51-87) or CTL_BLOCK_BASIC (resnet.py:19-48)
  *                        blocks with `stage_blocks` blocks per stage (bottleneck: {3, 4, 6, 3} = ResNet50, {3, 4, 23, 3} =
  *                        ResNet101, {3, 8, 36, 3} = ResNet152; basic: {2, 2, 2, 2} = ResNet18, {3, 4, 6, 3} = ResNet34;
  *                        each >= 1), IBN-a when `ibn` != 0 (bottleneck only), MODEL.LAST_STRIDE 1 or 2.  An unknown
  *                        `block`, or a basic block with `ibn` != 0, is CTL_ERR_INVALID_ARGUMENT before any device work.
- *   ctl_trunk_create   : ctl_trunk_create_ex with block = CTL_BLOCK_BOTTLENECK.
  *   ctl_trunk_feature_dim: width of the trunk output and of the features below: 2048 (bottleneck) or 512 (basic).
  *                        Host only.
  *   ctl_weights_pack   : `tensors` = the reference's `base.*`-stripped state_dict as DEVICE fp32 pointers, by name
@@ -499,8 +498,7 @@ typedef struct ctl_named_tensor {
 } ctl_named_tensor;
 #define CTL_BLOCK_BOTTLENECK 0
 #define CTL_BLOCK_BASIC 1
-int ctl_trunk_create(ctl_trunk** out, int32_t ibn, int32_t last_stride, const int32_t stage_blocks[4]);
-int ctl_trunk_create_ex(ctl_trunk** out, int32_t block, int32_t ibn, int32_t last_stride, const int32_t stage_blocks[4]);
+int ctl_trunk_create(ctl_trunk** out, int32_t block, int32_t ibn, int32_t last_stride, const int32_t stage_blocks[4]);
 int32_t ctl_trunk_feature_dim(const ctl_trunk* h);
 void ctl_trunk_destroy(ctl_trunk* h);
 int ctl_weights_pack(ctl_trunk* h, const ctl_named_tensor* tensors, int32_t n_tensors, ctl_stream_t stream);
@@ -535,7 +533,9 @@ int ctl_conv2d_wgrad_nhwc_f16_ex(const void* x, int32_t n, int32_t h, int32_t w,
                                  float out_scale, int32_t param_layout, ctl_stream_t stream);
 /* Operand packs of every convolution of a training step in ONE launch: table = device array of
  * {const float* src [cout][cin][k][k]; void* fwd fp16 [cout][k][k][cin]; void* dgrad fp16 [cin][k][k][cout] with flipped
- * taps (may be NULL); int32 cout, cin, k, pad; int64 chunk_begin} (48 bytes; chunks of 8192 source elements). */
+ * taps (may be NULL); int32 cout, cin, k, pad; int64 chunk_begin} (48 bytes; chunk_begin = running sum of
+ * ceil(numel / CTL_PACK_CHUNK) over the preceding entries). */
+#define CTL_PACK_CHUNK 8192
 int ctl_train_pack_weights(const void* table_device, int32_t n_tensors, int64_t n_chunks, ctl_stream_t stream);
 
 /* BatchNorm2d with batch statistics (torch.nn.BatchNorm2d in train mode, resnet.py:72-85) over NHWC fp16
@@ -587,19 +587,16 @@ int ctl_upsample2_zero_nhwc_f16(const void* x, int32_t n, int32_t h, int32_t w, 
                                 ctl_stream_t stream);
 int ctl_stem_im2col_f16(const float* x_nchw, int32_t n, int32_t h, int32_t w, void* out, ctl_stream_t stream);
 
-/* ---- optimizer step (solver/build.py:9-47, train_ctl_model.py:155-159, modelling/bases.py:102-133) ---- */
-
 /* ---- train-mode trunk behind an opaque handle (SURVEY 8b: the train forward / backward variants) ----
  * replaces: torch autograd through ResNet.forward / ResNet_IBN.forward in train mode (modelling/backbones/resnet.py:67-87,
  * 122-133, resnet_ibn_a.py:18-32,126-141) + Baseline.forward's pooling (modelling/baseline.py:91-96) inside
  * CTLModel.training_step (train_ctl_model.py:38-179): x -> global_feat [n][feature_dim], then d(loss)/d(global_feat) ->
  * every parameter gradient.  This is the training trunk's only driver; modelling/backbones/engine_train.py::TrunkTrainer
  * is its ctypes form.
- *   ctl_trainer_create_ex   : ResNet of `block` (CTL_BLOCK_BOTTLENECK or CTL_BLOCK_BASIC) blocks with `stage_blocks`
+ *   ctl_trainer_create      : ResNet of `block` (CTL_BLOCK_BOTTLENECK or CTL_BLOCK_BASIC) blocks with `stage_blocks`
  *                             blocks per stage ({3, 4, 6, 3} = ResNet50 / ResNet34, {3, 4, 23, 3} = ResNet101,
  *                             {2, 2, 2, 2} = ResNet18, each >= 1), IBN-a when `ibn` != 0 (bottleneck only),
- *                             MODEL.LAST_STRIDE 1 or 2, BatchNorm momentum.  Argument errors as ctl_trunk_create_ex.
- *   ctl_trainer_create      : ctl_trainer_create_ex with block = CTL_BLOCK_BOTTLENECK.
+ *                             MODEL.LAST_STRIDE 1 or 2, BatchNorm momentum in (0, 1].  Argument errors as ctl_trunk_create.
  *   ctl_trainer_feature_dim : 2048 (bottleneck) or 512 (basic).  Host only.
  *   ctl_trainer_bind        : `params` = the `base.*`-stripped fp32 parameters AND BatchNorm running buffers as device
  *                             pointers, by name (running_mean / running_var optional per layer, updated in place like
@@ -625,9 +622,8 @@ typedef struct ctl_named_buffer {
   float* data; /* device pointer, written */
   int64_t numel;
 } ctl_named_buffer;
-int ctl_trainer_create(ctl_trainer** out, int32_t ibn, int32_t last_stride, float momentum, const int32_t stage_blocks[4]);
-int ctl_trainer_create_ex(ctl_trainer** out, int32_t block, int32_t ibn, int32_t last_stride, float momentum,
-                          const int32_t stage_blocks[4]);
+int ctl_trainer_create(ctl_trainer** out, int32_t block, int32_t ibn, int32_t last_stride, float momentum,
+                       const int32_t stage_blocks[4]);
 int32_t ctl_trainer_feature_dim(const ctl_trainer* t);
 void ctl_trainer_destroy(ctl_trainer* t);
 int ctl_trainer_bind(ctl_trainer* t, const ctl_named_tensor* params, int32_t n_params, const ctl_named_buffer* grads,
@@ -638,6 +634,8 @@ int ctl_train_forward(ctl_trainer* t, const float* x_nchw, int32_t n, int32_t he
 int ctl_train_backward(ctl_trainer* t, const float* dfeat, float grad_scale, void* workspace, size_t workspace_bytes,
                        ctl_stream_t stream);
 int ctl_train_saved(const ctl_trainer* t, int32_t index, const void** y, const void** z, int32_t nhwc[4]);
+
+/* ---- optimizer step (solver/build.py:9-47, train_ctl_model.py:155-159, modelling/bases.py:102-133) ---- */
 
 /* One table entry per parameter tensor, resident on the device; chunk_begin = running sum of
  * ceil(numel / CTL_OPT_CHUNK) over the preceding entries. */

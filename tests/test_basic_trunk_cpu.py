@@ -83,21 +83,23 @@ def test_basic_params_state_dict_matches_reference(tag, name):
         ResNetParams(1, B.BASIC_LAYERS[name], ibn=True, block="basic")
 
 
-def test_ex_create_argument_errors_without_a_gpu():
-    """Unknown block kinds and IBN-a BasicBlocks are rejected by both _ex entry points before any device work; the
-    plain create calls are the bottleneck form of _ex; feature_dim is a host query."""
+def test_create_argument_errors_without_a_gpu():
+    """Unknown block kinds, IBN-a BasicBlocks and a last stride of 3 are rejected by both create calls before any device
+    work; feature_dim is a host query of the block kind."""
     from ctl_b200 import _native as N
 
     L = N.lib()
     r18 = (C.c_int32 * 4)(2, 2, 2, 2)
     cases = [
-        lambda: L.ctl_trunk_create_ex(C.byref(C.c_void_p()), 2, 0, 1, r18),                 # unknown block
-        lambda: L.ctl_trunk_create_ex(C.byref(C.c_void_p()), -1, 0, 1, r18),                # unknown block
-        lambda: L.ctl_trunk_create_ex(C.byref(C.c_void_p()), N.CTL_BLOCK_BASIC, 1, 1, r18),  # basic + IBN
-        lambda: L.ctl_trunk_create_ex(C.byref(C.c_void_p()), N.CTL_BLOCK_BASIC, 0, 3, r18),  # LAST_STRIDE 3
-        lambda: L.ctl_trainer_create_ex(C.byref(C.c_void_p()), 2, 0, 1, 0.1, r18),
-        lambda: L.ctl_trainer_create_ex(C.byref(C.c_void_p()), N.CTL_BLOCK_BASIC, 1, 1, 0.1, r18),
-        lambda: L.ctl_trainer_create_ex(C.byref(C.c_void_p()), N.CTL_BLOCK_BASIC, 0, 1, 0.0, r18),  # momentum 0
+        lambda: L.ctl_trunk_create(C.byref(C.c_void_p()), 2, 0, 1, r18),                          # unknown block
+        lambda: L.ctl_trunk_create(C.byref(C.c_void_p()), -1, 0, 1, r18),                         # unknown block
+        lambda: L.ctl_trunk_create(C.byref(C.c_void_p()), N.CTL_BLOCK_BASIC, 1, 1, r18),           # basic + IBN
+        lambda: L.ctl_trunk_create(C.byref(C.c_void_p()), N.CTL_BLOCK_BASIC, 0, 3, r18),           # LAST_STRIDE 3
+        lambda: L.ctl_trainer_create(C.byref(C.c_void_p()), 2, 0, 1, 0.1, r18),                   # unknown block
+        lambda: L.ctl_trainer_create(C.byref(C.c_void_p()), -1, 0, 1, 0.1, r18),                  # unknown block
+        lambda: L.ctl_trainer_create(C.byref(C.c_void_p()), N.CTL_BLOCK_BASIC, 1, 1, 0.1, r18),    # basic + IBN
+        lambda: L.ctl_trainer_create(C.byref(C.c_void_p()), N.CTL_BLOCK_BASIC, 0, 3, 0.1, r18),    # LAST_STRIDE 3
+        lambda: L.ctl_trainer_create(C.byref(C.c_void_p()), N.CTL_BLOCK_BASIC, 0, 1, 0.0, r18),    # momentum 0
         lambda: L.ctl_conv3x3_dual_nhwc_f16(C.c_void_p(16), 64, C.c_void_p(16), 7, 8, 64, 2, 1, C.c_void_p(16),
                                             C.c_void_p(16), C.c_void_p(16), 128, 1, None),     # odd H2, stride 2
     ]
@@ -109,8 +111,8 @@ def test_ex_create_argument_errors_without_a_gpu():
             N.check(rc)
     for block, dim in ((N.CTL_BLOCK_BOTTLENECK, 2048), (N.CTL_BLOCK_BASIC, 512)):
         h, t = C.c_void_p(), C.c_void_p()
-        assert L.ctl_trunk_create_ex(C.byref(h), block, 0, 1, r18) == 0
-        assert L.ctl_trainer_create_ex(C.byref(t), block, 0, 1, 0.1, r18) == 0
+        assert L.ctl_trunk_create(C.byref(h), block, 0, 1, r18) == 0
+        assert L.ctl_trainer_create(C.byref(t), block, 0, 1, 0.1, r18) == 0
         assert L.ctl_trunk_feature_dim(h) == dim and L.ctl_trainer_feature_dim(t) == dim
         L.ctl_trunk_destroy(h)
         L.ctl_trainer_destroy(t)
@@ -127,8 +129,8 @@ def test_basic_handles_plan_their_workspace_without_a_gpu():
     ev, tr = {}, {}
     for name, layers in B.BASIC_LAYERS.items():
         h, t = C.c_void_p(), C.c_void_p()
-        assert L.ctl_trunk_create_ex(C.byref(h), N.CTL_BLOCK_BASIC, 0, 1, (C.c_int32 * 4)(*layers)) == 0
-        assert L.ctl_trainer_create_ex(C.byref(t), N.CTL_BLOCK_BASIC, 0, 1, 0.1, (C.c_int32 * 4)(*layers)) == 0
+        assert L.ctl_trunk_create(C.byref(h), N.CTL_BLOCK_BASIC, 0, 1, (C.c_int32 * 4)(*layers)) == 0
+        assert L.ctl_trainer_create(C.byref(t), N.CTL_BLOCK_BASIC, 0, 1, 0.1, (C.c_int32 * 4)(*layers)) == 0
         ev[name], tr[name] = L.ctl_embed_workspace_bytes(h, n, H, W), L.ctl_train_workspace_bytes(t, n, H, W)
         slot = n * hp * wp * 64 * 2
         # three slots of layer1's output; the tensor-core stem's temporary [n, 128, 64, 64] starts at slot 1
@@ -140,7 +142,7 @@ def test_basic_handles_plan_their_workspace_without_a_gpu():
     assert 0 < tr["resnet18"] < tr["resnet34"]
     assert 0 < ev["resnet18"] <= ev["resnet34"]
     hb = C.c_void_p()
-    assert L.ctl_trunk_create_ex(C.byref(hb), N.CTL_BLOCK_BOTTLENECK, 0, 1, (C.c_int32 * 4)(3, 4, 6, 3)) == 0
+    assert L.ctl_trunk_create(C.byref(hb), N.CTL_BLOCK_BOTTLENECK, 0, 1, (C.c_int32 * 4)(3, 4, 6, 3)) == 0
     assert ev["resnet34"] < L.ctl_embed_workspace_bytes(hb, n, H, W)
     L.ctl_trunk_destroy(hb)
 

@@ -90,6 +90,7 @@ def test_c_abi_argument_errors_are_reported_without_a_gpu():
     L = N.lib()
     one = C.c_void_p(16)  # a non-null, 16-byte-aligned dummy pointer: argument checks come before any dereference
     r50 = (C.c_int32 * 4)(3, 4, 6, 3)
+    B = N.CTL_BLOCK_BOTTLENECK
     cases = [
         lambda: L.ctl_conv2d_nhwc_f16(one, 1, 8, 8, 48, one, one, None, one, 64, 1, 1, 0, 0, None),          # Cin % 64
         lambda: L.ctl_conv2d_nhwc_f16(one, 1, 8, 8, 64, one, one, None, one, 64, 5, 1, 0, 0, None),          # 5x5
@@ -108,13 +109,17 @@ def test_c_abi_argument_errors_are_reported_without_a_gpu():
         lambda: L.ctl_loss_scale_update(one, one, one, one, 1024.0, 0.5, 0.5, 2000, None),                    # growth < 1
         lambda: L.ctl_conv1x1_dual_nhwc_f16(one, 64, one, 7, 8, 64, 2, 1, one, one, one, 256, 1, None),       # odd H2, stride 2
         lambda: L.ctl_augment_batch_u8(one, 1, 8, 8, -1, one, (C.c_float * 3)(0, 0, 0), (C.c_float * 3)(1, 1, 1), one, None),
-        lambda: L.ctl_trainer_create(C.byref(C.c_void_p()), 0, 3, 0.1, r50),                                 # LAST_STRIDE 3
-        lambda: L.ctl_trainer_create(C.byref(C.c_void_p()), 0, 1, 0.0, r50),                                 # momentum 0
-        lambda: L.ctl_trainer_create(C.byref(C.c_void_p()), 0, 1, 0.1, (C.c_int32 * 4)(3, 0, 6, 3)),         # empty stage
-        lambda: L.ctl_trunk_create(None, 0, 1, r50),                                                          # null handle
-        lambda: L.ctl_trunk_create(C.byref(C.c_void_p()), 0, 1, None),                                       # null stages
-        lambda: L.ctl_trunk_create(C.byref(C.c_void_p()), 0, 3, r50),                                        # LAST_STRIDE 3
-        lambda: L.ctl_trunk_create(C.byref(C.c_void_p()), 0, 1, (C.c_int32 * 4)(3, 4, 0, 3)),                # empty stage
+        lambda: L.ctl_trainer_create(C.byref(C.c_void_p()), B, 0, 3, 0.1, r50),                              # LAST_STRIDE 3
+        lambda: L.ctl_trainer_create(C.byref(C.c_void_p()), B, 0, 1, 0.0, r50),                              # momentum 0
+        lambda: L.ctl_trainer_create(C.byref(C.c_void_p()), B, 0, 1, 0.1, (C.c_int32 * 4)(3, 0, 6, 3)),      # empty stage
+        lambda: L.ctl_trainer_create(C.byref(C.c_void_p()), B, 0, 1, 0.1, (C.c_int32 * 4)(3, 4, 0, 3)),      # empty stage
+        lambda: L.ctl_trainer_create(None, B, 0, 1, 0.1, r50),                                               # null handle
+        lambda: L.ctl_trainer_create(C.byref(C.c_void_p()), B, 0, 1, 0.1, None),                             # null stages
+        lambda: L.ctl_trunk_create(None, B, 0, 1, r50),                                                       # null handle
+        lambda: L.ctl_trunk_create(C.byref(C.c_void_p()), B, 0, 1, None),                                    # null stages
+        lambda: L.ctl_trunk_create(C.byref(C.c_void_p()), B, 0, 3, r50),                                     # LAST_STRIDE 3
+        lambda: L.ctl_trunk_create(C.byref(C.c_void_p()), B, 0, 1, (C.c_int32 * 4)(3, 0, 6, 3)),             # empty stage
+        lambda: L.ctl_trunk_create(C.byref(C.c_void_p()), B, 0, 1, (C.c_int32 * 4)(3, 4, 0, 3)),             # empty stage
     ]
     for i, call in enumerate(cases):
         rc = call()
@@ -136,8 +141,8 @@ def test_trainer_handle_plans_its_workspace_without_a_gpu():
     L = N.lib()
     for ibn in (0, 1):
         h, h101 = C.c_void_p(), C.c_void_p()
-        assert L.ctl_trainer_create(C.byref(h), ibn, 1, 0.1, (C.c_int32 * 4)(3, 4, 6, 3)) == 0
-        assert L.ctl_trainer_create(C.byref(h101), ibn, 1, 0.1, (C.c_int32 * 4)(3, 4, 23, 3)) == 0
+        assert L.ctl_trainer_create(C.byref(h), N.CTL_BLOCK_BOTTLENECK, ibn, 1, 0.1, (C.c_int32 * 4)(3, 4, 6, 3)) == 0
+        assert L.ctl_trainer_create(C.byref(h101), N.CTL_BLOCK_BOTTLENECK, ibn, 1, 0.1, (C.c_int32 * 4)(3, 4, 23, 3)) == 0
         b16, b32 = L.ctl_train_workspace_bytes(h, 16, 256, 128), L.ctl_train_workspace_bytes(h, 32, 256, 128)
         assert b16 > 0 and 1.8 < b32 / b16 < 2.05
         # saved y + z alone: ~29 MB per 256x128 image (fp16), the whole step stays below 3x that
@@ -162,7 +167,7 @@ def test_trunk_handle_stage_calls_check_arguments_without_a_gpu():
     L = N.lib()
     one = C.c_void_p(256)
     h = C.c_void_p()
-    assert L.ctl_trunk_create(C.byref(h), 0, 1, (C.c_int32 * 4)(3, 4, 6, 3)) == 0
+    assert L.ctl_trunk_create(C.byref(h), N.CTL_BLOCK_BOTTLENECK, 0, 1, (C.c_int32 * 4)(3, 4, 6, 3)) == 0
     try:
         n, H, W, hp, wp = 2, 256, 128, 64, 32
         need = L.ctl_embed_workspace_bytes(h, n, H, W)
