@@ -966,7 +966,8 @@ __global__ void __launch_bounds__(S3_THREADS, 1) stem_pool_kernel(const __grid_c
   }
 }
 
-// maxpool 3x3 / 2, pad 1, NHWC fp16; one thread = 8 channels of one output pixel
+// maxpool 3x3 / 2, pad 1, NHWC fp16; one thread = 8 channels of one output pixel.  Every window has an in-bounds tap,
+// so starting from -inf returns -inf only for a window of -inf inputs, as F.max_pool2d does.
 __global__ void __launch_bounds__(256) maxpool3x3s2_kernel(const __half* __restrict__ x, int N, int H, int W, int C,
                                                            __half* __restrict__ out, int Ho, int Wo) {
   pdl_launch_dependents();
@@ -982,7 +983,7 @@ __global__ void __launch_bounds__(256) maxpool3x3s2_kernel(const __half* __restr
   const int oh = (int)(t % Ho);
   const int n = (int)(t / Ho);
   __half2 m[4];
-  const __half2 neg = __float2half2_rn(-65504.f);
+  const __half2 neg = __float2half2_rn(-INFINITY);
 #pragma unroll
   for (int j = 0; j < 4; ++j) m[j] = neg;
   for (int r = 0; r < 3; ++r) {
@@ -1031,68 +1032,6 @@ __global__ void __launch_bounds__(256) gap_bn_kernel(const __half* __restrict__ 
   if (emb) {
     emb[(size_t)n * C + 2 * c2] = __fmaf_rn(f0, bn_scale[2 * c2], bn_shift[2 * c2]);
     emb[(size_t)n * C + 2 * c2 + 1] = __fmaf_rn(f1, bn_scale[2 * c2 + 1], bn_shift[2 * c2 + 1]);
-  }
-}
-
-// InstanceNorm2d(affine, instance statistics) + ReLU in place on channels [0, half) of an NHWC
-// fp16 tensor (IBN, resnet_ibn_a.py:18-32): one block per (image, 8-channel group).
-__global__ void __launch_bounds__(256) instnorm_relu_kernel(__half* __restrict__ x, int HW, int C, int half,
-                                                            const float* __restrict__ gamma,
-                                                            const float* __restrict__ beta, float eps) {
-  pdl_launch_dependents();
-  pdl_wait();
-  __shared__ float s_sum[8][8], s_sq[8][8];
-  __shared__ float s_mean[8], s_istd[8];
-  const int n = blockIdx.y, c0 = blockIdx.x * 8;
-  if (c0 >= half) return;
-  __half* base = x + (size_t)n * HW * C + c0;
-  float s[8] = {}, q[8] = {};
-  for (int p = threadIdx.x; p < HW; p += blockDim.x) {
-    const uint4 v = *reinterpret_cast<const uint4*>(base + (size_t)p * C);
-    const __half2* hv = reinterpret_cast<const __half2*>(&v);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float2 f = __half22float2(hv[j]);
-      s[2 * j] += f.x; q[2 * j] = __fmaf_rn(f.x, f.x, q[2 * j]);
-      s[2 * j + 1] += f.y; q[2 * j + 1] = __fmaf_rn(f.y, f.y, q[2 * j + 1]);
-    }
-  }
-  const int lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      s[j] += __shfl_xor_sync(0xffffffffu, s[j], o);
-      q[j] += __shfl_xor_sync(0xffffffffu, q[j], o);
-    }
-    if (lane == 0) { s_sum[wp][j] = s[j]; s_sq[wp][j] = q[j]; }
-  }
-  __syncthreads();
-  if (threadIdx.x < 8) {
-    float ts = 0.f, tq = 0.f;
-    for (int w = 0; w < 8; ++w) { ts += s_sum[w][threadIdx.x]; tq += s_sq[w][threadIdx.x]; }
-    const float mean = ts / (float)HW;
-    const float var = fmaxf(tq / (float)HW - mean * mean, 0.f);  // biased, like F.instance_norm
-    s_mean[threadIdx.x] = mean;
-    s_istd[threadIdx.x] = rsqrtf(var + eps);
-  }
-  __syncthreads();
-  float sc[8], sh[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    sc[j] = gamma[c0 + j] * s_istd[j];
-    sh[j] = beta[c0 + j] - s_mean[j] * sc[j];
-  }
-  for (int p = threadIdx.x; p < HW; p += blockDim.x) {
-    uint4 v = *reinterpret_cast<const uint4*>(base + (size_t)p * C);
-    __half2* hv = reinterpret_cast<__half2*>(&v);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float2 f = __half22float2(hv[j]);
-      hv[j] = __floats2half2_rn(fmaxf(__fmaf_rn(f.x, sc[2 * j], sh[2 * j]), 0.f),
-                                fmaxf(__fmaf_rn(f.y, sc[2 * j + 1], sh[2 * j + 1]), 0.f));
-    }
-    *reinterpret_cast<uint4*>(base + (size_t)p * C) = v;
   }
 }
 
@@ -1528,18 +1467,6 @@ int ctl_gap_bn_nhwc_f16(const void* x, int32_t n, int32_t hw, int32_t c, const f
   dim3 grid((c / 2 + 255) / 256, n);
   CTL_CUDA(launch_k(gap_bn_kernel, grid, dim3(256), 0, (cudaStream_t)stream, static_cast<const __half*>(x), (int)hw, (int)c,
                     bn_scale, bn_shift, feat, emb));
-  CTL_LAUNCH_CHECK();
-  return 0;
-}
-
-int ctl_instnorm_relu_nhwc_f16(void* x, int32_t n, int32_t hw, int32_t c, int32_t half, const float* gamma,
-                               const float* beta, float eps, ctl_stream_t stream) {
-  CTL_CHECK_ARG(x && gamma && beta && half % 8 == 0 && half <= c && c % 8 == 0, "bad arguments");
-  int rc = ctl_device_check();
-  if (rc) return rc;
-  dim3 grid(half / 8, n);
-  CTL_CUDA(launch_k(instnorm_relu_kernel, grid, dim3(256), 0, (cudaStream_t)stream, static_cast<__half*>(x), (int)hw, (int)c,
-                    (int)half, gamma, beta, eps));
   CTL_LAUNCH_CHECK();
   return 0;
 }

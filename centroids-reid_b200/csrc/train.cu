@@ -349,6 +349,9 @@ __device__ __forceinline__ void unpack8(const uint4& v, float (&f)[8]) {
     f[2 * i + 1] = t.y;
   }
 }
+// a 16-byte load by value: unpack8 of a dereferenced global pointer reads the four __half2 one by one
+__device__ __forceinline__ uint4 ldg16(const __half* p) { return *reinterpret_cast<const uint4*>(p); }
+
 __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
   uint4 v;
   __half2* h = reinterpret_cast<__half2*>(&v);
@@ -686,31 +689,80 @@ __device__ __forceinline__ void in_block_reduce(float (&acc)[2][8], float* sred 
   __syncthreads();
 }
 
-// Block reduction of per-thread (count, mean, M2 = sum of squared deviations) of 8 channels by Chan's pairwise update,
-// in a fixed tree order (deterministic).  Returns the block's mean and M2 to every thread.
-__device__ __forceinline__ void in_block_welford(float cnt, float (&mean)[8], float (&m2)[8], float* sred /* [256][16] */,
-                                                 float* scnt /* [256] */) {
+// Chan's pairwise update: (na, ma, m2a) becomes the count, mean and M2 of both parts
+__device__ __forceinline__ void in_chan_merge(float& na, float nb, float (&ma)[8], float (&m2a)[8], const float (&mb)[8],
+                                              const float (&m2b)[8]) {
+  const float nab = na + nb, wb = nb * __frcp_rn(nab);
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
-    sred[threadIdx.x * 16 + i] = mean[i];
-    sred[threadIdx.x * 16 + 8 + i] = m2[i];
+    const float d = mb[i] - ma[i];
+    ma[i] = fmaf(d, wb, ma[i]);
+    m2a[i] += m2b[i] + d * d * na * wb;
   }
-  scnt[threadIdx.x] = cnt;
+  na = nab;
+}
+
+// Block reduction of per-thread (count, mean, M2 = sum of squared deviations) of 8 channels by Chan's pairwise update,
+// in a fixed tree order (deterministic): thread t takes in t + off for off = 128, 64, .., 1, the three cross-warp levels
+// through shared memory (value-major, so a warp's accesses hit 32 banks) and the five in-warp levels in warp 0 through
+// shuffles.  Returns the block's mean and M2 to every thread.
+__device__ __forceinline__ void in_block_welford(float cnt, float (&mean)[8], float (&m2)[8], float* sred /* [16][256] */,
+                                                 float* scnt /* [256] */) {
+  const int t = threadIdx.x;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    sred[i * 256 + t] = mean[i];
+    sred[(8 + i) * 256 + t] = m2[i];
+  }
+  scnt[t] = cnt;
   __syncthreads();
-  for (int off = 128; off > 0; off >>= 1) {
-    const int t = threadIdx.x;
+  for (int off = 128; off >= 32; off >>= 1) {
     if (t < off && scnt[t + off] > 0.f) {
-      const float na = scnt[t], nb = scnt[t + off], nab = na + nb, wb = nb * __frcp_rn(nab);
+      float mb[8], m2b[8];
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
-        const float ma = sred[t * 16 + i], d = sred[(t + off) * 16 + i] - ma;
-        sred[t * 16 + i] = fmaf(d, wb, ma);
-        sred[t * 16 + 8 + i] += sred[(t + off) * 16 + 8 + i] + d * d * na * wb;
+        mean[i] = sred[i * 256 + t];
+        m2[i] = sred[(8 + i) * 256 + t];
+        mb[i] = sred[i * 256 + t + off];
+        m2b[i] = sred[(8 + i) * 256 + t + off];
       }
-      scnt[t] = nab;
+      float na = scnt[t];
+      in_chan_merge(na, scnt[t + off], mean, m2, mb, m2b);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        sred[i * 256 + t] = mean[i];
+        sred[(8 + i) * 256 + t] = m2[i];
+      }
+      scnt[t] = na;
     }
     __syncthreads();
   }
+  if (t < 32) {
+    float na = scnt[t];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      mean[i] = sred[i * 256 + t];
+      m2[i] = sred[(8 + i) * 256 + t];
+    }
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+      const float nb = __shfl_down_sync(0xffffffffu, na, off);
+      float mb[8], m2b[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        mb[i] = __shfl_down_sync(0xffffffffu, mean[i], off);
+        m2b[i] = __shfl_down_sync(0xffffffffu, m2[i], off);
+      }
+      if (t < off && nb > 0.f) in_chan_merge(na, nb, mean, m2, mb, m2b);
+    }
+    if (t == 0)
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        sred[i] = mean[i];
+        sred[8 + i] = m2[i];
+      }
+  }
+  __syncthreads();
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
     mean[i] = sred[i];
@@ -721,11 +773,12 @@ __device__ __forceinline__ void in_block_welford(float cnt, float (&mean)[8], fl
 
 // statistics in ONE pass over the instance with Welford's update per thread and Chan's combination across threads (the
 // update PyTorch's own normalisation kernels use), not E[y^2] - mean^2, which cancels catastrophically in fp32 when
-// |mean| >> std
-__global__ void __launch_bounds__(256) in_train_forward_kernel(const __half* __restrict__ y, int HW, int pitch, int half,
+// |mean| >> std.  The eval trunk runs it in place (out == y, each thread rewrites only the rows it read) without saving
+// the statistics (save_mean == save_invstd == nullptr).
+__global__ void __launch_bounds__(256) in_train_forward_kernel(const __half* y, int HW, int pitch, int half,
                                                                const float* __restrict__ gamma, const float* __restrict__ beta,
                                                                float eps, float* __restrict__ save_mean,
-                                                               float* __restrict__ save_invstd, __half* __restrict__ out) {
+                                                               float* __restrict__ save_invstd, __half* out) {
   pdl_launch_dependents();
   pdl_wait();
   __shared__ float sred[256 * 16];
@@ -737,7 +790,7 @@ __global__ void __launch_bounds__(256) in_train_forward_kernel(const __half* __r
   for (int i = 0; i < 8; ++i) m[i] = m2[i] = 0.f;
   for (int r = threadIdx.x; r < HW; r += blockDim.x) {
     float f[8];
-    unpack8(*reinterpret_cast<const uint4*>(y + base + (size_t)r * pitch), f);
+    unpack8(ldg16(y + base + (size_t)r * pitch), f);
     cnt += 1.f;
     const float inv = __frcp_rn(cnt);
 #pragma unroll
@@ -755,14 +808,14 @@ __global__ void __launch_bounds__(256) in_train_forward_kernel(const __half* __r
     const float is = rsqrtf(var + eps);
     sc[i] = gamma[g * 8 + i] * is;
     sh[i] = beta[g * 8 + i] - m[i] * sc[i];
-    if (threadIdx.x == 0) {
+    if (threadIdx.x == 0 && save_mean) {
       save_mean[(size_t)n * half + g * 8 + i] = m[i];
       save_invstd[(size_t)n * half + g * 8 + i] = is;
     }
   }
   for (int r = threadIdx.x; r < HW; r += blockDim.x) {
     float f[8];
-    unpack8(*reinterpret_cast<const uint4*>(y + base + (size_t)r * pitch), f);
+    unpack8(ldg16(y + base + (size_t)r * pitch), f);
 #pragma unroll
     for (int i = 0; i < 8; ++i) f[i] = fmaxf(fmaf(f[i], sc[i], sh[i]), 0.f);
     *reinterpret_cast<uint4*>(out + base + (size_t)r * pitch) = pack8(f);
@@ -1265,7 +1318,8 @@ int ctl_bn_train_backward_nhwc_f16(const void* dz, const void* z, const void* y,
 int ctl_instnorm_train_forward_nhwc_f16(const void* y, int32_t n, int32_t hw, int32_t pitch, int32_t half, const float* gamma,
                                         const float* beta, float eps, float* save_mean, float* save_invstd, void* out,
                                         ctl_stream_t stream) {
-  CTL_CHECK_ARG(y && gamma && beta && save_mean && save_invstd && out, "null pointer");
+  CTL_CHECK_ARG(y && gamma && beta && out, "null pointer");
+  CTL_CHECK_ARG(!save_mean == !save_invstd, "save_mean and save_invstd are both given or both null");
   CTL_CHECK_ARG(n >= 1 && hw >= 1 && half >= 8 && half % 8 == 0 && pitch >= half && pitch % 8 == 0, "bad shape");
   int rc = ctl_device_check();
   if (rc) return rc;
@@ -1273,6 +1327,11 @@ int ctl_instnorm_train_forward_nhwc_f16(const void* y, int32_t n, int32_t hw, in
                     static_cast<const __half*>(y), (int)hw, (int)pitch, (int)half, gamma, beta, eps, save_mean, save_invstd,
                     static_cast<__half*>(out)));
   return 0;
+}
+
+int ctl_instnorm_relu_nhwc_f16(void* x, int32_t n, int32_t hw, int32_t c, int32_t half, const float* gamma,
+                               const float* beta, float eps, ctl_stream_t stream) {
+  return ctl_instnorm_train_forward_nhwc_f16(x, n, hw, c, half, gamma, beta, eps, nullptr, nullptr, x, stream);
 }
 
 int ctl_instnorm_train_backward_nhwc_f16(void* dz, const void* z, const void* y, int32_t n, int32_t hw, int32_t pitch,

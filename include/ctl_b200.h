@@ -559,7 +559,8 @@ int ctl_bn_train_backward_nhwc_f16(const void* dz, const void* z, const void* y,
                                    ctl_stream_t stream);
 /* InstanceNorm2d(affine) + ReLU of an IBN layer's first `half` channels in train mode (resnet_ibn_a.py:18-32): y, out,
  * dz, z, dy are NHWC fp16 with rows of `pitch` elements ([n][hw][pitch]); instance statistics (biased variance) per
- * (image, channel) are saved as [n][half] fp32.  backward: g = dz * (z > 0) is written back over dz; dgamma_part /
+ * (image, channel) are saved as [n][half] fp32, unless save_mean and save_invstd are both null; out may equal y (in place,
+ * as ctl_instnorm_relu_nhwc_f16 runs it).  backward: g = dz * (z > 0) is written back over dz; dgamma_part /
  * dbeta_part are per-image partials [n][half] (sum over n = the parameter gradient), multiplied by grad_unscale. */
 int ctl_instnorm_train_forward_nhwc_f16(const void* y, int32_t n, int32_t hw, int32_t pitch, int32_t half, const float* gamma,
                                         const float* beta, float eps, float* save_mean, float* save_invstd, void* out,

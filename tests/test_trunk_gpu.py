@@ -117,62 +117,6 @@ def test_conv_relu_from_channel():
     _conv_case(2, 32, 16, 256, 128, 1, 1, True, False, relu_from=64, seed=3)
 
 
-def test_stem_tc_maxpool_gap_instnorm():
-    from ctl_b200 import _native as N
-
-    L = N.lib()
-    g = torch.Generator().manual_seed(5)
-    n, H, W = 3, 64, 48
-    x = torch.randn(n, 3, H, W, generator=g)
-    w = torch.randn(64, 3, 7, 7, generator=g) * 0.1
-    b = torch.randn(64, generator=g) * 0.1
-    for relu in (0, 1):
-        ref16 = F.conv2d(x.half().double(), w.half().double(), b.double(), 2, 3)
-        if relu:
-            ref16 = ref16.clamp(min=0)
-        ho, wo = ref16.shape[2:]
-        xd, bd = x.cuda(), b.cuda()  # keep the device buffers alive across the call
-        # tensor-core stem: fp16 operands ([64][192] weights, k = (c*7 + r)*8 + s), fp32 accumulate
-        wk192 = torch.zeros(64, 21, 8)
-        wk192[:, :, :7] = w.reshape(64, 21, 7)
-        wk192 = torch.cat((wk192.reshape(64, 168), torch.zeros(64, 24)), 1).half().cuda()
-        out_tc = torch.full((n, ho, wo, 64), float("nan"), dtype=torch.float16, device="cuda")
-        N.check(L.ctl_stem_conv7x7_tc(xd.data_ptr(), n, H, W, wk192.data_ptr(), bd.data_ptr(), relu,
-                                      out_tc.data_ptr(), N.stream_ptr()))
-        torch.cuda.synchronize()
-        got_tc = out_tc.cpu().double().permute(0, 3, 1, 2)
-        assert torch.isfinite(got_tc).all()
-        assert float((got_tc - ref16).abs().max()) <= float(ref16.abs().max()) * 2.0 ** -10 + 1e-4
-    s = out_tc  # relu'd stem output, NHWC fp16
-    hp, wp = (ho + 2 - 3) // 2 + 1, (wo + 2 - 3) // 2 + 1
-    pooled = torch.empty(n, hp, wp, 64, dtype=torch.float16, device="cuda")
-    N.check(L.ctl_maxpool3x3s2_nhwc_f16(s.data_ptr(), n, ho, wo, 64, pooled.data_ptr(), N.stream_ptr()))
-    refp = F.max_pool2d(s.cpu().float().permute(0, 3, 1, 2), 3, 2, 1).permute(0, 2, 3, 1)
-    assert torch.equal(pooled.cpu().float(), refp)
-    # global average pool + eval BatchNorm1d
-    act = (torch.randn(4, 16, 8, 2048, generator=g)).half().cuda()
-    sc, sh = (torch.rand(2048, generator=g) + 0.5).cuda(), torch.randn(2048, generator=g).cuda()
-    feat, emb = torch.empty(4, 2048, device="cuda"), torch.empty(4, 2048, device="cuda")
-    N.check(L.ctl_gap_bn_nhwc_f16(act.data_ptr(), 4, 128, 2048, sc.data_ptr(), sh.data_ptr(), feat.data_ptr(),
-                                  emb.data_ptr(), N.stream_ptr()))
-    rf = act.cpu().double().mean(dim=(1, 2))
-    np.testing.assert_allclose(feat.cpu().numpy(), rf.numpy(), rtol=1e-5, atol=1e-6)
-    np.testing.assert_allclose(emb.cpu().numpy(), (rf * sc.cpu().double() + sh.cpu().double()).numpy(), rtol=1e-5,
-                               atol=1e-5)
-    # InstanceNorm + ReLU on the first half of the channels, second half untouched
-    t = (torch.randn(2, 20, 12, 128, generator=g) * 2 + 0.3).half()
-    gam, bet = torch.rand(64, generator=g) + 0.5, torch.randn(64, generator=g) * 0.2
-    td, gd, btd = t.clone().cuda(), gam.cuda(), bet.cuda()
-    N.check(L.ctl_instnorm_relu_nhwc_f16(td.data_ptr(), 2, 240, 128, 64, gd.data_ptr(), btd.data_ptr(),
-                                         1e-5, N.stream_ptr()))
-    torch.cuda.synchronize()
-    ref_in = F.relu(F.instance_norm(t[..., :64].double().permute(0, 3, 1, 2), None, None, gam.double(), bet.double(),
-                                    True, 0.1, 1e-5)).permute(0, 2, 3, 1)
-    got = td.cpu()
-    assert torch.equal(got[..., 64:], t[..., 64:])
-    assert float((got[..., :64].double() - ref_in).abs().max()) <= float(ref_in.abs().max()) * 2.0 ** -10 + 2e-3
-
-
 @pytest.mark.parametrize("tag,ibn,hw", [("r50", False, (256, 128)), ("ibn", True, (128, 64))])
 def test_full_trunk_matches_checker_and_reference_golden(tag, ibn, hw):
     from ctl_b200.modelling.backbones.engine import TrunkEngine

@@ -1,4 +1,7 @@
-"""Per-launch profile of the ResNet50 eval trunk at the bench shape (bs 256, 256x128, last_stride 1, BN head).
+"""Per-launch profile of the eval trunk (last_stride 1, BN head), by default ResNet50 at the bench shape (bs 256, 256x128).
+
+--ibn profiles ResNet50-IBN-a and --size sets the crop, e.g. --ibn --size 320x320 --batch 128 (config 4's per-GPU eval
+shape).
 
 Runs eager forwards under torch.profiler (CUDA activities only) and lists every kernel of one forward in walk order:
 layer/block/role, M, K, Cout, n-tiles, the time the launch adds to the forward, its FLOPs, its algorithmic bytes (each
@@ -7,9 +10,10 @@ larger of the two bounds at the H100 SXM data-sheet peaks (989 TFLOP/s dense FP1
 
 "time" is the step from the previous kernel's end to this kernel's end, the median over the profiled forwards: with
 programmatic dependent launch a kernel's prologue overlaps its predecessor's tail, so raw durations overlap and do not
-add up to the forward; these steps do.  "dur" is the kernel's own duration.
+add up to the forward; these steps do.  "dur" is the kernel's own duration.  The launches that are not convolutions
+(stem, pools, IBN-a's InstanceNorm, head) are listed by kernel name and summed per kernel at the end.
 
-    python tools/prof_trunk.py [--batch 256] [--iters 20] [--json FILE]
+    python tools/prof_trunk.py [--batch 256] [--ibn] [--size 256x128] [--iters 20] [--json FILE]
 """
 import argparse
 import json
@@ -45,7 +49,8 @@ def _bn(cout, chained):
 
 
 def conv_walk(n, H, W, last_stride=1):
-    """The convolution launches of csrc/trunk.cu run_blocks for the bottleneck ResNet50 (no IBN), in launch order."""
+    """The convolution launches of csrc/trunk.cu run_blocks for the bottleneck ResNet50, in launch order (IBN-a runs
+    the same convolutions; its InstanceNorm launches are not convolutions)."""
     h, w = H // 4, W // 4  # stem 7x7/2 + maxpool 3x3/2 on even sides
     cin = 64
     out = []
@@ -97,6 +102,8 @@ def kernel_kind(name):
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--batch", type=int, default=256)
+    ap.add_argument("--ibn", action="store_true", help="ResNet50-IBN-a instead of ResNet50")
+    ap.add_argument("--size", default="256x128", help="HxW of the input crops")
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--json", default=None, help="also write the rows to this file")
     args = ap.parse_args()
@@ -106,9 +113,11 @@ def main():
     from ctl_b200.modelling.backbones.engine import TrunkEngine
     from torch.profiler import ProfilerActivity, profile
 
-    H, W = 256, 128
+    H, W = (int(v) for v in args.size.split("x"))
+    model = "ResNet50-IBN-a" if args.ibn else "ResNet50"
     dev = torch.device("cuda", 0)
-    eng = TrunkEngine(synth.make_trunk_state(seed=0), dev, ibn=False, last_stride=1, bn_head=synth.make_head_bn(0))
+    eng = TrunkEngine(synth.make_trunk_state(seed=0, ibn=args.ibn), dev, ibn=args.ibn, last_stride=1,
+                      bn_head=synth.make_head_bn(0))
     x = torch.randn(args.batch, 3, H, W, generator=torch.Generator().manual_seed(1234)).to(dev)
     for _ in range(5):
         eng.forward(x, want_emb=True)
@@ -143,7 +152,7 @@ def main():
         rows.append(row)
 
     name, power = card()
-    print(f"# {name}, power limit {power}; ResNet50 eval forward, bs {args.batch}, {H}x{W}, last_stride 1; "
+    print(f"# {name}, power limit {power}; {model} eval forward, bs {args.batch}, {H}x{W}, last_stride 1; "
           f"median of {args.iters} eager forwards under torch.profiler")
     print(f"{'#':>3} {'launch':44} {'M':>6} {'K':>5} {'Cout':>5} {'nt':>3} {'time_us':>8} {'dur_us':>8} {'GFLOP':>7} "
           f"{'MB':>7} {'bound_us':>8} {'bnd':>4} {'TFLOP/s':>8} {'GB/s':>6} {'of_bnd':>6}")
@@ -161,9 +170,19 @@ def main():
               f"{r['dur_us']:8.1f} {r['flops'] / 1e9:7.1f} {r['bytes'] / 1e6:7.1f} {r['bound_us']:8.1f} {r['bound']:>4} "
               f"{r['flops'] / t / 1e6:8.1f} {r['bytes'] / t / 1e3:6.0f} {r['bound_us'] / t:6.2f}")
     print(f"# forward {tot_t / 1e3:.3f} ms (sum of steps); convolution bounds sum {tot_b / 1e3:.3f} ms")
+    others = {}
+    for r in rows:
+        if r["kernel"] == "other":
+            k = others.setdefault(r["launch"], [0, 0.0, 0.0])
+            k[0] += 1
+            k[1] += r["time_us"]
+            k[2] += r["dur_us"]
+    for k, (cnt, t, d) in others.items():
+        print(f"# {k}: {cnt} launches, time {t:.1f} us, dur {d:.1f} us")
     if args.json:
         with open(args.json, "w") as f:
-            json.dump({"gpu": name, "power_limit": power, "batch": args.batch, "rows": rows}, f, indent=1)
+            json.dump({"gpu": name, "power_limit": power, "model": model, "batch": args.batch, "size": [H, W],
+                       "rows": rows}, f, indent=1)
 
 
 if __name__ == "__main__":
