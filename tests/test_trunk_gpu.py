@@ -141,38 +141,6 @@ def test_full_trunk_matches_checker_and_reference_golden(tag, ibn, hw):
     np.testing.assert_allclose(out["emb"].cpu().numpy(), emb_ref.numpy(), rtol=1e-5, atol=1e-5)
 
 
-@pytest.mark.gpu
-@pytest.mark.parametrize("shape", [(3, 64, 48), (2, 256, 128), (40, 64, 32), (5, 128, 64), (1, 8, 8)])
-def test_stem_pool_fused(shape):
-    """conv1 + folded bn1 (+ReLU) + maxpool in one kernel (wgmma windows over raw input rows) against the fp16-operand
-    convolution followed by max_pool2d; ranges that start inside an image and cross images are both exercised."""
-    from ctl_b200 import _native as N
-    from ctl_b200.modelling.backbones.engine import pack_stem_fused
-
-    L = N.lib()
-    n, H, W = shape
-    g = torch.Generator().manual_seed(11)
-    x = torch.randn(n, 3, H, W, generator=g)
-    w = torch.randn(64, 3, 7, 7, generator=g) * 0.1
-    b = torch.randn(64, generator=g) * 0.1
-    xd, bd, wd = x.cuda(), b.cuda(), pack_stem_fused(w.cuda())
-    pad = torch.zeros(L.ctl_stem_pad_bytes(n, H, W), dtype=torch.uint8, device="cuda")
-    for relu in (0, 1):
-        ref = F.conv2d(x.half().double(), w.half().double(), b.double(), 2, 3)
-        if relu:
-            ref = ref.clamp(min=0)
-        refp = F.max_pool2d(ref, 3, 2, 1)
-        hp, wp = refp.shape[2:]
-        out = torch.full((n, hp, wp, 64), float("nan"), dtype=torch.float16, device="cuda")
-        for _ in range(2):  # the second call reuses the staging buffer (borders must still be zero)
-            N.check(L.ctl_stem_pool_fused(xd.data_ptr(), n, H, W, pad.data_ptr(), wd.data_ptr(), bd.data_ptr(), relu,
-                                          out.data_ptr(), N.stream_ptr()))
-        torch.cuda.synchronize()
-        got = out.cpu().double().permute(0, 3, 1, 2)
-        assert torch.isfinite(got).all()
-        assert float((got - refp).abs().max()) <= float(refp.abs().max()) * 2.0 ** -10 + 1e-4
-
-
 @pytest.mark.parametrize("tag,ibn,hw,big", [("r50", False, (256, 128), 256), ("ibn", True, (320, 320), 128)])
 def test_batch_invariance_at_bench_shapes(tag, ibn, hw, big):
     """The bench configurations themselves (256 x 256x128 ResNet50 = metric M1; 128 x 320x320 IBN-a = config 4's per-GPU
