@@ -71,15 +71,39 @@ struct ConvKernelParams {
   ConvTap tap9;
 };
 
+// Operands wait in two rings with their own depths and producers.  The A ring's 16 KiB slots carry the activation
+// k-blocks and the residual slabs (one [128 px][64 ch] slab per slot); the B ring's slots carry the weight k-blocks
+// and a chained launch's W2 slabs (N2 x 64 fp16, no larger than a BN = 128 slot).  So a residual slab holds one
+// 16 KiB slot instead of a whole activation + weight stage, and activations, which come from HBM whenever the
+// previous launch's output outgrew L2, are fetched further ahead than the L2-resident weights.
 template <int BN>
 struct ConvCfg {
   static constexpr int B_TILE_BYTES = BN * CBK * 2;
-  static constexpr int STAGE_BYTES = A_TILE_BYTES + B_TILE_BYTES;
-  static constexpr int STAGES = BN == 64 ? 5 : (BN == 128 ? 4 : 3);
-  static constexpr int OUT_SLABS = 4;                  // [128 px][64 ch] fp16 staging slabs for the TMA stores
+  // Depths from a sweep of the eval trunk at the bench shape on H100: at BN = 256, two weight slots leave the MMAs
+  // waiting on L2 and cost more than any activation depth gains, so B gets three slots, A five, and the staging
+  // slabs give up two of their four to make room; BN = 128 / 64 fill the same budget.
+  static constexpr int A_SLOTS = BN == 256 ? 5 : 6;
+  static constexpr int B_SLOTS = BN == 256 ? 3 : (BN == 128 ? 5 : 8);
+  static constexpr int OUT_SLABS = 2;                  // [128 px][64 ch] fp16 staging slabs for the TMA stores
   static constexpr int BIAS_BYTES = 2048 * 4;          // the layer's whole bias vector (Cout <= 2048), loaded once
-  static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + OUT_SLABS * A_TILE_BYTES + BIAS_BYTES + 1024 + 256;
+  static constexpr size_t SMEM =
+      (size_t)(A_SLOTS + OUT_SLABS) * A_TILE_BYTES + (size_t)B_SLOTS * B_TILE_BYTES + BIAS_BYTES + 1024 + 256;
   static_assert(SMEM <= 227 * 1024, "conv_gemm_kernel shared memory");
+  static_assert(A_SLOTS >= 2 && B_SLOTS >= 2 && 2 * (A_SLOTS + B_SLOTS) * 8 <= 256, "ring depths / barrier space");
+};
+
+// a position in a ring of S slots: the slot, and the parity of the current pass over the ring (the mbarrier phase)
+template <int S>
+struct RingPos {
+  int slot = 0;
+  uint32_t phase = 0;
+  __device__ __forceinline__ void next() {
+    if (++slot == S) {
+      slot = 0;
+      phase ^= 1u;
+    }
+  }
+  __device__ __forceinline__ int prev() const { return slot == 0 ? S - 1 : slot - 1; }
 };
 
 // Tile order: n fastest, then pixel tiles row-major inside an image, then images.  An unchained launch of more than
@@ -160,7 +184,7 @@ __device__ __forceinline__ void store_subtile_f16(const float* d, uint8_t* slab,
 // k-block (nt * BN / 64 + j) of the next 1x1 convolution (K2 = Cout, N2 outputs), so once a slab is complete each
 // consumer warpgroup issues that k-block (m64 nN2 k16 x 4, the shape and k order of the stand-alone launch: same bits)
 // into a second accumulator that lives across the m-tile's n-tiles; its weight slab W2[:, 64 kb .. 64 kb + 63] rides
-// the operand ring after the sub-tile's residual slab.  After the last n-tile the second accumulator goes through the
+// the B ring after the tile's weight k-blocks.  After the last n-tile the second accumulator goes through the
 // same epilogue into out2, so the block output is never re-read from HBM.  Each CTA owns whole m-tiles.
 template <int BN, int N2 = 0>
 __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid_constant__ ConvKernelParams p) {
@@ -169,17 +193,22 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid
   static_assert(N2 == 0 || N2 == 64 || N2 == 128, "chained 1x1 width");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t out_stage = smem_base + Cfg::STAGES * Cfg::STAGE_BYTES;
+  const uint32_t ring_b = smem_base + Cfg::A_SLOTS * A_TILE_BYTES;
+  const uint32_t out_stage = ring_b + Cfg::B_SLOTS * Cfg::B_TILE_BYTES;
   const uint32_t bias_sm = out_stage + Cfg::OUT_SLABS * A_TILE_BYTES;
   const uint32_t bar_base = bias_sm + Cfg::BIAS_BYTES;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (Cfg::STAGES + s); };
+  auto a_slot = [&](int s) { return smem_base + s * A_TILE_BYTES; };
+  auto b_slot = [&](int s) { return ring_b + s * Cfg::B_TILE_BYTES; };
+  auto a_full = [&](int s) { return bar_base + 8u * s; };
+  auto a_empty = [&](int s) { return bar_base + 8u * (Cfg::A_SLOTS + s); };
+  auto b_full = [&](int s) { return bar_base + 8u * (2 * Cfg::A_SLOTS + s); };
+  auto b_empty = [&](int s) { return bar_base + 8u * (2 * Cfg::A_SLOTS + Cfg::B_SLOTS + s); };
   uint8_t* gsm = smem_raw + (smem_base - smem_u32(smem_raw));  // generic view of the aligned arena
 
   const int warp = threadIdx.x >> 5;
   const int num_tiles = p.m_tiles * p.n_tiles;
   const int conv_kblocks = p.k_blocks;
-  // this CTA's tiles: t_begin, t_begin + t_step, ... < t_end (see "Tile order"); the producer and both consumer
+  // this CTA's tiles: t_begin, t_begin + t_step, ... < t_end (see "Tile order"); both producers and both consumer
   // warpgroups walk the same sequence
   int t_begin = (int)blockIdx.x, t_end = num_tiles, t_step = (int)gridDim.x;
   if (N2 > 0 || p.n_tiles == 1) {  // a contiguous, balanced range of whole m-tiles
@@ -190,9 +219,13 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid
   }
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < Cfg::STAGES; ++s) {
-      mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 2);  // one arrive per consumer warpgroup
+    for (int s = 0; s < Cfg::A_SLOTS; ++s) {
+      mbar_init(a_full(s), 1);
+      mbar_init(a_empty(s), 2);  // one arrive per consumer warpgroup
+    }
+    for (int s = 0; s < Cfg::B_SLOTS; ++s) {
+      mbar_init(b_full(s), 1);
+      mbar_init(b_empty(s), 2);
     }
     fence_barrier_init();
     for (int i = 0; i < 4; ++i) tma_prefetch_desc(&p.a_map[i]);
@@ -214,11 +247,12 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid
   pdl_wait();               // activations of the previous kernel are complete and visible
 
   if (warp < 4) {
-    // ===================== TMA producer =====================
+    // ===================== TMA producers: one thread per ring =====================
     setmaxnreg_dec<PRODUCER_REGS>();
     if (threadIdx.x == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
+      // A ring: the tile's activation k-blocks, then its residual slabs, one per 64 output channels, each read by
+      // the epilogue of that sub-tile straight from its slot
+      RingPos<Cfg::A_SLOTS> ra;
       TileIter it;
       it.init(t_begin, p);
       for (int tile = t_begin; tile < t_end; tile += t_step, it.advance(tile, t_step, p)) {
@@ -226,50 +260,52 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid
         for (int t = 0; t < p.n_taps; ++t) {
           const ConvTap tap = t < 9 ? p.taps[t] : p.tap9;
           for (int cb = 0; cb < tap.cblocks; ++cb) {
-            mbar_wait(empty_bar(stage), phase ^ 1u);
-            const uint32_t dst = smem_base + stage * Cfg::STAGE_BYTES;
-            mbar_arrive_expect_tx(full_bar(stage), Cfg::STAGE_BYTES);
-            tma_load_4d(dst, &p.a_map[tap.map], full_bar(stage), cb * CBK, w0 + tap.dw, h0 + tap.dh, it.img);
-            tma_load_2d(dst + A_TILE_BYTES, &p.b_map, full_bar(stage), tap.koff + cb * CBK, it.nt * BN);
-            if (++stage == Cfg::STAGES) {
-              stage = 0;
-              phase ^= 1u;
-            }
+            mbar_wait(a_empty(ra.slot), ra.phase ^ 1u);
+            mbar_arrive_expect_tx(a_full(ra.slot), A_TILE_BYTES);
+            tma_load_4d(a_slot(ra.slot), &p.a_map[tap.map], a_full(ra.slot), cb * CBK, w0 + tap.dw, h0 + tap.dh,
+                        it.img);
+            ra.next();
           }
         }
-        if (p.has_residual || N2 > 0) {
-          // the residual rides the same ring: one [128 px][64 ch] slab per 64 output channels, read by
-          // the epilogue of that sub-tile straight from its ring slot; a chained launch follows each with
-          // the W2 slab of that sub-tile's GEMM2 k-block
+        if (p.has_residual) {
           for (int j = 0; j < NSUB; ++j) {
-            if (p.has_residual) {
-              mbar_wait(empty_bar(stage), phase ^ 1u);
-              mbar_arrive_expect_tx(full_bar(stage), A_TILE_BYTES);
-              tma_load_4d(smem_base + stage * Cfg::STAGE_BYTES, &p.res_map, full_bar(stage), it.nt * BN + j * 64, w0, h0,
-                          it.img);
-              if (++stage == Cfg::STAGES) {
-                stage = 0;
-                phase ^= 1u;
-              }
-            }
-            if constexpr (N2 > 0) {
-              mbar_wait(empty_bar(stage), phase ^ 1u);
-              mbar_arrive_expect_tx(full_bar(stage), N2 * CBK * 2);
-              tma_load_2d(smem_base + stage * Cfg::STAGE_BYTES, &p.b2_map, full_bar(stage), it.nt * BN + j * 64, 0);
-              if (++stage == Cfg::STAGES) {
-                stage = 0;
-                phase ^= 1u;
-              }
-            }
+            mbar_wait(a_empty(ra.slot), ra.phase ^ 1u);
+            mbar_arrive_expect_tx(a_full(ra.slot), A_TILE_BYTES);
+            tma_load_4d(a_slot(ra.slot), &p.res_map, a_full(ra.slot), it.nt * BN + j * 64, w0, h0, it.img);
+            ra.next();
+          }
+        }
+      }
+    } else if (threadIdx.x == 32) {
+      // B ring: the tile's weight k-blocks, then (chained launch) the W2 slab of each sub-tile's GEMM2 k-block
+      RingPos<Cfg::B_SLOTS> rb;
+      TileIter it;
+      it.init(t_begin, p);
+      for (int tile = t_begin; tile < t_end; tile += t_step, it.advance(tile, t_step, p)) {
+        for (int t = 0; t < p.n_taps; ++t) {
+          const ConvTap tap = t < 9 ? p.taps[t] : p.tap9;
+          for (int cb = 0; cb < tap.cblocks; ++cb) {
+            mbar_wait(b_empty(rb.slot), rb.phase ^ 1u);
+            mbar_arrive_expect_tx(b_full(rb.slot), Cfg::B_TILE_BYTES);
+            tma_load_2d(b_slot(rb.slot), &p.b_map, b_full(rb.slot), tap.koff + cb * CBK, it.nt * BN);
+            rb.next();
+          }
+        }
+        if constexpr (N2 > 0) {
+          for (int j = 0; j < NSUB; ++j) {
+            mbar_wait(b_empty(rb.slot), rb.phase ^ 1u);
+            mbar_arrive_expect_tx(b_full(rb.slot), N2 * CBK * 2);
+            tma_load_2d(b_slot(rb.slot), &p.b2_map, b_full(rb.slot), it.nt * BN + j * 64, 0);
+            rb.next();
           }
         }
       }
     }
   } else {
     // ===== consumers: warpgroup wg issues the wgmmas of tile rows [64 wg, 64 wg + 64) (M = 64, N = BN) into its
-    // registers, then drains them in 64-channel sub-tiles: (+residual from the ring, +bias, ReLU) -> fp16 -> swizzled
-    // staging slab shared by both warpgroups -> one TMA store per sub-tile; four slabs keep up to three stores in
-    // flight.
+    // registers, then drains them in 64-channel sub-tiles: (+residual from the A ring, +bias, ReLU) -> fp16 ->
+    // swizzled staging slab shared by both warpgroups -> one TMA store per sub-tile; OUT_SLABS slabs keep up to
+    // OUT_SLABS - 1 stores in flight.
     setmaxnreg_inc<CONSUMER_REGS>();
     const int wg = (threadIdx.x >> 7) - 1;
     const bool wg_leader = (threadIdx.x & 127) == 0;
@@ -279,42 +315,43 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid
     const float* bias_s = reinterpret_cast<const float*>(gsm + (bias_sm - smem_base));
     float acc[BN / 2];
     [[maybe_unused]] float acc2[N2 > 0 ? N2 / 2 : 1];  // GEMM2 (chained launch only)
-    int stage = 0;
-    uint32_t phase = 0;
+    RingPos<Cfg::A_SLOTS> ra;
+    RingPos<Cfg::B_SLOTS> rb;
     uint32_t g = 0;  // running sub-tile counter -> staging slab
     TileIter it;
     it.init(t_begin, p);
     for (int tile = t_begin; tile < t_end; tile += t_step, it.advance(tile, t_step, p)) {
       const int h0 = it.th * p.TH, w0 = it.tw * p.TW;
-      int held = -1;  // ring slot still read by the wgmma group in flight
       for (int kb = 0; kb < conv_kblocks; ++kb) {
-        mbar_wait(full_bar(stage), phase);
-        const uint32_t base = smem_base + stage * Cfg::STAGE_BYTES;
-        const uint64_t da = make_sw128_kmajor_desc(base + wg * A_HALF_BYTES);
-        const uint64_t db = make_sw128_kmajor_desc(base + A_TILE_BYTES);
+        mbar_wait(a_full(ra.slot), ra.phase);
+        mbar_wait(b_full(rb.slot), rb.phase);
+        const uint64_t da = make_sw128_kmajor_desc(a_slot(ra.slot) + wg * A_HALF_BYTES);
+        const uint64_t db = make_sw128_kmajor_desc(b_slot(rb.slot));
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < CBK / 16; ++k)
           wgmma_f16<BN>(acc, desc_advance_k(da, k), desc_advance_k(db, k), (kb > 0 || k > 0) ? 1u : 0u);
         wgmma_commit();
-        wgmma_wait<1>();  // the previous k-block's group is done reading its slot
-        if (held >= 0 && wg_leader) mbar_arrive(empty_bar(held));
-        held = stage;
-        if (++stage == Cfg::STAGES) {
-          stage = 0;
-          phase ^= 1u;
+        wgmma_wait<1>();  // the previous k-block's group is done reading its slots
+        if (kb > 0 && wg_leader) {
+          mbar_arrive(a_empty(ra.prev()));
+          mbar_arrive(b_empty(rb.prev()));
         }
+        ra.next();
+        rb.next();
       }
       wgmma_wait<0>();
-      if (held >= 0 && wg_leader) mbar_arrive(empty_bar(held));
-      [[maybe_unused]] int held2 = -1;  // ring slot of the W2 slab read by the GEMM2 group in flight
+      if (wg_leader) {  // the last k-block's slots
+        mbar_arrive(a_empty(ra.prev()));
+        mbar_arrive(b_empty(rb.prev()));
+      }
 #pragma unroll
       for (int j = 0; j < NSUB; ++j, ++g) {
         const uint32_t b = g & (Cfg::OUT_SLABS - 1);
         const uint8_t* res = nullptr;
-        if (p.has_residual) {  // this sub-tile's residual slab, next in the ring
-          mbar_wait(full_bar(stage), phase);
-          res = gsm + stage * Cfg::STAGE_BYTES;
+        if (p.has_residual) {  // this sub-tile's residual slab, next in the A ring
+          mbar_wait(a_full(ra.slot), ra.phase);
+          res = gsm + ra.slot * A_TILE_BYTES;
         }
         // slab b was handed to a TMA store OUT_SLABS sub-tiles ago: wait until that store has read it
         if (leader) tma_store_wait_read<Cfg::OUT_SLABS - 1>();
@@ -324,11 +361,8 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid
         fence_proxy_async();     // staging writes (generic proxy) -> visible to the TMA store (async proxy)
         named_bar_sync(1, 256);  // slab complete; both warpgroups are done with the residual slot
         if (p.has_residual) {
-          if (wg_leader) mbar_arrive(empty_bar(stage));
-          if (++stage == Cfg::STAGES) {
-            stage = 0;
-            phase ^= 1u;
-          }
+          if (wg_leader) mbar_arrive(a_empty(ra.slot));
+          ra.next();
         }
         if (leader) {
           tma_store_4d(&p.out_map, out_stage + b * A_TILE_BYTES, it.nt * BN + j * 64, w0, h0, it.img);
@@ -337,9 +371,9 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid
         if constexpr (N2 > 0) {
           // GEMM2 k-block nt * NSUB + j from this warpgroup's 64 rows of slab b.  Each warpgroup reads only the rows it
           // wrote, and the group reading slab b has completed (wgmma_wait<1> one sub-tile later) before it is rewritten.
-          mbar_wait(full_bar(stage), phase);
+          mbar_wait(b_full(rb.slot), rb.phase);
           const uint64_t da = make_sw128_kmajor_desc(out_stage + b * A_TILE_BYTES + wg * A_HALF_BYTES);
-          const uint64_t db = make_sw128_kmajor_desc(smem_base + stage * Cfg::STAGE_BYTES);
+          const uint64_t db = make_sw128_kmajor_desc(b_slot(rb.slot));
           const bool first = it.nt == 0 && j == 0;
           wgmma_fence();
 #pragma unroll
@@ -347,17 +381,13 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_gemm_kernel(const __grid
             wgmma_f16<N2>(acc2, desc_advance_k(da, k), desc_advance_k(db, k), (!first || k > 0) ? 1u : 0u);
           wgmma_commit();
           wgmma_wait<1>();
-          if (held2 >= 0 && wg_leader) mbar_arrive(empty_bar(held2));  // the previous W2 slab
-          held2 = stage;
-          if (++stage == Cfg::STAGES) {
-            stage = 0;
-            phase ^= 1u;
-          }
+          if (j > 0 && wg_leader) mbar_arrive(b_empty(rb.prev()));  // the previous W2 slab, one slot back in the B ring
+          rb.next();
         }
       }
       if constexpr (N2 > 0) {
         wgmma_wait<0>();
-        if (wg_leader) mbar_arrive(empty_bar(held2));
+        if (wg_leader) mbar_arrive(b_empty(rb.prev()));  // the last W2 slab
         if (it.nt == p.n_tiles - 1) {  // the m-tile's GEMM2 is complete: its epilogue, into out2
 #pragma unroll
           for (int j = 0; j < N2 / 64; ++j, ++g) {
