@@ -75,6 +75,26 @@ class NamedTensor(C.Structure):
     _fields_ = [("name", C.c_char_p), ("data", _p), ("numel", _i64)]
 
 
+class JpegDesc(C.Structure):
+    """struct ctl_jpeg_desc (include/ctl_b200.h)."""
+
+    _fields_ = [("h", _i32), ("w", _i32), ("scan_begin", C.c_uint32), ("scan_end", C.c_uint32),
+                ("dqt", C.c_uint32 * 3), ("dht_dc", C.c_uint32 * 3), ("dht_ac", C.c_uint32 * 3),
+                ("restart_interval", C.c_uint16), ("ncomp", C.c_uint8), ("dqt16", C.c_uint8),
+                ("hs", C.c_uint8 * 3), ("vs", C.c_uint8 * 3), ("reserved", C.c_uint8 * 2)]
+
+
+class JpegEntry(C.Structure):
+    """struct ctl_jpeg_entry (include/ctl_b200.h)."""
+
+    _fields_ = [("offset", _i64), ("nbytes", _i64), ("kind", _i32), ("reserved", _i32), ("desc", JpegDesc)]
+
+
+CTL_JPEG_ENTRY_JPEG = 0
+CTL_JPEG_ENTRY_RAW = 1
+CTL_JPEG_ENTRY_MOCK = 2
+
+
 # name -> (restype, argtypes); kept in one table so tests can check it against the header
 SIGNATURES = {
     "ctl_last_error": (C.c_char_p, []),
@@ -174,6 +194,9 @@ SIGNATURES = {
     "ctl_augment_batch_u8": (C.c_int, [_p, _i32, _i32, _i32, _i32, _p, _p, _p, _p, _p]),
     "ctl_resize_bilinear_u8_workspace_bytes": (_sz, [_i64, _i32, _i32]),
     "ctl_resize_bilinear_u8": (C.c_int, [_p, _i64, _p, _i64, _i32, _i32, _p, _p, _p, _sz, _p]),
+    "ctl_jpeg_parse": (C.c_int, [_p, _i64, C.POINTER(JpegDesc), C.POINTER(_i32), C.POINTER(_i32)]),
+    "ctl_jpeg_decode_workspace_bytes": (_sz, [_p, _i64]),
+    "ctl_jpeg_decode": (C.c_int, [_p, _i64, _p, _i64, _p, _p, _i64, _p, _p, _sz, _p]),
     "ctl_adam_multi_step": (C.c_int, [_p, _i32, C.c_int64, _f, _f, _f, _f, _f, C.c_int64, _f, _p, _p]),
     "ctl_sgd_step": (C.c_int, [_p, _p, C.c_int64, _f, _f, _p, _p]),
     "ctl_loss_scale_update": (C.c_int, [_p, _p, _p, _p, _f, _f, _f, _i32, _p]),

@@ -1,6 +1,7 @@
 """Device-side transforms: the arithmetic of ReidTransforms.build_transforms (datasets/transforms/build.py:15-33) for a
-whole batch -- `T.Resize` of native-size images packed in a RaggedImages (pack_images -> resize_batch, bit for bit
-PIL's BILINEAR resize), then the training chain after it in one kernel (augment_batch) or the eval chain
+whole batch -- the loaders' JPEG decode (pack_jpegs -> decode_batch, bit for bit Pillow's
+`Image.open(p).convert("RGB")`), `T.Resize` of native-size images packed in a RaggedImages (pack_images -> resize_batch,
+bit for bit PIL's BILINEAR resize), then the training chain after it in one kernel (augment_batch) or the eval chain
 (normalize_batch, or TrunkEngine.forward_u8, which folds it into the stem).  This module alone knows the ragged layout.
 
 The reference draws its random numbers per image inside torchvision / `random` (flip: torch.rand(1) < p;
@@ -136,6 +137,153 @@ def pack_images(images, pin: bool = True) -> RaggedImages:
             flat[o: o + a.nbytes] = a.reshape(-1)
     t = torch.from_numpy(table)
     return RaggedImages(data, t.pin_memory() if pin else t, int(table[:, 1].sum()))
+
+
+class JpegBatch:
+    """A batch of image files packed back to back (any byte alignment) in one uint8 buffer `data`, for decode_batch.
+    `entries` uint8 [n, 88] holds one struct ctl_jpeg_entry per image: a JPEG with the descriptor ctl_jpeg_parse read
+    from its header, raw HWC RGB bytes (a file the device decode does not cover, decoded by Pillow in pack_jpegs), or a
+    mock row.  `out_table` int64 [n, 3] = {byte offset, h, w} is the table of the RaggedImages decode_batch returns,
+    `out_bytes` its buffer size, `rows` the sum of its heights; `workspace_bytes` is ctl_jpeg_decode_workspace_bytes of
+    the entries; `fallback` lists the indices decoded on the host, with the parser's reason for each."""
+
+    def __init__(self, data, entries, out_table, out_bytes, rows, workspace_bytes, fallback=()):
+        self.data, self.entries, self.out_table = data, entries, out_table
+        self.out_bytes, self.rows, self.workspace_bytes = int(out_bytes), int(rows), int(workspace_bytes)
+        self.fallback = list(fallback)
+
+    def __len__(self):
+        return self.entries.shape[0]
+
+    @property
+    def device(self):
+        return self.data.device
+
+    def to(self, device, non_blocking: bool = True) -> "JpegBatch":
+        """The same batch on `device`; from pinned host buffers the copies do not block the host."""
+        return JpegBatch(self.data.to(device, non_blocking=non_blocking),
+                         self.entries.to(device, non_blocking=non_blocking),
+                         self.out_table.to(device, non_blocking=non_blocking), self.out_bytes, self.rows,
+                         self.workspace_bytes, self.fallback)
+
+
+def parse_jpeg(data):
+    """ctl_jpeg_parse of one file's bytes -> (struct ctl_jpeg_desc, None), or (None, the reason the device decode
+    does not cover it)."""
+    buf = bytes(data)
+    desc = N.JpegDesc()
+    rc = N.lib().ctl_jpeg_parse(buf, len(buf), C.byref(desc), None, None)
+    if rc != 0:
+        return None, N.lib().ctl_last_error().decode("utf-8", "replace")
+    return desc, None
+
+
+def _read_item(i, item):
+    if isinstance(item, (bytes, bytearray, memoryview)):
+        return bytes(item)
+    if isinstance(item, (str, bytes)) or hasattr(item, "__fspath__"):
+        with open(item, "rb") as f:
+            return f.read()
+    raise ValueError(f"item {i}: expected file bytes, a path or None, got {type(item).__name__}")
+
+
+def pack_jpegs(items, pin: bool = True) -> JpegBatch:
+    """Image files -- bytes, or paths read here, with `None` for a mock row -> one host JpegBatch (pinned when `pin`).
+    A file ctl_jpeg_parse rejects (progressive, CMYK, PNG, ...) is decoded here with `Image.open(...).convert("RGB")`,
+    as the reference's loaders do (datasets/bases.py:32-33), and stored as raw RGB bytes, so a mixed dataset still
+    gives one batch whose decode equals the reference's.  Meant for loader workers: the collate of file bytes."""
+    import io
+
+    from PIL import Image
+
+    blobs, descs, fallback = [], [], []
+    for i, item in enumerate(items):
+        if item is None:
+            blobs.append(None)
+            descs.append(None)
+            continue
+        raw = _read_item(i, item)
+        desc, why = parse_jpeg(raw)
+        if desc is None:
+            try:
+                with Image.open(io.BytesIO(raw)) as im:
+                    rgb = np.ascontiguousarray(np.asarray(im.convert("RGB")))
+            except Exception as exc:  # noqa: BLE001 -- any Pillow failure means the item is not an image
+                raise ValueError(f"item {i}: neither a JPEG this decode covers ({why}) nor an image Pillow "
+                                 f"reads ({exc})") from exc
+            fallback.append((i, why))
+            blobs.append(rgb)
+        else:
+            blobs.append(raw)
+        descs.append(desc)
+    n = len(blobs)
+    if n == 0:
+        raise ValueError("pack_jpegs: no items")
+    entries = (N.JpegEntry * n)()
+    out_table = np.zeros((n, 3), dtype=np.int64)
+    off = out_off = 0
+    for i, (blob, desc) in enumerate(zip(blobs, descs)):
+        e = entries[i]
+        if blob is None:
+            e.kind = N.CTL_JPEG_ENTRY_MOCK
+            continue
+        if isinstance(blob, np.ndarray):
+            e.kind = N.CTL_JPEG_ENTRY_RAW
+            e.desc.h, e.desc.w = blob.shape[0], blob.shape[1]
+            nbytes = blob.nbytes
+        else:
+            e.kind = N.CTL_JPEG_ENTRY_JPEG
+            e.desc = desc
+            nbytes = len(blob)
+        e.offset, e.nbytes = off, nbytes
+        out_table[i] = out_off, e.desc.h, e.desc.w
+        off += nbytes
+        out_off += e.desc.h * e.desc.w * 3
+    data = torch.empty(max(off, 1), dtype=torch.uint8, pin_memory=pin)
+    flat = data.numpy()
+    for i, blob in enumerate(blobs):
+        if blob is not None:
+            o = entries[i].offset
+            flat[o: o + entries[i].nbytes] = np.frombuffer(blob, dtype=np.uint8) if isinstance(blob, bytes) \
+                else blob.reshape(-1)
+    ws = N.lib().ctl_jpeg_decode_workspace_bytes(C.addressof(entries), n)
+    ent = torch.from_numpy(np.frombuffer(entries, dtype=np.uint8).reshape(n, C.sizeof(N.JpegEntry)).copy())
+    tab = torch.from_numpy(out_table)
+    if pin:
+        ent, tab = ent.pin_memory(), tab.pin_memory()
+    return JpegBatch(data, ent, tab, out_off, int(out_table[:, 1].sum()), ws, fallback)
+
+
+def _decode_enqueue(batch: JpegBatch, out: torch.Tensor, status: torch.Tensor, workspace: torch.Tensor):
+    """ctl_jpeg_decode (enqueue only, capturable in a CUDA graph); the caller reads `status` back."""
+    N.check(N.lib().ctl_jpeg_decode(batch.data.data_ptr(), batch.data.numel(), batch.entries.data_ptr(), len(batch),
+                                    batch.out_table.data_ptr(), out.data_ptr(), batch.out_bytes, status.data_ptr(),
+                                    workspace.data_ptr(), workspace.numel(), N.stream_ptr()))
+
+
+def decode_batch(batch: JpegBatch) -> RaggedImages:
+    """`Image.open(p).convert("RGB")` of every image of a device JpegBatch -> a device RaggedImages (the input of
+    resize_batch), bit for bit Pillow's output; mock rows stay mock rows.  Reads the per-image status back (one
+    synchronisation) and raises ValueError naming the images whose data is corrupt or whose entry does not fit; their
+    output is zeros."""
+    N.require_cuda(batch.data, batch.entries, batch.out_table)
+    if batch.data.dtype != torch.uint8 or batch.entries.dtype != torch.uint8 or batch.out_table.dtype != torch.int64:
+        raise ValueError("decode_batch: expected a JpegBatch from pack_jpegs")
+    dev = batch.device
+    with torch.cuda.device(dev):
+        out = torch.empty(max(batch.out_bytes, 1), dtype=torch.uint8, device=dev)
+        status = torch.empty(len(batch), dtype=torch.int32, device=dev)
+        ws = torch.empty(max(batch.workspace_bytes, 1), dtype=torch.uint8, device=dev)
+        _decode_enqueue(batch, out, status, ws)
+        st = status.cpu().numpy()
+    bad = np.flatnonzero(st)
+    if bad.size:
+        what = {1: "corrupt or truncated entropy-coded data", 2: "entry outside the data buffer",
+                4: "output entry does not fit", 8: "workspace too short"}
+        detail = ", ".join(f"{i}: " + " / ".join(v for k, v in what.items() if st[i] & k) for i in bad[:16])
+        raise ValueError(f"decode_batch: {bad.size} image(s) failed ({detail}{', ...' if bad.size > 16 else ''}); "
+                         "their output is zeros")
+    return RaggedImages(out, batch.out_table, batch.rows)
 
 
 def _resize_size(size):

@@ -12,8 +12,9 @@ the embeddings on the device and copies them to the host ONCE (the reference doe
 inference_utils.py:123-125), `calculate_centroids` is the segmented-mean kernel, and `get_similar` streams
 query x gallery distances into a per-query top-k without materialising the [Q, G] matrix or its argsort
 (get_similar.py:112-119); with `topk == 0` the full matrix path of the reference is kept.
-The image-folder datasets / PIL loading of the reference stay where they are (host JPEG decode is out of scope); a
-loader that ships the decoded images at native size as a RaggedImages has `T.Resize` run on the device.
+The image-folder datasets of the reference stay where they are.  A loader that ships file bytes as a JpegBatch
+(datasets.transforms.pack_jpegs) has the JPEG decode and `T.Resize` run on the device, bit for bit Pillow's; one that
+ships decoded images at native size as a RaggedImages has `T.Resize` run there.
 """
 from __future__ import annotations
 
@@ -25,7 +26,7 @@ import numpy as np
 import torch
 
 from .. import retrieval as R
-from ..datasets.transforms import RaggedImages, resize_batch
+from ..datasets.transforms import JpegBatch, RaggedImages, decode_batch, resize_batch
 from ..modelling.baseline import embed
 from ..reduce import calculate_centroids  # noqa: F401  (re-export: inference_utils.py:147-159)
 from ..utils.reid_metric import get_dist_func
@@ -37,10 +38,15 @@ def _inference(model, batch, use_cuda=True, normalize_with_bn=True, cfg=None):
     """inference_utils.py:104-113.  `model` exposes `.backbone` (ctl_b200 Baseline) and `.bn`.  `batch[0]` is the
     reference's float tensor [B, 3, H, W], or a RaggedImages of native-size images (datasets.transforms.pack_images):
     those are resized on the device to cfg.INPUT.SIZE_TEST (`T.Resize`, bit for bit PIL's) and embedded from uint8
-    with cfg.INPUT.PIXEL_MEAN / PIXEL_STD (TrunkEngine.forward_u8), so the loader ships native-size bytes only."""
+    with cfg.INPUT.PIXEL_MEAN / PIXEL_STD (TrunkEngine.forward_u8), so the loader ships native-size bytes only.  A
+    JpegBatch of file bytes (datasets.transforms.pack_jpegs) is first decoded on the device (decode_batch)."""
     if not use_cuda:
         raise RuntimeError("ctl_b200 has no CPU path (use_cuda=False); run the reference for CPU inference")
     data, _, filename = batch
+    if isinstance(data, JpegBatch):
+        if cfg is None:
+            raise ValueError("_inference: a JpegBatch needs cfg (INPUT.SIZE_TEST, PIXEL_MEAN, PIXEL_STD)")
+        data = decode_batch(data.to("cuda"))
     if isinstance(data, RaggedImages):
         if cfg is None:
             raise ValueError("_inference: a RaggedImages batch needs cfg (INPUT.SIZE_TEST, PIXEL_MEAN, PIXEL_STD)")
@@ -61,7 +67,8 @@ def _inference(model, batch, use_cuda=True, normalize_with_bn=True, cfg=None):
 
 def run_inference(model, val_loader, cfg, print_freq, use_cuda=True):
     """inference_utils.py:116-131 -> (embeddings float32 [N, D] numpy, paths numpy array).  The loader yields float
-    tensors as the reference's does, or RaggedImages of native-size images (resized on the device, see _inference)."""
+    tensors as the reference's does, RaggedImages of native-size images (resized on the device, see _inference), or
+    JpegBatch of file bytes (decoded and resized on the device)."""
     chunks, paths = [], []
     for pos, x in enumerate(val_loader):
         if pos % print_freq == 0:

@@ -709,6 +709,73 @@ int ctl_resize_bilinear_u8(const void* src, int64_t src_bytes, const void* table
                            int32_t out_w, void* out_u8_nhwc, int32_t* status, void* workspace, size_t workspace_bytes,
                            ctl_stream_t stream);
 
+/* ---- JPEG decode: Image.open(p).convert("RGB") (datasets/bases.py:32-33, inference/inference_utils.py:33-34) ----
+ * Pillow decodes with libjpeg-turbo's defaults (JDCT_ISLOW, fancy upsampling), fixed integer arithmetic that this
+ * reproduces bit for bit for baseline (SOF0) and extended-sequential Huffman (SOF1) files with 8-bit samples and one
+ * interleaved scan, grayscale or YCbCr, any integral sampling factors (4:4:4, 4:2:2, 4:2:0, 4:4:0, 4:1:1), with or
+ * without restart intervals, 8- or 16-bit quantisation tables and any Huffman tables:
+ *   - coefficients: Huffman decode with byte stuffing, RSTn resync and DC-predictor resets;
+ *   - jpeg_idct_islow (jidctint.c): coef * (short)quantval, CONST_BITS 13, PASS1_BITS 2, 64-bit products, an int
+ *     workspace, then x = sample - 128 clamped: sample = min(max(x + 128, 0), 255).  Pillow runs libjpeg-turbo's
+ *     SIMD IDCT, which saturates; the C path's range_limit[x & 1023] (jdmaster.c prepare_range_limit_table) agrees
+ *     on [-384, 512) and wraps outside it, which encoder output does not reach;
+ *   - upsampling per component (jdsample.c): h2v1 / h2v2 triangle ("fancy") filters when the component's downsampled
+ *     width is > 2, replication otherwise; h1v2 fancy always; replication for other integral ratios.  Neighbours are
+ *     clamped to the component's real downsampled width and height; rounding +1/+2 (h2v1, h1v2), +8/+7 (h2v2);
+ *   - ycc_rgb_convert (jdcolor.c): R = Y + ((91881 Cr' + 2^15) >> 16), G = Y + ((-46802 Cr' - 22554 Cb' + 2^15) >> 16),
+ *     B = Y + ((116130 Cb' + 2^15) >> 16) (Cb' = Cb - 128, Cr' = Cr - 128), each clamped to 0..255; grayscale gives
+ *     R = G = B = Y, as convert("RGB") of an "L" image does.
+ *
+ * ctl_jpeg_parse (host-only) reads the marker segments of one file up to SOS, never its entropy-coded data, and fills
+ * *desc (and *h, *w when not null).  It returns 0, or CTL_ERR_UNSUPPORTED for a JPEG this decode does not cover
+ * (progressive, lossless, hierarchical, arithmetic coding, not 8-bit, CMYK / YCCK, Adobe RGB (transform 0) or
+ * R/G/B component ids without JFIF, a first scan without every component, non-integral sampling factors), or
+ * CTL_ERR_INVALID_ARGUMENT for data that is not a JPEG or whose header is truncated or corrupt; ctl_last_error()
+ * names the reason.  The colour space follows libjpeg's guess: JFIF, Adobe transform 1 or other ids mean YCbCr.
+ * Offsets in the descriptor count from the file's first byte; the tables are the last definitions before SOS. */
+typedef struct ctl_jpeg_desc {
+  int32_t h, w;
+  uint32_t scan_begin, scan_end; /* entropy-coded data: from after SOS to the end of the file */
+  uint32_t dqt[3];               /* per component: its 64 quantisation values, zig-zag order */
+  uint32_t dht_dc[3], dht_ac[3]; /* per component: its DHT tables' 16 code-length counts, then their symbols */
+  uint16_t restart_interval;     /* MCUs per interval, 0: none */
+  uint8_t ncomp;                 /* 1 (grayscale) or 3 (YCbCr) */
+  uint8_t dqt16;                 /* bit c: component c's quantisation values are 16-bit big-endian */
+  uint8_t hs[3], vs[3];          /* sampling factors; 1 for grayscale */
+  uint8_t reserved[2];
+} ctl_jpeg_desc;
+
+#define CTL_JPEG_ENTRY_JPEG 0 /* a JPEG file described by desc */
+#define CTL_JPEG_ENTRY_RAW 1  /* HWC RGB uint8 bytes of desc.h x desc.w, copied through */
+#define CTL_JPEG_ENTRY_MOCK 2 /* a mock row: no bytes, an output entry with h = w = 0 */
+
+typedef struct ctl_jpeg_entry {
+  int64_t offset; /* first byte of the entry in src */
+  int64_t nbytes;
+  int32_t kind;   /* CTL_JPEG_ENTRY_* */
+  int32_t reserved;
+  ctl_jpeg_desc desc;
+} ctl_jpeg_entry;
+
+/* ctl_jpeg_decode: src holds n entries packed back to back at any byte alignment (entries_device: n struct
+ * ctl_jpeg_entry in device memory).  Entry i is written as HWC RGB uint8 at out_u8 + out_table_device[i].offset
+ * (struct ctl_resize_entry, whose h and w must be the entry's: 0 for a mock row), so the output is the ragged
+ * input of ctl_resize_bilinear_u8.  status: int32 [n] on the device, written for every entry (the call needs no
+ * clearing): 0 or an OR of 1 (entropy-coded data ending before the last MCU, a Huffman code that does not exist, a
+ * coefficient index > 63, a missing RSTn marker), 2 (an entry outside src_bytes, or a descriptor ctl_jpeg_parse
+ * cannot have written), 4 (an output entry of another size or outside out_bytes), 8 (a workspace too short for the
+ * entry).  Such an entry's output is zeros (status 4: untouched); the others are unaffected, and nothing outside the
+ * buffers is read or written.  workspace: planned by ctl_jpeg_decode_workspace_bytes (host-only, from the host copy
+ * of the entries; 0 for null or n < 1): an offset per entry, then per JPEG its int16 coefficients and uint8
+ * component planes (3 bytes per coefficient).  Three launches (entropy decode, one thread per image; IDCT; upsample +
+ * colour convert); no host synchronisation, no allocation: capturable in a CUDA graph.  A null pointer, n < 1, a
+ * negative buffer size or a workspace shorter than its header is CTL_ERR_INVALID_ARGUMENT before any device work. */
+int ctl_jpeg_parse(const void* bytes, int64_t nbytes, ctl_jpeg_desc* desc, int32_t* h, int32_t* w);
+size_t ctl_jpeg_decode_workspace_bytes(const ctl_jpeg_entry* entries_host, int64_t n);
+int ctl_jpeg_decode(const void* src, int64_t src_bytes, const void* entries_device, int64_t n,
+                    const void* out_table_device, void* out_u8, int64_t out_bytes, int32_t* status, void* workspace,
+                    size_t workspace_bytes, ctl_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
