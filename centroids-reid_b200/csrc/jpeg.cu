@@ -14,9 +14,10 @@
 //     +1/+2 (h2v1, h1v2) and +8/+7 (h2v2);
 //   * ycc_rgb_convert (jdcolor.c): SCALEBITS 16 tables with ONE_HALF rounding, then a clamp; grayscale writes
 //     R = G = B = Y as convert("RGB") of an "L" image does.
-// Three launches, one image per CTA row: entropy decode (one thread per image, its Huffman tables built by its warp
-// in shared memory from the file's own DHT bytes), IDCT (eight threads per 8x8 block), upsample + colour convert
-// (one thread per output pixel).  The host parser below (ctl_jpeg_parse) reads the marker segments up to SOS; it is the
+// Three launches, one image per CTA row: entropy decode (one CTA per image, its Huffman tables built in shared memory
+// from the file's own DHT bytes, its entropy-coded data split into up to 256 subsequences decoded in parallel and
+// brought into step by sync rounds), IDCT (eight threads per 8x8 block), upsample + colour convert (one thread per
+// output pixel).  The host parser below (ctl_jpeg_parse) reads the marker segments up to SOS; it is the
 // only code that knows the JPEG file format, and it never reads the entropy-coded data.
 #include <stdint.h>
 #include <string.h>
@@ -89,6 +90,33 @@ __host__ __device__ inline size_t jpeg_header_bytes(long long n) {
 
 // ---------------------------------------------------------------------------------------------------------------
 // entropy decode
+//
+// One CTA of JD_ENTROPY_THREADS threads per image, each thread one subsequence of the entropy-coded data.
+// Positions are bit offsets in scan coordinates: the bytes after SOS with the stuffed 0x00 of every 0xFF 0x00 pair left
+// out (marker bytes count), so a restart segment (the data between SOS or an RSTn and the next marker) is one
+// contiguous range.  The image's S-bit subsequences partition them; S = max(JD_SUB_MIN_BITS, ceil(bits / T)) rounded
+// to a word, so an image never has more than T subsequences.  The decode state at a position is (block u of the MCU,
+// coefficient index k); restart-segment starts are exact states (0, 0).
+//   1. marker scan: each thread scans T-th of the bytes for stuffing zeros and marker runs; CTA-wide scans of the
+//      counts give each chunk's scan coordinate and each marker its index, and the restart-segment table (start,
+//      data end, the RST number that follows) is written to the image's plane region, which the IDCT fills later.
+//   2. speculative pass: thread i decodes from the start of subsequence i as if a block began there (an invalid code
+//      resumes at the next bit with state (0, 0)) until it crosses into subsequence i + 1, and records that exit.
+//   3. sync rounds: every thread whose predecessor's exit changed decodes again from it, until no exit changes.  The
+//      decoder self-synchronises, so this takes a few rounds; round r has the first r subsequences exact, so the
+//      loop ends after at most T rounds.
+//   4. counts: from the converged decodes, CTA-wide segmented scans of the blocks each subsequence completes and of
+//      its DC differences (32-bit wrapping sums, the low 16 bits of the serial predictors) give every subsequence its
+//      first block and DC predictors; they restart at every restart segment.
+//   5. write pass: each thread decodes its part of the true path again and stores the dezigzagged coefficients.
+// Errors count on the true path only, before the image's last block, and are the serial reader's: an invalid code, a
+// DC magnitude > 15, a coefficient index > 63, bits consumed past a marker or the end of the data (zeros are read
+// there), an RSTn missing or out of sequence after an interval (the bytes the reader had not loaded before it may be
+// padding without 0xFF, and 0xFF fill bytes may precede the marker).
+
+constexpr int JD_ENTROPY_THREADS = 256;
+constexpr long long JD_SUB_MIN_BITS = 1024;
+constexpr long long JD_TERMINAL = 1LL << 62;  // the state past the last restart segment
 
 struct HuffTable {
   uint16_t lut[512];  // 9-bit lookahead: (code length << 8) | symbol, 0 for a longer code
@@ -97,15 +125,31 @@ struct HuffTable {
   uint8_t val[256];
 };
 
-struct BitReader {
-  const uint8_t* p;
-  const uint8_t* end;
-  uint64_t buf;  // next bits, MSB first
-  int n;         // valid bits in buf
-  int fake;      // zero bits appended past a marker or the end of the data (the last `fake` of the n)
-  bool marker;   // stopped at a marker
-  bool bad;
+// restart segment j: starts at file byte s_off (scan coordinate s_u bytes), its data ends at the marker at q_off
+// (q_u), which is RSTn with n = rst, or rst = -1 (another marker, or the end of the data)
+struct JSeg {
+  uint32_t s_off, s_u, q_off, q_u;
+  int32_t rst;
+};
 
+struct BitReader {
+  const uint8_t* p;  // next byte to load
+  const uint8_t* end;
+  uint64_t buf;      // next bits, MSB first
+  int n;             // valid bits in buf
+  bool marker;       // stopped at a marker: zeros from here on
+  long long pos;     // scan-coordinate bit of the next unconsumed bit
+  long long pu;      // scan-coordinate byte of p
+
+  __device__ __forceinline__ void init(const uint8_t* at, const uint8_t* e, long long ubyte) {
+    p = at;
+    end = e;
+    buf = 0;
+    n = 0;
+    marker = false;
+    pos = ubyte * 8;
+    pu = ubyte;
+  }
   __device__ __forceinline__ void fill() {
     while (n <= 56) {
       uint32_t b = 0;
@@ -114,16 +158,15 @@ struct BitReader {
         if (b == 0xFF) {
           if (p + 1 < end && p[1] == 0x00) {
             p += 2;
+            ++pu;
           } else {
             marker = true;  // a marker (or the end of the data) inside a stuffed pair: zeros from here on
             b = 0;
-            fake += 8;
           }
         } else {
           ++p;
+          ++pu;
         }
-      } else {
-        fake += 8;
       }
       buf |= (uint64_t)b << (56 - n);
       n += 8;
@@ -133,23 +176,24 @@ struct BitReader {
   __device__ __forceinline__ void consume(int k) {
     buf <<= k;
     n -= k;
-    if (n < fake) bad = true;  // decoded bits that the data does not contain
+    pos += k;
   }
-  __device__ __forceinline__ int decode(const HuffTable& t) {
+  // the symbol of the code at the head of the buffer and its length (0: no code of up to 16 bits); consumes nothing
+  __device__ __forceinline__ int lookup(const HuffTable& t, int& len) const {
     const uint32_t e = t.lut[peek(9)];
     if (e) {
-      consume(e >> 8);
+      len = e >> 8;
       return e & 0xFF;
     }
     const uint32_t code = peek(16);
     for (int l = 10; l <= 16; ++l) {
       const int c = (int)(code >> (16 - l));
       if (c <= t.maxcode[l]) {
-        consume(l);
+        len = l;
         return t.val[(t.valoff[l] + c) & 0xFF];
       }
     }
-    bad = true;  // no code of up to 16 bits
+    len = 0;
     return 0;
   }
   __device__ __forceinline__ int receive_extend(int s) {
@@ -158,16 +202,11 @@ struct BitReader {
     consume(s);
     return v < (1 << (s - 1)) ? v - (1 << s) + 1 : v;
   }
-  // the RSTn marker expected after a restart interval: drop the buffered bits and resume after it
-  __device__ bool restart(int expect) {
-    buf = 0;
-    n = fake = 0;
-    marker = false;
-    while (p < end && *p != 0xFF) ++p;  // bits the encoder padded past the interval: not expected, tolerated
-    while (p < end && *p == 0xFF) ++p;
-    if (p >= end || *p != 0xD0 + expect) return false;
-    ++p;
-    return true;
+  // file offset of the byte holding scan byte x <= pu (x within the data loaded so far): back from p over whole bytes
+  __device__ __forceinline__ uint32_t locate(long long x, const uint8_t* file, const uint8_t* scan) const {
+    const uint8_t* q = p;
+    for (long long u = pu; u > x; --u) q -= (q - 2 >= scan && q[-1] == 0x00 && q[-2] == 0xFF) ? 2 : 1;
+    return (uint32_t)(q - file);
   }
 };
 
@@ -176,7 +215,8 @@ __constant__ uint8_t kZigzag[64] = {0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 
                                     35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23, 30, 37, 44, 51,
                                     58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
 
-// false for a table whose symbols fall outside the file or whose code lengths overflow the code space
+// false for a table whose symbols fall outside the file or whose code lengths overflow the code space; called by
+// warp 0
 __device__ bool build_huff(const uint8_t* file, long long nbytes, uint32_t off, HuffTable& t) {
   const int lane = threadIdx.x;
   __shared__ int ok_s;
@@ -218,65 +258,337 @@ __device__ bool build_huff(const uint8_t* file, long long nbytes, uint32_t off, 
 
 __device__ __forceinline__ bool in_file(uint32_t off, long long len, long long nbytes) { return (long long)off + len <= nbytes; }
 
-// One warp per entry: validates the entry, its output slot and its workspace region (whose offset it records in the
-// workspace header), builds the Huffman tables, then lane 0 decodes every MCU into int16 coefficient blocks.
-__global__ void __launch_bounds__(32) jpeg_entropy_kernel(const uint8_t* __restrict__ src, long long src_bytes,
-                                                          const ctl_jpeg_entry* __restrict__ entries,
-                                                          const ctl_resize_entry* __restrict__ out_table,
-                                                          long long out_bytes, uint8_t* __restrict__ ws,
-                                                          long long ws_bytes, long long n, int* __restrict__ status) {
+// element of the CTA-wide segmented scans: f marks a restart inside the element (its v then count from it)
+struct JAgg {
+  int f;
+  uint32_t v[4];
+};
+
+__device__ __forceinline__ JAgg jagg_combine(const JAgg& a, const JAgg& b) {
+  if (b.f) return b;
+  JAgg r = a;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) r.v[q] += b.v[q];
+  return r;
+}
+
+__device__ __forceinline__ JAgg jagg_shfl_up(const JAgg& a, int o) {
+  JAgg r;
+  r.f = __shfl_up_sync(0xffffffffu, a.f, o);
+#pragma unroll
+  for (int q = 0; q < 4; ++q) r.v[q] = __shfl_up_sync(0xffffffffu, a.v[q], o);
+  return r;
+}
+
+// exclusive segmented scan over the CTA's threads in thread order; `tot` is shared scratch of a warp count
+__device__ JAgg jagg_exclusive_scan(JAgg x, JAgg* tot) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  constexpr int nwarps = JD_ENTROPY_THREADS / 32;
+  const JAgg zero = {0, {0, 0, 0, 0}};
+  JAgg inc = x;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const JAgg y = jagg_shfl_up(inc, o);
+    if (lane >= o) inc = jagg_combine(y, inc);
+  }
+  if (lane == 31) tot[warp] = inc;
+  __syncthreads();
+  if (warp == 0) {
+    JAgg w = lane < nwarps ? tot[lane] : zero;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const JAgg y = jagg_shfl_up(w, o);
+      if (lane >= o) w = jagg_combine(y, w);
+    }
+    if (lane < nwarps) tot[lane] = w;
+  }
+  __syncthreads();
+  JAgg before = jagg_shfl_up(inc, 1);
+  if (lane == 0) before = zero;
+  const JAgg r = warp ? jagg_combine(tot[warp - 1], before) : before;
+  __syncthreads();  // tot is reused by the next scan
+  return r;
+}
+
+// what the decoding threads of one image share
+struct JCtx {
+  const uint8_t* file;
+  const uint8_t* scan;  // file + scan_begin
+  const uint8_t* end;   // file + scan_end
+  const JSeg* seg;      // restart-segment table (in the image's plane region)
+  int nseg;             // segments the data has, at most `needed`
+  int needed;           // segments the image has: ceil(MCUs / restart interval), 1 without restarts
+  int ri, bpm;          // restart interval (MCUs, 0: none), blocks per MCU
+  long long total;      // blocks of the image
+  const HuffTable* dc;
+  const HuffTable* ac;
+  const uint8_t* comp;  // component of each block of an MCU
+  __device__ __forceinline__ long long base(int j) const { return ri ? (long long)j * ri * bpm : 0; }
+  __device__ __forceinline__ long long quota(int j) const {
+    return ri ? min((long long)ri * bpm, total - base(j)) : total;
+  }
+  __device__ __forceinline__ long long seg_end(int j) const { return (long long)seg[j].q_u * 8; }
+};
+
+// decode state at a position: segment j, block u of the MCU, coefficient k; off = file offset of the byte of pos
+struct JState {
+  long long pos;
+  uint32_t off;
+  int j, u, k;
+};
+
+// Speculative / sync decode from s until a step would start at or past `stop`; s becomes the exit.  rec: blocks
+// completed and DC differences per component since the entry, or, once a restart segment began (f = 1), its first
+// block index and the differences since that start.
+__device__ void jd_walk(const JCtx& cx, JState& s, long long stop, JAgg& rec) {
+  rec = JAgg{0, {0, 0, 0, 0}};
+  if (s.j >= cx.nseg || s.pos >= stop) return;
+  BitReader br;
+  br.init(cx.file + s.off, cx.end, s.pos >> 3);
+  br.fill();
+  br.consume((int)(s.pos & 7));
+  int u = s.u, k = s.k, j = s.j;
+  long long segend = cx.seg_end(j);
+  for (;;) {
+    if (br.pos >= segend) {  // the next restart segment starts fresh
+      rec = JAgg{1, {0, 0, 0, 0}};
+      if (++j >= cx.nseg) {
+        s = JState{JD_TERMINAL, 0, cx.nseg, 0, 0};
+        return;
+      }
+      rec.v[0] = (uint32_t)cx.base(j);
+      u = k = 0;
+      br.init(cx.file + cx.seg[j].s_off, cx.end, cx.seg[j].s_u);
+      segend = cx.seg_end(j);
+      continue;
+    }
+    if (br.pos >= stop) break;
+    br.fill();
+    const int c = cx.comp[u];
+    int len;
+    const int sym = br.lookup(k ? cx.ac[c] : cx.dc[c], len);
+    if (k == 0) {
+      if (!len || sym > 15) {  // not a block start: resume at the next bit
+        br.consume(1);
+        u = 0;
+        continue;
+      }
+      br.consume(len);
+      rec.v[1 + c] += (uint32_t)br.receive_extend(sym);
+      k = 1;
+    } else {
+      const int r = sym >> 4, sz = sym & 15;
+      if (!len || (sz && k + r > 63)) {
+        br.consume(1);
+        u = k = 0;
+        continue;
+      }
+      br.consume(len);
+      if (sz) {
+        br.consume(sz);
+        k += r + 1;
+      } else {
+        k = r == 15 ? k + 16 : 64;  // ZRL or end of block
+      }
+    }
+    if (k >= 64) {
+      k = 0;
+      u = u + 1 == cx.bpm ? 0 : u + 1;
+      ++rec.v[0];
+    }
+  }
+  s = JState{br.pos, br.locate(br.pos >> 3, cx.file, cx.scan), j, u, k};
+}
+
+// the serial reader's check at the end of interval j: from where it stopped loading, only padding without 0xFF up to
+// the marker, and the marker is RSTn with n = j mod 8
+__device__ __forceinline__ bool jd_restart_ok(const JCtx& cx, int j, const uint8_t* p) {
+  const JSeg sg = cx.seg[j];
+  if (sg.rst != (j & 7)) return false;
+  for (const uint8_t* q = p; q < cx.file + sg.q_off; ++q)
+    if (*q == 0xFF) return false;
+  return true;
+}
+
+// Write pass of one subsequence: the true path from s (block sb, DC predictors pred) until `stop`, storing the
+// coefficients; true on an error of the serial decode.
+__device__ bool jd_write(const JCtx& cx, JState s, long long stop, long long sb, int pred[3], const JGeom& g,
+                         int16_t* const coef[3], const uint8_t* vrow, const uint8_t* hcol) {
+  if (s.j >= cx.nseg || s.pos >= stop) return false;
+  BitReader br;
+  br.init(cx.file + s.off, cx.end, s.pos >> 3);
+  br.fill();
+  br.consume((int)(s.pos & 7));
+  int u = s.u, k = s.k, j = s.j;
+  long long segend = cx.seg_end(j), base = cx.base(j), quota = cx.quota(j);
+  bool completed = false;  // the last step ended a block
+  int16_t* blk = nullptr;
+  for (;;) {
+    const bool done = sb - base >= quota;
+    if (done || br.pos >= segend) {
+      if (!done) return true;                                          // the data ends inside the interval
+      if (j + 1 >= cx.needed) return false;                            // the image's last block is written
+      if (completed && !jd_restart_ok(cx, j, br.p)) return true;       // checked by the thread that ended it
+      if (++j >= cx.nseg) return false;                                // (then the check above failed)
+      base = sb = cx.base(j);
+      quota = cx.quota(j);
+      pred[0] = pred[1] = pred[2] = 0;
+      u = k = 0;
+      br.init(cx.file + cx.seg[j].s_off, cx.end, cx.seg[j].s_u);
+      segend = cx.seg_end(j);
+      completed = false;
+      continue;
+    }
+    if (br.pos >= stop) return false;
+    completed = false;
+    const int c = cx.comp[u];
+    if (k == 0 || !blk) {
+      const long long m = sb / cx.bpm;
+      const int my = (int)(m / g.mcux), mx = (int)(m % g.mcux);
+      blk = coef[c] + ((size_t)(my * g.vs[c] + vrow[u]) * g.bw[c] + mx * g.hs[c] + hcol[u]) * 64;
+    }
+    br.fill();
+    int len;
+    const int sym = br.lookup(k ? cx.ac[c] : cx.dc[c], len);
+    if (!len) return true;
+    br.consume(len);
+    if (k == 0) {
+      if (sym > 15) return true;
+      pred[c] = (int)((uint32_t)pred[c] + (uint32_t)br.receive_extend(sym));
+      blk[0] = (int16_t)pred[c];
+      k = 1;
+    } else {
+      const int r = sym >> 4, sz = sym & 15;
+      if (sz) {
+        k += r;
+        if (k > 63) return true;
+        blk[kZigzag[k]] = (int16_t)br.receive_extend(sz);
+        ++k;
+      } else {
+        k = r == 15 ? k + 16 : 64;
+      }
+    }
+    if (br.pos > segend) return true;  // bits consumed past the data
+    if (k >= 64) {
+      k = 0;
+      u = u + 1 == cx.bpm ? 0 : u + 1;
+      ++sb;
+      completed = true;
+    }
+  }
+}
+
+// file offset of scan byte x, from the chunk table (chunk_u[c]: scan byte at file byte begin + c * csize; ~0u past
+// the data): the first byte at or after the chunk start with x scan bytes before it that is not a stuffed zero
+__device__ uint32_t jd_map(const uint8_t* file, uint32_t begin, uint32_t end, uint32_t csize, const uint32_t* chunk_u,
+                           long long x) {
+  if (begin >= end) return begin;
+  int lo = 0, hi = JD_ENTROPY_THREADS - 1;  // chunk_u[0] = 0 <= x
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if ((long long)chunk_u[mid] <= x) lo = mid;
+    else hi = mid - 1;
+  }
+  uint32_t i = begin + (uint32_t)lo * csize;
+  long long u = chunk_u[lo];
+  for (; i < end; ++i) {
+    if (i > begin && file[i] == 0x00 && file[i - 1] == 0xFF) continue;
+    if (u == x) break;
+    ++u;
+  }
+  return i;
+}
+
+__device__ __forceinline__ bool jd_stuffed(const uint8_t* f, uint32_t i, uint32_t begin) {
+  return i > begin && f[i] == 0x00 && f[i - 1] == 0xFF;
+}
+__device__ __forceinline__ bool jd_marker(const uint8_t* f, uint32_t i, uint32_t begin, uint32_t end) {
+  return f[i] == 0xFF && (i + 1 == end || f[i + 1] != 0x00) && (i == begin || f[i - 1] != 0xFF);
+}
+
+// One CTA per entry.  Warp 0 validates the entry, its output slot and its workspace region (whose offset it records in
+// the workspace header) and builds the Huffman tables; then the CTA decodes the image as described above.
+__global__ void __launch_bounds__(JD_ENTROPY_THREADS, 1) jpeg_entropy_kernel(
+    const uint8_t* __restrict__ src, long long src_bytes, const ctl_jpeg_entry* __restrict__ entries,
+    const ctl_resize_entry* __restrict__ out_table, long long out_bytes, uint8_t* __restrict__ ws, long long ws_bytes,
+    long long n, int* __restrict__ status) {
+  constexpr int T = JD_ENTROPY_THREADS;
   __shared__ HuffTable dc[3], ac[3];
+  __shared__ uint32_t chunk_u[T];
+  __shared__ long long x_pos[T];
+  __shared__ uint32_t x_off[T];
+  __shared__ int x_j[T], x_uk[T];
+  __shared__ JAgg tot[T / 32];
+  __shared__ uint8_t comp[10], vrow[10], hcol[10];
+  __shared__ long long region_s;
+  __shared__ int go_s, first_other_s, err_s;
   pdl_launch_dependents();
   pdl_wait();
-  const int b = blockIdx.x, lane = threadIdx.x;
-  long long region = 0;
-  for (long long j = lane; j < b; j += 32) region += jpeg_region_bytes(entries[j]);
-  for (int o = 16; o > 0; o >>= 1) region += __shfl_xor_sync(0xffffffffu, region, o);
-  region += jpeg_header_bytes(n);
+  const int b = blockIdx.x, tid = threadIdx.x;
   const ctl_jpeg_entry e = entries[b];
-  const ctl_resize_entry o = out_table[b];
-  long long* ws_off = reinterpret_cast<long long*>(ws);
-  if (lane == 0) ws_off[b] = region;
-
-  int st = 0;
-  JGeom g;
-  const bool jpeg = e.kind == CTL_JPEG_ENTRY_JPEG;
-  if (e.kind == CTL_JPEG_ENTRY_MOCK) {
-    if (o.h != 0 || o.w != 0) st |= JS_OUTPUT;
-  } else if (!jpeg && e.kind != CTL_JPEG_ENTRY_RAW) {
-    st |= JS_ENTRY;
-  } else {
-    if (e.offset < 0 || e.nbytes < 0 || e.offset > src_bytes || e.nbytes > src_bytes - e.offset) st |= JS_ENTRY;
-    if (e.desc.h < 1 || e.desc.w < 1 || e.desc.h > JD_MAX_SIDE || e.desc.w > JD_MAX_SIDE) st |= JS_ENTRY;
-    if (!jpeg && e.nbytes != (long long)e.desc.h * e.desc.w * 3) st |= JS_ENTRY;
-    if (jpeg) {
-      const ctl_jpeg_desc& d = e.desc;
-      if (!jpeg_geom(d, g) || d.scan_begin > d.scan_end || !in_file(d.scan_end, 0, e.nbytes)) st |= JS_ENTRY;
-      for (int c = 0; c < d.ncomp && c < 3; ++c)
-        if (!in_file(d.dqt[c], (d.dqt16 >> c & 1) ? 128 : 64, e.nbytes)) st |= JS_ENTRY;
-      if (!st && region + jpeg_region_bytes(e) > ws_bytes) st |= JS_WORKSPACE;
+  if (tid < 32) {
+    const int lane = tid;
+    long long region = 0;
+    for (long long j = lane; j < b; j += 32) region += jpeg_region_bytes(entries[j]);
+    for (int o = 16; o > 0; o >>= 1) region += __shfl_xor_sync(0xffffffffu, region, o);
+    region += jpeg_header_bytes(n);
+    const ctl_resize_entry o = out_table[b];
+    if (lane == 0) reinterpret_cast<long long*>(ws)[b] = region;
+    int st = 0;
+    JGeom g;
+    const bool jpeg = e.kind == CTL_JPEG_ENTRY_JPEG;
+    if (e.kind == CTL_JPEG_ENTRY_MOCK) {
+      if (o.h != 0 || o.w != 0) st |= JS_OUTPUT;
+    } else if (!jpeg && e.kind != CTL_JPEG_ENTRY_RAW) {
+      st |= JS_ENTRY;
+    } else {
+      if (e.offset < 0 || e.nbytes < 0 || e.offset > src_bytes || e.nbytes > src_bytes - e.offset) st |= JS_ENTRY;
+      if (e.desc.h < 1 || e.desc.w < 1 || e.desc.h > JD_MAX_SIDE || e.desc.w > JD_MAX_SIDE) st |= JS_ENTRY;
+      if (!jpeg && e.nbytes != (long long)e.desc.h * e.desc.w * 3) st |= JS_ENTRY;
+      if (jpeg) {
+        const ctl_jpeg_desc& d = e.desc;
+        if (!jpeg_geom(d, g) || d.scan_begin > d.scan_end || !in_file(d.scan_end, 0, e.nbytes)) st |= JS_ENTRY;
+        for (int c = 0; c < d.ncomp && c < 3; ++c)
+          if (!in_file(d.dqt[c], (d.dqt16 >> c & 1) ? 128 : 64, e.nbytes)) st |= JS_ENTRY;
+        if (!st && region + jpeg_region_bytes(e) > ws_bytes) st |= JS_WORKSPACE;
+      }
+      if (o.h != e.desc.h || o.w != e.desc.w || o.offset < 0 || o.offset > out_bytes ||
+          o.h * o.w * 3 > out_bytes - o.offset)
+        st |= JS_OUTPUT;
     }
-    if (o.h != e.desc.h || o.w != e.desc.w || o.offset < 0 || o.offset > out_bytes ||
-        o.h * o.w * 3 > out_bytes - o.offset)
-      st |= JS_OUTPUT;
+    bool go = jpeg && !st;
+    if (go) {
+      const uint8_t* file = src + e.offset;
+      bool ok = true;
+      for (int c = 0; c < g.nc; ++c) {
+        ok = build_huff(file, e.nbytes, e.desc.dht_dc[c], dc[c]) && ok;
+        ok = build_huff(file, e.nbytes, e.desc.dht_ac[c], ac[c]) && ok;
+      }
+      if (!ok) st = JS_ENTRY;
+      go = ok;
+    }
+    if (lane == 0) {
+      if (!go) status[b] = st;
+      region_s = region;
+      go_s = go;
+      first_other_s = INT32_MAX;
+      err_s = 0;
+      if (go) {
+        int i = 0;
+        for (int c = 0; c < g.nc; ++c)
+          for (int v = 0; v < g.vs[c]; ++v)
+            for (int h = 0; h < g.hs[c]; ++h, ++i) comp[i] = (uint8_t)c, vrow[i] = (uint8_t)v, hcol[i] = (uint8_t)h;
+      }
+    }
   }
-  if (!jpeg || st) {
-    if (lane == 0) status[b] = st;
-    return;
-  }
+  __syncthreads();
+  if (!go_s) return;  // CTA-uniform
 
+  JGeom g;
+  jpeg_geom(e.desc, g);
+  const long long region = region_s;
   const uint8_t* file = src + e.offset;
-  bool ok = true;
-  for (int c = 0; c < g.nc; ++c) {
-    ok = build_huff(file, e.nbytes, e.desc.dht_dc[c], dc[c]) && ok;
-    ok = build_huff(file, e.nbytes, e.desc.dht_ac[c], ac[c]) && ok;
-  }
-  if (!ok) {
-    if (lane == 0) status[b] = JS_ENTRY;
-    return;
-  }
-  if (lane != 0) return;
-
+  const uint32_t begin = e.desc.scan_begin, end = e.desc.scan_end;
   int16_t* coef[3];
   {
     int16_t* base = reinterpret_cast<int16_t*>(ws + region);
@@ -284,59 +596,132 @@ __global__ void __launch_bounds__(32) jpeg_entropy_kernel(const uint8_t* __restr
       coef[c] = base;
       base += (size_t)g.bw[c] * g.bh[c] * 64;
     }
+    uint4* z = reinterpret_cast<uint4*>(ws + region);  // the write pass stores only the nonzero coefficients
+    for (long long i = tid; i < g.blocks * 8; i += T) z[i] = make_uint4(0, 0, 0, 0);
   }
-  BitReader br{file + e.desc.scan_begin, file + e.desc.scan_end, 0, 0, 0, false, false};
-  int pred[3] = {0, 0, 0};
-  const int ri = e.desc.restart_interval;
+  JSeg* seg = reinterpret_cast<JSeg*>(ws + region + g.blocks * 128);  // <= MCUs entries of 20 B in 64 B per block
   const long long mcus = (long long)g.mcux * g.mcuy;
-  int rst = 0;
-  for (long long m = 0; m < mcus && !br.bad; ++m) {
-    if (ri && m && m % ri == 0) {
-      if (!br.restart(rst)) {
-        br.bad = true;
-        break;
-      }
-      rst = (rst + 1) & 7;
-      pred[0] = pred[1] = pred[2] = 0;
-    }
-    const int my = (int)(m / g.mcux), mx = (int)(m % g.mcux);
-    for (int c = 0; c < g.nc && !br.bad; ++c) {
-      for (int v = 0; v < g.vs[c]; ++v) {
-        for (int h = 0; h < g.hs[c]; ++h) {
-          int16_t* blk = coef[c] + ((size_t)(my * g.vs[c] + v) * g.bw[c] + mx * g.hs[c] + h) * 64;
-          uint4* z = reinterpret_cast<uint4*>(blk);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) z[i] = make_uint4(0, 0, 0, 0);
-          br.fill();
-          const int s = br.decode(dc[c]);
-          if (s > 15) br.bad = true;
-          pred[c] += br.receive_extend(s & 15);
-          blk[0] = (int16_t)pred[c];
-          for (int k = 1; k < 64;) {
-            br.fill();
-            const int rs = br.decode(ac[c]);
-            const int r = rs >> 4, sz = rs & 15;
-            if (sz) {
-              k += r;
-              if (k > 63) {
-                br.bad = true;
-                break;
-              }
-              blk[kZigzag[k]] = (int16_t)br.receive_extend(sz);
-            } else if (r != 15) {
-              break;  // end of block
-            } else {
-              k += 15;  // ZRL
-            }
-            ++k;
-          }
-          if (br.bad) break;
+  const int ri = e.desc.restart_interval;
+  const int needed = ri ? (int)((mcus + ri - 1) / ri) : 1;
+
+  // 1. marker scan over T chunks of the scan bytes
+  const uint32_t len = end - begin, csize = (len + T - 1) / T;
+  const uint32_t c0 = min(begin + (uint32_t)tid * csize, end), c1 = min(c0 + csize, end);
+  JAgg cnt = {0, {0, 0, 0, 0}};
+  for (uint32_t i = c0; i < c1; ++i) {
+    cnt.v[0] += jd_stuffed(file, i, begin);
+    cnt.v[1] += jd_marker(file, i, begin, end);
+  }
+  const JAgg pre = jagg_exclusive_scan(cnt, tot);
+  chunk_u[tid] = c0 < end ? (uint32_t)(c0 - begin) - pre.v[0] : ~0u;
+  {
+    long long u = (long long)(c0 - begin) - pre.v[0];
+    long long m = pre.v[1];
+    for (uint32_t i = c0; i < c1 && m < needed; ++i) {
+      if (jd_stuffed(file, i, begin)) continue;
+      if (jd_marker(file, i, begin, end)) {
+        uint32_t r = i;
+        while (r < end && file[r] == 0xFF) ++r;
+        const int rst = ri && r < end && file[r] >= 0xD0 && file[r] <= 0xD7 ? file[r] - 0xD0 : -1;
+        seg[m].q_off = i;
+        seg[m].q_u = (uint32_t)u;
+        seg[m].rst = rst;
+        if (rst < 0) atomicMin(&first_other_s, (int)m);
+        if (rst >= 0 && m + 1 < needed) {
+          seg[m + 1].s_off = r + 1;
+          seg[m + 1].s_u = (uint32_t)(u + (r + 1 - i));
         }
-        if (br.bad) break;
+        ++m;
       }
+      ++u;
     }
   }
-  status[b] = br.bad ? JS_DATA : 0;
+  if (tid == T - 1) {  // totals: the inclusive scan of the last chunk
+    const uint32_t marks = pre.v[1] + cnt.v[1];
+    const uint32_t bytes = len - (pre.v[0] + cnt.v[0]);
+    x_off[0] = marks;  // handed to the CTA below
+    x_off[1] = bytes;
+  }
+  if (tid == 0) {
+    seg[0].s_off = begin;
+    seg[0].s_u = 0;
+  }
+  __syncthreads();
+  const uint32_t marks = x_off[0], scan_bytes = x_off[1];
+  const int nseg = min(needed, min(first_other_s, marks > (uint32_t)INT32_MAX ? INT32_MAX : (int)marks) + 1);
+  __syncthreads();
+  if (tid == 0 && (uint32_t)(nseg - 1) >= marks) {  // the last segment runs to the end of the data
+    seg[nseg - 1].q_off = end;
+    seg[nseg - 1].q_u = scan_bytes;
+    seg[nseg - 1].rst = -1;
+  }
+  __syncthreads();
+
+  JCtx cx;
+  cx.file = file;
+  cx.scan = file + begin;
+  cx.end = file + end;
+  cx.seg = seg;
+  cx.nseg = nseg;
+  cx.needed = needed;
+  cx.ri = ri;
+  cx.bpm = (int)(g.blocks / mcus);
+  cx.total = g.blocks;
+  cx.dc = dc;
+  cx.ac = ac;
+  cx.comp = comp;
+
+  // 2. speculative pass
+  const long long bits = cx.seg_end(nseg - 1);
+  const long long S = (max(JD_SUB_MIN_BITS, (bits + T - 1) / T) + 31) & ~31LL;
+  const int nsub = (int)max(1LL, (bits + S - 1) / S);
+  const bool live = tid < nsub;
+  const long long stop = tid + 1 == nsub ? JD_TERMINAL : (tid + 1) * S;
+  JState entry{0, begin, 0, 0, 0};
+  JAgg rec = {0, {0, 0, 0, 0}};
+  if (live) {
+    const long long p0 = tid * S;
+    int lo = 0, hi = nseg - 1;  // the segment holding p0: the last one starting at or before it
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if ((long long)seg[mid].s_u * 8 <= p0) lo = mid;
+      else hi = mid - 1;
+    }
+    entry = JState{p0, jd_map(file, begin, end, csize, chunk_u, p0 >> 3), lo, 0, 0};
+    JState s = entry;
+    jd_walk(cx, s, stop, rec);
+    x_pos[tid] = s.pos;
+    x_off[tid] = s.off;
+    x_j[tid] = s.j;
+    x_uk[tid] = s.u | s.k << 8;
+  }
+  // 3. sync rounds
+  for (;;) {
+    __syncthreads();
+    JState in = entry;
+    if (live && tid > 0) in = JState{x_pos[tid - 1], x_off[tid - 1], x_j[tid - 1], x_uk[tid - 1] & 0xFF, x_uk[tid - 1] >> 8};
+    const bool redo = live && (in.pos != entry.pos || in.u != entry.u || in.k != entry.k);
+    __syncthreads();
+    if (redo) {
+      entry = in;
+      JState s = in;
+      jd_walk(cx, s, stop, rec);
+      x_pos[tid] = s.pos;
+      x_off[tid] = s.off;
+      x_j[tid] = s.j;
+      x_uk[tid] = s.u | s.k << 8;
+    }
+    if (!__syncthreads_or(redo)) break;
+  }
+  // 4. counts
+  const JAgg at = jagg_exclusive_scan(rec, tot);
+  // 5. write pass
+  if (live) {
+    int pred[3] = {(int)at.v[1], (int)at.v[2], (int)at.v[3]};
+    if (jd_write(cx, entry, stop, (long long)at.v[0], pred, g, coef, vrow, hcol)) err_s = 1;
+  }
+  __syncthreads();
+  if (tid == 0) status[b] = err_s ? JS_DATA : 0;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -761,8 +1146,8 @@ int ctl_jpeg_decode(const void* src, int64_t src_bytes, const void* entries_devi
   // the later launches loop over an image's blocks / pixels; sized for the mean image the buffers were planned for
   const long long mean_blocks = (long long)((workspace_bytes - jpeg_header_bytes(n)) / (64 * 3)) / n;
   const long long mean_pixels = out_bytes / 3 / n;
-  CTL_CUDA(launch_k(jpeg_entropy_kernel, dim3((unsigned)n), dim3(32), 0, st, s, (long long)src_bytes, entries, table,
-                    (long long)out_bytes, ws, (long long)workspace_bytes, (long long)n, stat));
+  CTL_CUDA(launch_k(jpeg_entropy_kernel, dim3((unsigned)n), dim3(JD_ENTROPY_THREADS), 0, st, s, (long long)src_bytes,
+                    entries, table, (long long)out_bytes, ws, (long long)workspace_bytes, (long long)n, stat));
   CTL_CUDA(launch_k(jpeg_idct_kernel, dim3((unsigned)n, jd_grid_y(mean_blocks, JD_IDCT_THREADS / 8)),
                     dim3(JD_IDCT_THREADS), 0, st, s, entries, ws, (const int*)stat));
   CTL_CUDA(launch_k(jpeg_color_kernel, dim3((unsigned)n, jd_grid_y(mean_pixels, JD_COLOR_THREADS)),

@@ -767,9 +767,10 @@ typedef struct ctl_jpeg_entry {
  * entry).  Such an entry's output is zeros (status 4: untouched); the others are unaffected, and nothing outside the
  * buffers is read or written.  workspace: planned by ctl_jpeg_decode_workspace_bytes (host-only, from the host copy
  * of the entries; 0 for null or n < 1): an offset per entry, then per JPEG its int16 coefficients and uint8
- * component planes (3 bytes per coefficient).  Three launches (entropy decode, one thread per image; IDCT; upsample +
- * colour convert); no host synchronisation, no allocation: capturable in a CUDA graph.  A null pointer, n < 1, a
- * negative buffer size or a workspace shorter than its header is CTL_ERR_INVALID_ARGUMENT before any device work. */
+ * component planes (3 bytes per coefficient).  Three launches (entropy decode, one CTA per image decoding up to 256
+ * subsequences of its entropy-coded data in parallel; IDCT; upsample + colour convert); no host synchronisation, no
+ * allocation: capturable in a CUDA graph.  A null pointer, n < 1, a negative buffer size or a workspace shorter than
+ * its header is CTL_ERR_INVALID_ARGUMENT before any device work. */
 int ctl_jpeg_parse(const void* bytes, int64_t nbytes, ctl_jpeg_desc* desc, int32_t* h, int32_t* w);
 size_t ctl_jpeg_decode_workspace_bytes(const ctl_jpeg_entry* entries_host, int64_t n);
 int ctl_jpeg_decode(const void* src, int64_t src_bytes, const void* entries_device, int64_t n,

@@ -5,7 +5,11 @@ eval pipeline.  Sources are seeded smooth colour fields (photograph-like spectra
            ragged batch of seeded sizes between 60x30 and 400x200, and ~500 px sources (seeded sizes between 400x250
            and 600x350); windows of --replays replays alternated with the ResNet50 eval step (TrunkEngine.forward_u8,
            graph) at the shape the decoded batch is resized to (256x128), so the decode's share of the step is read off
-           the same windows.
+           the same windows.  With --parent-lib, the same decode by another build of libctl_b200.so (the C ABI is
+           the same) runs in the same alternation, so two builds are compared in one process.
+  profile: with --profile DIR (a run of its own: tracing slows the host), torch.profiler's per-kernel device time of
+           the decode's three launches for each case (and for --parent-lib's), averaged over --replays calls; the
+           trace is written under DIR.
   e2e    : eval end to end from pinned HOST buffers, double-buffered (H2D of step i + 1 on a copy stream overlaps step
            i; embeddings copied back on a third stream): pinned 128x64 JPEG bytes -> H2D -> decode -> resize ->
            forward_u8 -> D2H, in windows alternated with the same pipeline from pinned native-size decoded 128x64
@@ -15,7 +19,7 @@ eval pipeline.  Sources are seeded smooth colour fields (photograph-like spectra
 Every line is JSON with the card's name and power limit and the mean JPEG bytes per image; times are medians of
 --windows windows with their range.
 
-    python tools/bench_jpeg.py [--windows 7] [--replays 50] [--steps 20]
+    python tools/bench_jpeg.py [--windows 7] [--replays 50] [--steps 20] [--parent-lib PATH] [--profile DIR]
 """
 import argparse
 import io
@@ -67,14 +71,25 @@ def files(case, seed):
 
 
 class GraphedDecode:
-    """decode of one device JpegBatch into static buffers, replayed from a CUDA graph; the status is checked once."""
+    """decode of one device JpegBatch into static buffers, replayed from a CUDA graph; the status is checked once.
+    `fn`: the ctl_jpeg_decode of another library build (default: the tree's)."""
 
-    def __init__(self, batch):
+    def __init__(self, batch, fn=None):
         self.batch = batch
         self.out = torch.empty(max(batch.out_bytes, 1), dtype=torch.uint8, device="cuda")
         self.status = torch.zeros(len(batch), dtype=torch.int32, device="cuda")
         self.ws = torch.empty(batch.workspace_bytes, dtype=torch.uint8, device="cuda")
-        self.call = GraphedCall(lambda: T._decode_enqueue(self.batch, self.out, self.status, self.ws), "cuda")
+        self.fn = fn
+        self.call = GraphedCall(self.enqueue, "cuda")
+
+    def enqueue(self):
+        if self.fn is None:
+            return T._decode_enqueue(self.batch, self.out, self.status, self.ws)
+        b = self.batch
+        rc = self.fn(b.data.data_ptr(), b.data.numel(), b.entries.data_ptr(), len(b), b.out_table.data_ptr(),
+                     self.out.data_ptr(), b.out_bytes, self.status.data_ptr(), self.ws.data_ptr(), self.ws.numel(),
+                     torch.cuda.current_stream().cuda_stream)
+        assert rc == 0, rc
 
     def __call__(self):
         self.call()
@@ -84,14 +99,31 @@ class GraphedDecode:
         assert not self.status.any(), "decode status set"
 
 
+CASES = ("market_128x64", "duke_ragged", "about_500px")
+
+
+def parent_decoder(a):
+    if not a.parent_lib:
+        return None
+    from tools.make_jpeg_corrupt_golden import library
+
+    return library(a.parent_lib)
+
+
 def bench_decode(a, eng, name, power):
-    for case in ("market_128x64", "duke_ragged", "about_500px"):
+    parent = parent_decoder(a)
+    for case in CASES:
         fs = files(case, 1)
         batch = T.pack_jpegs(fs).to("cuda")
         dec = GraphedDecode(batch)
         ref = T.decode_batch(batch)
         dec()
         assert torch.equal(dec.out, ref.data)
+        old = None
+        if parent is not None:
+            old = GraphedDecode(batch, parent)
+            old()
+            assert torch.equal(old.out, ref.data), "the two builds decode differently"
         data, table = ref.data.cpu().numpy(), ref.table.cpu().numpy()
         for i in range(0, B, 51):  # spot check against Pillow
             o, h, w = table[i]
@@ -99,14 +131,22 @@ def bench_decode(a, eng, name, power):
             assert np.array_equal(data[o: o + h * w * 3].reshape(h, w, 3), pil)
         crops = T.resize_batch(ref, SIZE)
         step = GraphedCall(lambda: eng.forward_u8(crops, want_emb=True), "cuda")
-        t_dec, t_step = [], []
+        t_dec, t_step, t_old = [], [], []
         for _ in range(a.windows):
             t_dec.append(window_ms(dec, a.replays))
             t_step.append(window_ms(step, max(a.replays // 10, 3)))
+            if old is not None:
+                t_old.append(window_ms(old, max(a.replays // 10, 3)))
         dec.check()
         ms, rng = med(t_dec)
         sms, srng = med(t_step)
-        print(json.dumps({"bench": "decode", "case": case, "B": B, "decode_ms": ms, "decode_ms_range": rng,
+        extra = {}
+        if old is not None:
+            old.check()
+            oms, orng = med(t_old)
+            extra = {"parent_decode_ms": oms, "parent_decode_ms_range": orng, "speedup": round(oms / ms, 2),
+                     "parent_decode_over_step": round(oms / sms, 4)}
+        print(json.dumps({"bench": "decode", "case": case, "B": B, "decode_ms": ms, "decode_ms_range": rng, **extra,
                           "decoded_pixels": int(ref.rows and (table[:, 1] * table[:, 2]).sum()),
                           "mean_jpeg_bytes": round(float(np.mean([len(f) for f in fs])), 1),
                           "eval_step_ms_forward_u8_256x128": sms, "eval_step_ms_range": srng,
@@ -218,15 +258,50 @@ def bench_host(a, name, power):
                           "power_limit": power}), flush=True)
 
 
+def profile_decode(a, name, power):
+    """per-kernel device time of the decode's launches, from torch.profiler, for each case and build"""
+    from torch.profiler import ProfilerActivity, profile
+
+    parent = parent_decoder(a)
+    os.makedirs(a.profile, exist_ok=True)
+    for case in CASES:
+        batch = T.pack_jpegs(files(case, 1)).to("cuda")
+        for build, fn in (("this", None), ("parent", parent)):
+            if build == "parent" and fn is None:
+                continue
+            dec = GraphedDecode(batch, fn)
+            n = a.replays if build == "this" else max(a.replays // 10, 3)
+            for _ in range(3):
+                dec.enqueue()
+            torch.cuda.synchronize()
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                for _ in range(n):
+                    dec.enqueue()
+                torch.cuda.synchronize()
+            prof.export_chrome_trace(os.path.join(a.profile, f"jpeg_{case}_{build}.pt.trace.json"))
+            per = {}
+            for ev in prof.key_averages():
+                if "jpeg" in ev.key:
+                    t = getattr(ev, "device_time_total", None) or getattr(ev, "cuda_time_total", 0)
+                    per[ev.key.split("(")[0].split("::")[-1]] = round(t / n / 1e3, 4)
+            print(json.dumps({"bench": "decode_profile", "case": case, "build": build, "B": B, "calls": n,
+                              "ms_per_call": per, "card": name, "power_limit": power}), flush=True)
+
+
 def main():
     p = argparse.ArgumentParser()
     p.add_argument("--windows", type=int, default=7)
     p.add_argument("--replays", type=int, default=50)
     p.add_argument("--steps", type=int, default=20)
+    p.add_argument("--parent-lib", default=None, help="another build of libctl_b200.so to time beside this one")
+    p.add_argument("--profile", default=None, help="directory for a torch.profiler run of the decode (only that)")
     a = p.parse_args()
     if not torch.cuda.is_available():
         sys.exit("bench_jpeg.py needs a CUDA device")
     name, power = card()
+    if a.profile:
+        profile_decode(a, name, power)
+        return
     eng = engine()
     bench_decode(a, eng, name, power)
     bench_e2e(a, eng, name, power)
