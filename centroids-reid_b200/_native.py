@@ -18,7 +18,6 @@ CTL_DIST_EUCLIDEAN = 0
 CTL_DIST_COSINE = 1
 CTL_FLAG_NORMALIZE = 2
 CTL_DIST_SQRT = 4
-CTL_FLAG_EXACT_PASS = 8
 CTL_BLOCK_BOTTLENECK = 0
 CTL_BLOCK_BASIC = 1
 
@@ -103,12 +102,7 @@ SIGNATURES = {
     "ctl_planes_bytes": (_sz, [_i64, _i32]),
     "ctl_planes_build": (C.c_int, [_p, _i64, _i32, _i32, _p, _p]),
     "ctl_dist_matrix": (C.c_int, [_p, _i64, _p, _i64, _i32, _i32, _p, _i64, _p]),
-    "ctl_topk_workspace_bytes": (_sz, [_i64, _i64, _i32]),
-    "ctl_l2_topk": (C.c_int, [_p, _i64, _p, _i64, _i32, _i32, _i32, _i64, _p, _p, _p, _p, _sz, _p]),
-    "ctl_eval_collect": (C.c_int, [_p, _i64, _p, _i64, _i32, _i32, _p, _p, _p, _p, _i64, _i32, _p, _p, _p, _p]),
     "ctl_sort_key_rows": (C.c_int, [_p, _p, _i64, _i32, _p]),
-    "ctl_eval_count": (C.c_int, [_p, _i64, _p, _i64, _i32, _i32, _p, _p, _p, _p, _i64, _i32, _p, _p, _p, _p]),
-    "ctl_eval_finalize": (C.c_int, [_p, _p, _i64, _i32, _p, _p, _p]),
     "ctl_eval_finalize_packed": (C.c_int, [_p, _p, _i64, _i32, _p, _p, _p, _p, _p]),
     "ctl_dist_pass": (C.c_int, [_p, _i64, _p, _i64, _i32, _i32, C.POINTER(PassDesc), _p]),
     "ctl_topk_plan": (C.c_int, [_i64, _i32, C.POINTER(_i32), C.POINTER(_i32), C.POINTER(_i32), C.POINTER(_i32)]),

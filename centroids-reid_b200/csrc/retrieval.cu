@@ -970,7 +970,6 @@ struct TopkPlan {
   bool emit_all;
   int n_groups;   // GROUP_W-wide groups
   int merge;      // groups merged per selection slot
-  int n_merged_pow2;
   int cap;        // candidate capacity per query
 };
 static constexpr int EMIT_ALL_MAX = 4096;
@@ -982,7 +981,6 @@ static int plan_topk(int64_t ng, int k, TopkPlan* pl) {
   if (ng <= EMIT_ALL_MAX) {
     pl->emit_all = true;
     pl->merge = 1;
-    pl->n_merged_pow2 = 0;
     pl->cap = next_pow2((int)ng);
     return 0;
   }
@@ -993,7 +991,6 @@ static int plan_topk(int64_t ng, int k, TopkPlan* pl) {
     set_error("k=%d needs at least k column groups (have %d); use ctl_dist_matrix for k this large", k, n_merged);
     return CTL_ERR_UNSUPPORTED;
   }
-  pl->n_merged_pow2 = next_pow2(n_merged);
   long long cap = (long long)pl->merge * GROUP_W * (k - 1) + 512;  // strict bound + room for ties at tau
   cap = next_pow2((int)std::min<long long>(cap, (long long)ng));
   if (cap > CAP_MAX) {
@@ -1035,140 +1032,11 @@ int ctl_dist_matrix(const void* q_planes, int64_t nq, const void* g_planes, int6
   return launch_gemm_pass(q_planes, nq, g_planes, ng, d, flags, p, (cudaStream_t)stream);
 }
 
-size_t ctl_topk_workspace_bytes(int64_t nq, int64_t ng, int32_t k) {
-  TopkPlan pl;
-  if (plan_topk(ng, k, &pl)) return 0;
-  Workspace ws(nullptr, 0);
-  ws.take<float>((size_t)nq * pl.n_groups);
-  ws.take<float>((size_t)nq);
-  ws.take<unsigned long long>((size_t)nq * pl.cap);
-  ws.take<int>((size_t)nq);
-  ws.take<int>(worklist_ints(nq, ng));
-  return ws.off;
-}
-
-int ctl_l2_topk(const void* q_planes, int64_t nq, const void* g_planes, int64_t ng, int32_t d, int32_t flags, int32_t k,
-                int64_t g_index_offset, int64_t* out_idx, float* out_dist, int32_t* overflow, void* workspace,
-                size_t workspace_bytes, ctl_stream_t stream_) {
-  cudaStream_t stream = (cudaStream_t)stream_;
-  CTL_CHECK_ARG(out_idx && out_dist && workspace && overflow, "null pointer");
-  CTL_CHECK_ARG(k >= 1 && k <= ng, "k=%d must be in [1, ng=%lld]", k, (long long)ng);
-  CTL_CHECK_ARG(g_index_offset >= 0 && g_index_offset + ng < (1ll << 32), "gallery index out of uint32 range");
-  TopkPlan pl;
-  int rc = plan_topk(ng, k, &pl);
-  if (rc) return rc;
-  Workspace ws(workspace, workspace_bytes);
-  float* gmin = ws.take<float>((size_t)nq * pl.n_groups);
-  float* tau = ws.take<float>((size_t)nq);
-  unsigned long long* cand = ws.take<unsigned long long>((size_t)nq * pl.cap);
-  int* cand_count = ws.take<int>((size_t)nq);
-  int* work = ws.take<int>(worklist_ints(nq, ng));
-  if (!gmin || !tau || !cand || !cand_count || !work) {
-    set_error("workspace too small: need %zu bytes, have %zu", ws.off, workspace_bytes);
-    return CTL_ERR_WORKSPACE;
-  }
-  CTL_CUDA(cudaMemsetAsync(cand_count, 0, (size_t)nq * sizeof(int), stream));
-  CTL_CUDA(cudaMemsetAsync(overflow, 0, sizeof(int), stream));
-  if (pl.emit_all) {
-    // small gallery: every row is a candidate (tau = +inf), one GEMM pass
-    fill_f32_kernel<<<(unsigned)((nq + 255) / 256), 256, 0, stream>>>(tau, nq, INFINITY);
-    CTL_LAUNCH_CHECK();
-  } else {
-    // pass A: minima of 16-column groups -> tau = k-th smallest group minimum, an upper bound of the k-th smallest
-    // distance.  ANY subset of the groups gives such a bound, so pass A only runs every `stride`-th gallery tile (about
-    // 2.5 k groups: the bound gets looser, the candidate lists longer -- still exact); the other groups read +inf.
-    const int n_tiles = (int)((ng + BN - 1) / BN), m_tiles = (int)((nq + BM - 1) / BM);
-    int stride = (flags & CTL_FLAG_EXACT_PASS) ? 1 : subset_stride(n_tiles, pl.merge, k);
-    if ((long long)m_tiles * n_tiles > WORK_MAX_TILES || m_tiles + n_tiles > WL_MAX_ROW_TILES) stride = 1;
-    GemmPass a = {};
-    a.gmin = gmin;
-    a.n_groups = pl.n_groups;
-    if (stride > 1) {
-      fill_f32_kernel<<<(unsigned)(((size_t)nq * pl.n_groups + 255) / 256), 256, 0, stream>>>(gmin, (int64_t)nq * pl.n_groups, INFINITY);
-      CTL_LAUNCH_CHECK();
-      if ((rc = launch_worklist(nullptr, nq, nullptr, ng, stride, work, stream))) return rc;
-      a.work = work;
-    }
-    if ((rc = launch_gemm_pass(q_planes, nq, g_planes, ng, d, flags, a, stream))) return rc;
-    select_tau_kernel<<<(unsigned)nq, 256, pl.n_merged_pow2 * sizeof(uint32_t), stream>>>(gmin, pl.n_groups, pl.merge, k,
-                                                                                         pl.n_merged_pow2, tau);
-    CTL_LAUNCH_CHECK();
-  }
-  // pass B: rows with distance <= tau become (distance, index) keys
-  GemmPass b = {};
-  b.tau = tau;
-  b.cand_keys = cand;
-  b.cand_count = cand_count;
-  b.cand_cap = pl.cap;
-  b.g_off = g_index_offset;
-  b.overflow = overflow;
-  if ((rc = launch_gemm_pass(q_planes, nq, g_planes, ng, d, flags, b, stream))) return rc;
-  if ((rc = sort_rows(cand, cand_count, nq, pl.cap, stream))) return rc;
-  const int64_t total = nq * k;
-  topk_emit_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(cand, cand_count, pl.cap, k, nq,
-                                                                     (long long*)out_idx, out_dist, overflow);
-  CTL_LAUNCH_CHECK();
-  return 0;
-}
-
 int ctl_sort_key_rows(uint64_t* keys, const int32_t* counts, int64_t rows, int32_t row_stride, ctl_stream_t stream) {
   CTL_CHECK_ARG(keys && counts && rows > 0 && row_stride > 0, "bad arguments");
   int rc = ctl_device_check();
   if (rc) return rc;
   return sort_rows(reinterpret_cast<unsigned long long*>(keys), counts, rows, row_stride, (cudaStream_t)stream);
-}
-
-static int check_ids(const int32_t* q_pid, const int32_t* q_cam, const int32_t* g_pid, const uint64_t* g_cammask,
-                     int64_t ng, int64_t g_index_offset, int32_t max_pos) {
-  CTL_CHECK_ARG(q_pid && q_cam && g_pid && g_cammask, "null identity arrays");
-  CTL_CHECK_ARG(max_pos >= 1, "max_pos must be >= 1");
-  CTL_CHECK_ARG(g_index_offset >= 0 && g_index_offset + ng < (1ll << 32), "gallery index out of uint32 range");
-  return 0;
-}
-
-int ctl_eval_collect(const void* q_planes, int64_t nq, const void* g_planes, int64_t ng, int32_t d, int32_t flags,
-                     const int32_t* q_pid, const int32_t* q_cam, const int32_t* g_pid, const uint64_t* g_cammask,
-                     int64_t g_index_offset, int32_t max_pos, uint64_t* pos_keys, int32_t* pos_count,
-                     int32_t* overflow, ctl_stream_t stream) {
-  int rc = check_ids(q_pid, q_cam, g_pid, g_cammask, ng, g_index_offset, max_pos);
-  if (rc) return rc;
-  CTL_CHECK_ARG(pos_keys && pos_count && overflow, "null output");
-  GemmPass p = {};
-  p.q_pid = q_pid;
-  p.q_cam = q_cam;
-  p.g_pid = g_pid;
-  p.g_mask = reinterpret_cast<const unsigned long long*>(g_cammask);
-  p.pos_keys = reinterpret_cast<unsigned long long*>(pos_keys);
-  p.pos_count = pos_count;
-  p.max_pos = max_pos;
-  p.g_off = g_index_offset;
-  p.overflow = overflow;
-  return launch_gemm_pass(q_planes, nq, g_planes, ng, d, flags, p, (cudaStream_t)stream);
-}
-
-int ctl_eval_count(const void* q_planes, int64_t nq, const void* g_planes, int64_t ng, int32_t d, int32_t flags,
-                   const int32_t* q_pid, const int32_t* q_cam, const int32_t* g_pid, const uint64_t* g_cammask,
-                   int64_t g_index_offset, int32_t max_pos, const uint64_t* pos_keys_sorted, const int32_t* pos_count,
-                   int32_t* buckets, ctl_stream_t stream) {
-  int rc = check_ids(q_pid, q_cam, g_pid, g_cammask, ng, g_index_offset, max_pos);
-  if (rc) return rc;
-  CTL_CHECK_ARG(pos_keys_sorted && pos_count && buckets, "null pointer");
-  GemmPass p = {};
-  p.q_pid = q_pid;
-  p.q_cam = q_cam;
-  p.g_pid = g_pid;
-  p.g_mask = reinterpret_cast<const unsigned long long*>(g_cammask);
-  p.thr_keys = reinterpret_cast<const unsigned long long*>(pos_keys_sorted);
-  p.thr_count = pos_count;
-  p.buckets = buckets;
-  p.max_pos = max_pos;
-  p.g_off = g_index_offset;
-  return launch_gemm_pass(q_planes, nq, g_planes, ng, d, flags, p, (cudaStream_t)stream);
-}
-
-int ctl_eval_finalize(const int32_t* buckets, const int32_t* pos_count, int64_t nq, int32_t max_pos, int32_t* ranks,
-                      double* ap, ctl_stream_t stream) {
-  return ctl_eval_finalize_packed(buckets, pos_count, nq, max_pos, ranks, ap, nullptr, nullptr, stream);
 }
 
 int ctl_eval_finalize_packed(const int32_t* buckets, const int32_t* pos_count, int64_t nq, int32_t max_pos, int32_t* ranks,

@@ -120,27 +120,17 @@ def dist_matrix(x: torch.Tensor, y: torch.Tensor, dist: str = "euclidean", norma
 
 
 def topk(qp: Planes, gp: Planes, k: int, g_index_offset: int = 0, exact_threshold_pass: bool = False):
-    """k nearest gallery rows per query in ascending (distance, index) order.
+    """k nearest gallery rows per query in ascending (distance, index) order: the top-k-only passes of _streamed_enqueue,
+    enqueued without a read-back.  Results report gallery row + g_index_offset.
     Returns (idx int64 [nq, k], dist float32 [nq, k], overflow flag) on the device.  The threshold pass runs every s-th
     gallery tile only (any subset of the gallery bounds the k-th distance from above; ctl_dist_subset_stride) unless
     `exact_threshold_pass`: identical results, the subset only trades longer candidate lists for ~2/3 of that pass."""
     if qp.order is not None or gp.order is not None:
         raise ValueError("topk() takes planes in the caller's row order (use topk_and_eval for pid-sorted planes)")
-    L = N.lib()
-    k = int(min(k, gp.n))
-    dev = qp.buf.device
-    idx = torch.empty(qp.n, k, dtype=torch.int64, device=dev)
-    dst = torch.empty(qp.n, k, dtype=torch.float32, device=dev)
-    ovf = torch.zeros(1, dtype=torch.int32, device=dev)
-    ws_bytes = L.ctl_topk_workspace_bytes(qp.n, gp.n, k)
-    if ws_bytes == 0:
-        N.check(-3)
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        flags = qp.flags | (N.CTL_FLAG_EXACT_PASS if exact_threshold_pass else 0)
-        N.check(L.ctl_l2_topk(qp.ptr, qp.n, gp.ptr, gp.n, qp.d, flags, k, g_index_offset, idx.data_ptr(),
-                              dst.data_ptr(), ovf.data_ptr(), ws.data_ptr(), ws_bytes, N.stream_ptr()))
-    return idx, dst, ovf
+    with torch.cuda.device(qp.buf.device):
+        out = _streamed_enqueue(ShardExchange(None), qp, gp, None, int(min(k, gp.n)), not exact_threshold_pass,
+                                g_index_offset)
+    return out["rows"] + (out["ovf"],)
 
 
 def topk_dense(q: torch.Tensor, g: torch.Tensor, k: int, dist: str = "euclidean", normalize: bool = False,
@@ -179,7 +169,7 @@ def topk_similar(q: torch.Tensor, g: torch.Tensor, k: int = 100, dist: str = "eu
     k = int(min(k, g.shape[0]))
     a, b, c, d_ = C.c_int32(), C.c_int32(), C.c_int32(), C.c_int32()
     rc = N.lib().ctl_topk_plan(g.shape[0], k, C.byref(a), C.byref(b), C.byref(c), C.byref(d_))
-    if rc == 0 and N.lib().ctl_topk_workspace_bytes(q.shape[0], g.shape[0], k) > 0:
+    if rc == 0:
         qp, gp = build_planes(q, dist, normalize), build_planes(g, dist, normalize)
         for exact in (False, True):  # a candidate overflow of the bounded threshold pass: once more with the exact one
             idx, dst, ovf = topk(qp, gp, k, exact_threshold_pass=exact)
@@ -346,15 +336,15 @@ def _tile_lists_enabled(qp: Planes, gp: Planes) -> bool:
     return qp.order is not None and gp.order is not None
 
 
-def _tile_list(qp: Planes, gp: Planes, ids: "EncodedIds", keep_stride: int) -> Optional[torch.Tensor]:
-    """ctl_dist_worklist: the tiles that can hold a positive (+ every keep_stride-th gallery tile for the threshold).
-    None when the problem is beyond the list builder (the pass then runs every tile)."""
+def _tile_list(qp: Planes, gp: Planes, ids: "Optional[EncodedIds]", keep_stride: int) -> Optional[torch.Tensor]:
+    """ctl_dist_worklist: the tiles that can hold a positive (none when `ids` is None) + every keep_stride-th gallery
+    tile for the threshold.  None when the problem is beyond the list builder (the pass then runs every tile)."""
     L = N.lib()
     if ((qp.n + 127) // 128) * ((gp.n + 127) // 128) > (1 << 20) or (qp.n + 127) // 128 + (gp.n + 127) // 128 > 5632:
         return None
     work = torch.empty(L.ctl_dist_worklist_bytes(qp.n, gp.n) // 4, dtype=torch.int32, device=qp.buf.device)
-    N.check(L.ctl_dist_worklist(ids.q_pid.data_ptr(), qp.n, ids.g_pid.data_ptr(), gp.n, int(keep_stride), work.data_ptr(),
-                                N.stream_ptr()))
+    q_pid, g_pid = (None, None) if ids is None else (ids.q_pid, ids.g_pid)
+    N.check(L.ctl_dist_worklist(N.ptr(q_pid), qp.n, N.ptr(g_pid), gp.n, int(keep_stride), work.data_ptr(), N.stream_ptr()))
     return work
 
 
@@ -428,21 +418,6 @@ def _encode_identities_global(q_pids, g_pids, q_camids, g_camids):
     return q_pid, q_cam, g_pid, g_mask, max(1, max_pos)
 
 
-def merge_topk(idx_list: Sequence[torch.Tensor], dist_list: Sequence[torch.Tensor], k: int):
-    """k-way merge of per-shard (ascending) top-k lists under the canonical (distance, index)
-    order -- deterministic regardless of world size.  CUDA inputs are merged by the native packed-key row sort
-    (one launch, integer-exact); host tensors (the gloo tests) by two stable argsorts."""
-    idx = torch.cat(list(idx_list), 1)
-    dst = torch.cat(list(dist_list), 1)
-    if idx.is_cuda:
-        return merge_topk_keys(pack_keys(dst, idx), k)
-    # sort by index first (stable), then by distance (stable): lexicographic (distance, index)
-    o1 = torch.argsort(idx, dim=1, stable=True)
-    idx, dst = idx.gather(1, o1), dst.gather(1, o1)
-    o2 = torch.argsort(dst, dim=1, stable=True)
-    return idx.gather(1, o2)[:, :k], dst.gather(1, o2)[:, :k]
-
-
 def pack_keys(dst: torch.Tensor, idx: torch.Tensor) -> torch.Tensor:
     """(distance fp32, index) -> the kernels' uint64 key (carried as int64): orderable(fp32) << 32 | index, whose
     UNSIGNED integer order is the canonical ascending (distance, index) order (ctl_key_encode)."""
@@ -471,24 +446,14 @@ def merge_topk_keys(keys: torch.Tensor, k: int):
 
 def topk_sharded(q_local: torch.Tensor, g_local: torch.Tensor, k: int, g_index_offset: int, group,
                  dist: str = "euclidean", normalize: bool = False):
-    """BASELINE config 5: queries sharded by rank are all-gathered once (NCCL), the gallery
-    stays sharded; every rank returns the merged global top-k of ALL queries."""
-    import torch.distributed as tdist
-
-    world = tdist.get_world_size(group)
-    q_all = [torch.empty_like(q_local) for _ in range(world)]
-    tdist.all_gather(q_all, q_local.contiguous(), group=group)
-    q = torch.cat(q_all, 0)
+    """BASELINE config 5: queries sharded by rank (the same number on every rank) are all-gathered once, the gallery
+    stays sharded; every rank returns the merged global top-k of ALL queries -- the top-k-only passes of
+    _streamed_enqueue, whose exchange merges every rank's k best keys.  `group=None` is torch.distributed's default
+    group."""
+    ex = ShardExchange.default() if group is None else ShardExchange(group)
+    q = ex.rows(q_local, [q_local.shape[0]] * ex.world)
     qp, gp = build_planes(q, dist, normalize), build_planes(g_local, dist, normalize)
-    idx, dst, ovf = topk(qp, gp, k, g_index_offset)
-    idx_all = [torch.empty_like(idx) for _ in range(world)]
-    dst_all = [torch.empty_like(dst) for _ in range(world)]
-    tdist.all_gather(idx_all, idx, group=group)
-    tdist.all_gather(dst_all, dst, group=group)
-    tdist.all_reduce(ovf, group=group)
-    if int(ovf.item()) != 0:
-        raise OverflowError("top-k candidate capacity exceeded on some rank")
-    return merge_topk(idx_all, dst_all, k)
+    return _streamed(ex, qp, gp, None, k, None, gp.n, 0, g_index_offset, tile_lists=True)
 
 
 def topk_and_eval(qp: Planes, gp: Planes, k: int, q_pids, g_pids, q_camids, g_camids, max_rank: int = 50,
@@ -513,9 +478,10 @@ def topk_and_eval(qp: Planes, gp: Planes, k: int, q_pids, g_pids, q_camids, g_ca
 
 
 class ShardExchange:
-    """The exchanges of the sharded paths (the streamed passes of evaluate_streamed / topk_and_eval_sharded and the
-    row-blocked re-ranking), over the ranks of a torch.distributed group (None: one rank, nothing is exchanged).  Every
-    rank calls each method in the same order.  Tests substitute stand-ins with the same methods."""
+    """The exchanges of the sharded paths (the streamed passes of topk_sharded / evaluate_streamed /
+    topk_and_eval_sharded and the row-blocked re-ranking), over the ranks of a torch.distributed group (None: one rank,
+    nothing is exchanged).  Every rank calls each method in the same order.  Tests substitute stand-ins with the same
+    methods."""
 
     def __init__(self, group=None):
         import torch.distributed as dist
@@ -523,6 +489,15 @@ class ShardExchange:
         self.dist, self.group = dist, group
         self.world = 1 if group is None else dist.get_world_size(group)
         self.rank = 0 if group is None else dist.get_rank(group)
+
+    @classmethod
+    def default(cls) -> "ShardExchange":
+        """The ranks of torch.distributed's default group (the meaning torch.distributed gives `group=None`)."""
+        import torch.distributed as dist
+
+        if not dist.is_initialized():
+            raise ValueError("torch.distributed's default process group has not been initialized")
+        return cls(dist.group.WORLD)
 
     def objects(self, obj) -> list:
         """Every rank's picklable `obj`, in rank order."""
@@ -578,7 +553,7 @@ def _gather_keys(ex, pos_keys: torch.Tensor, pos_count: torch.Tensor):
     return keys, count
 
 
-def _streamed_enqueue(ex, qp: Planes, gp: Planes, ids: "EncodedIds", k: Optional[int], tile_lists: bool,
+def _streamed_enqueue(ex, qp: Planes, gp: Planes, ids: "Optional[EncodedIds]", k: Optional[int], tile_lists: bool,
                       g_index_offset: int = 0) -> dict:
     """The launch sequence of the streamed passes over this rank's gallery `gp` (the whole gallery at world 1), with the
     exchanges of `ex` (ShardExchange or a stand-in) between them:
@@ -588,16 +563,19 @@ def _streamed_enqueue(ex, qp: Planes, gp: Planes, ids: "EncodedIds", k: Optional
       exchange 2 (world > 1): sum of the bucket counts, MAX of the overflow flag, every rank's k best keys merged by
                               integer key order; at world 1 the top-k is emitted from the candidates
       finalize
-    k=None evaluates only: no minima, threshold or candidates.  `tile_lists`: pass 1 runs a tile list (topk_and_eval).
+    k=None evaluates only: no minima, threshold or candidates.  ids=None is the top-k only: no positives, counts or
+    finalize, and no pass 1 for a small gallery (tau = +inf).  `tile_lists`: pass 1 runs a tile list (topk_and_eval; with
+    ids=None the list of every s-th gallery tile, ctl_dist_subset_stride, for a threshold from a subset of the gallery).
     At world 1 nothing is exchanged and nothing waits for the host (capturable in a CUDA graph).  Returns the device
-    tensors {rows: (idx, dst) or (), ranks, pack} in the planes' query order."""
+    tensors {rows: (idx, dst) or (), ovf, ranks, pack} in the planes' query order; no ranks or pack with ids=None."""
     import ctypes as C
 
     L = N.lib()
     dev = qp.buf.device
     nq, ng, world = qp.n, gp.n, ex.world
-    mp_l = ids.max_pos  # capacity of one rank's positives (the same on every rank)
-    mp = mp_l * world   # capacity of the merged threshold list
+    if ids is not None:
+        mp_l = ids.max_pos  # capacity of one rank's positives (the same on every rank)
+        mp = mp_l * world   # capacity of the merged threshold list
     i32 = dict(dtype=torch.int32, device=dev)
     s = N.stream_ptr
     keep = []
@@ -616,39 +594,47 @@ def _streamed_enqueue(ex, qp: Planes, gp: Planes, ids: "EncodedIds", k: Optional
         cand = torch.empty(nq, cap, dtype=torch.int64, device=dev)
         zeros = torch.zeros(2 * nq + 1, **i32)
         cand_count, pos_count, ovf = zeros[:nq], zeros[nq: 2 * nq], zeros[2 * nq:]
-        pos_keys = torch.empty(nq, mp_l, dtype=torch.int64, device=dev)
-        buckets = torch.zeros(nq, mp + 1, **i32)
         keep += [gmin, tau, cand, zeros]
+        if ids is not None:
+            pos_keys = torch.empty(nq, mp_l, dtype=torch.int64, device=dev)
+            buckets = torch.zeros(nq, mp + 1, **i32)
     gmap = _g_index_map(gp, g_index_offset)  # keys carry the caller's gallery row (sharded: the GLOBAL row)
-    idp = dict(q_pid=ids.q_pid.data_ptr(), q_cam=ids.q_cam.data_ptr(), g_pid=ids.g_pid.data_ptr(),
-               g_cammask=ids.g_mask.data_ptr(), overflow=ovf.data_ptr(), g_index_offset=g_index_offset,
-               g_index_map=N.ptr(gmap))
-    p1 = N.PassDesc(pos_keys=pos_keys.data_ptr(), pos_count=pos_count.data_ptr(), max_pos=mp_l, **idp)
+    idp = dict(overflow=ovf.data_ptr(), g_index_offset=g_index_offset, g_index_map=N.ptr(gmap))
+    p1 = N.PassDesc()
+    if ids is not None:
+        idp.update(q_pid=ids.q_pid.data_ptr(), q_cam=ids.q_cam.data_ptr(), g_pid=ids.g_pid.data_ptr(),
+                   g_cammask=ids.g_mask.data_ptr())
+        p1 = N.PassDesc(pos_keys=pos_keys.data_ptr(), pos_count=pos_count.data_ptr(), max_pos=mp_l, **idp)
     if not emit_all:
         p1.gmin = gmin.data_ptr()
     work = None
     if tile_lists:  # (no threshold, or tau = +inf for a small gallery: stride 0, just the tiles that can hold a positive)
         stride = 0 if emit_all else L.ctl_dist_subset_stride(ng, k_loc)
-        if emit_all or stride > 1:
+        if stride > 1 or (emit_all and ids is not None):
             work = _tile_list(qp, gp, ids, stride)
     if work is not None:
         p1.tile_list = work.data_ptr()
         if not emit_all:
             N.check(L.ctl_fill_f32(gmin.data_ptr(), gmin.numel(), float("inf"), s()))  # groups of tiles not run
-    N.check(L.ctl_dist_pass(qp.ptr, nq, gp.ptr, ng, qp.d, qp.flags, C.byref(p1), s()))
+    if ids is not None or not emit_all:
+        N.check(L.ctl_dist_pass(qp.ptr, nq, gp.ptr, ng, qp.d, qp.flags, C.byref(p1), s()))
     if k is not None and emit_all:
         N.check(L.ctl_fill_f32(tau.data_ptr(), nq, float("inf"), s()))
     elif k is not None:
         N.check(L.ctl_select_tau(gmin.data_ptr(), nq, n_groups, merge, k_loc, tau.data_ptr(), s()))
-    thr, thr_count, sort_count = pos_keys, pos_count, pos_count
-    if world > 1:
-        thr, thr_count = _gather_keys(ex, pos_keys, pos_count)
-        sort_count = torch.full((nq,), mp, **i32)
-    N.check(L.ctl_sort_key_rows(thr.data_ptr(), sort_count.data_ptr(), nq, mp, s()))
-    if buckets is None:
-        buckets = torch.zeros(nq, mp + 1, **i32)
-    p2 = N.PassDesc(thr_keys=thr.data_ptr(), thr_count=thr_count.data_ptr(), buckets=buckets.data_ptr(), max_pos=mp,
-                    **idp)
+    if ids is None:
+        p2 = N.PassDesc(**idp)
+    else:
+        thr, thr_count, sort_count = pos_keys, pos_count, pos_count
+        if world > 1:
+            thr, thr_count = _gather_keys(ex, pos_keys, pos_count)
+            sort_count = torch.full((nq,), mp, **i32)
+        N.check(L.ctl_sort_key_rows(thr.data_ptr(), sort_count.data_ptr(), nq, mp, s()))
+        if buckets is None:
+            buckets = torch.zeros(nq, mp + 1, **i32)
+        p2 = N.PassDesc(thr_keys=thr.data_ptr(), thr_count=thr_count.data_ptr(), buckets=buckets.data_ptr(), max_pos=mp,
+                        **idp)
+        keep += [pos_keys, thr, sort_count, buckets]
     if k is not None:
         p2.tau, p2.cand_keys, p2.cand_count, p2.cand_cap = tau.data_ptr(), cand.data_ptr(), cand_count.data_ptr(), cap
     N.check(L.ctl_dist_pass(qp.ptr, nq, gp.ptr, ng, qp.d, qp.flags, C.byref(p2), s()))
@@ -656,7 +642,8 @@ def _streamed_enqueue(ex, qp: Planes, gp: Planes, ids: "EncodedIds", k: Optional
     if k is not None:
         N.check(L.ctl_sort_key_rows(cand.data_ptr(), cand_count.data_ptr(), nq, cap, s()))
     if world > 1:
-        ex.sum_(buckets)
+        if ids is not None:
+            ex.sum_(buckets)
         ex.max_(ovf)
         if k is not None:
             best = ex.rows(cand[:, :k_loc].contiguous(), [nq] * world)
@@ -668,21 +655,28 @@ def _streamed_enqueue(ex, qp: Planes, gp: Planes, ids: "EncodedIds", k: Optional
         N.check(L.ctl_topk_emit(cand.data_ptr(), cand_count.data_ptr(), nq, cap, k_loc, idx.data_ptr(), dst.data_ptr(),
                                 ovf.data_ptr(), s()))
         rows = (idx, dst)
-    ranks, pack = _finalize(buckets, thr_count, nq, mp, ovf)
-    return {"rows": rows, "ranks": ranks, "pack": pack, "keep": keep + [pos_keys, thr, sort_count, buckets, work, gmap]}
+    out = {"rows": rows, "ovf": ovf, "keep": keep + [work, gmap]}
+    if ids is not None:
+        out["ranks"], out["pack"] = _finalize(buckets, thr_count, nq, mp, ovf)
+    return out
 
 
-def _streamed(ex, qp: Planes, gp: Planes, ids: "EncodedIds", k: Optional[int], q_pids, num_g: int, max_rank: int,
-              g_index_offset: int = 0, tile_lists: Optional[bool] = None) -> tuple:
+def _streamed(ex, qp: Planes, gp: Planes, ids: "Optional[EncodedIds]", k: Optional[int], q_pids, num_g: int,
+              max_rank: int, g_index_offset: int = 0, tile_lists: Optional[bool] = None) -> tuple:
     """_streamed_enqueue, ONE read-back and _eval_result: (idx, dist, EvalResult) in the caller's query order, or
-    (EvalResult,) when k is None.  `tile_lists` defaults to both planes being stored in identity order.  When the looser
-    threshold of a tile-list pass 1 lets more rows through than a candidate list holds, the call runs once more with the
-    threshold from every tile; the overflow flag is MAX-reduced and `tile_lists` is the caller's, so every rank retries
-    together."""
+    (EvalResult,) when k is None, or (idx, dist) when ids is None (the top-k only, whose read-back is the overflow flag:
+    OverflowError when it is set).  `tile_lists` defaults to both planes being stored in identity order.  When the looser
+    threshold of a tile-list pass 1 lets more rows through than a candidate list holds, an evaluation runs once more with
+    the threshold from every tile; the overflow flag is MAX-reduced and `tile_lists` is the caller's, so every rank
+    retries together."""
     if tile_lists is None:
         tile_lists = _tile_lists_enabled(qp, gp)
     with torch.cuda.device(qp.buf.device):
         out = _streamed_enqueue(ex, qp, gp, ids, k, tile_lists, g_index_offset)
+        if ids is None:
+            if int(out["ovf"].item()):
+                raise OverflowError("top-k candidate capacity exceeded on some rank")
+            return out["rows"]
         h = out["pack"].cpu().numpy()
         if h[qp.n, 0] and tile_lists and k is not None:
             return _streamed(ex, qp, gp, ids, k, q_pids, num_g, max_rank, g_index_offset, tile_lists=False)

@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define CTL_ABI_VERSION 4
+#define CTL_ABI_VERSION 5
 
 #define CTL_OK 0
 #define CTL_ERR_INVALID_ARGUMENT (-1)
@@ -52,8 +52,6 @@ int ctl_device_check(void);
 #define CTL_DIST_COSINE 1    /* clamp(|1 - cos|, 1e-12) */
 #define CTL_FLAG_NORMALIZE 2 /* torch.nn.functional.normalize(x, dim=1, p=2) first */
 #define CTL_DIST_SQRT 4      /* euclidean only: sqrt(clamp(d, 1e-12)) -- losses/triplet_loss.py:27-41 */
-#define CTL_FLAG_EXACT_PASS 8 /* ctl_l2_topk: threshold pass over EVERY gallery tile (default: a subset of the tiles --
-                                 same results from a looser threshold and longer candidate lists) */
 
 /* Row planes: the fp32 rows split into two fp16 planes (hi + 2^-11 lo, per-row power-of-two
  * scale) plus fp32 squared norms, the operand format of the tensor-core distance kernel.
@@ -65,52 +63,40 @@ int ctl_planes_build(const float* x, int64_t n, int32_t d, int32_t flags, void* 
 int ctl_dist_matrix(const void* q_planes, int64_t nq, const void* g_planes, int64_t ng, int32_t d, int32_t flags,
                     float* out, int64_t ld_out, ctl_stream_t stream);
 
-/* Per-query k smallest distances in ascending (distance, gallery index) order, without
- * materialising the matrix.  out_idx = local gallery row + g_index_offset.  Requires
- * k <= ng.  *overflow (device int, written asynchronously) becomes non-zero if more rows
- * than the candidate capacity tie exactly at the selection threshold; the results are then
- * invalid and the shim raises CTL_ERR_CAPACITY after its result read-back. */
-size_t ctl_topk_workspace_bytes(int64_t nq, int64_t ng, int32_t k);
-int ctl_l2_topk(const void* q_planes, int64_t nq, const void* g_planes, int64_t ng, int32_t d, int32_t flags,
-                int32_t k, int64_t g_index_offset, int64_t* out_idx, float* out_dist, int32_t* overflow,
-                void* workspace, size_t workspace_bytes, ctl_stream_t stream);
-
-/* Streamed evaluation (eval_func semantics).  Identity / camera arrays: q_pid, g_pid int32;
+/* Streamed top-k and evaluation: passes of the distance GEMM (ctl_dist_pass) whose epilogues reduce each tile instead
+ * of storing it, so the [nq, ng] matrix is never materialised.  Keys are uint64 (distance, gallery index) pairs whose
+ * integer order is the ascending (distance, index) order (ctl_key_encode); the index is gallery row + g_index_offset,
+ * or g_index_map[row].
+ *
+ * Top-k: the k <= ng smallest distances per query, in that order, for the plan of ctl_topk_plan:
+ *   pass 1: gmin -> ctl_select_tau: tau = the k-th smallest group minimum, an upper bound of the k-th distance.  Any
+ *           subset of the groups gives such a bound, so pass 1 may run a tile list of every ctl_dist_subset_stride-th
+ *           gallery tile (gmin pre-filled with +inf): a looser tau, longer candidate lists, the same results.  With
+ *           emit_all there is no pass 1 and tau = +inf (ctl_fill_f32);
+ *   pass 2: tau + cand_keys -> ctl_sort_key_rows of the candidates -> ctl_topk_emit.
+ *   The caller zeroes cand_count and *overflow.  *overflow becomes non-zero if more rows than the candidate capacity
+ *   tie exactly at tau; the results are then invalid.
+ *
+ * Evaluation (eval_func semantics).  Identity / camera arrays: q_pid, g_pid int32;
  * q_cam = dense camera index in [0,64); g_cammask = bit set of the cameras a gallery row
  * (or centroid, utils/eval_reid.py:52-56 respect_camids) was built from.  A gallery row is
  * junk for a query iff same pid and bit q_cam of its mask is set; it is a positive iff
  * same pid and not junk.
- *   collect : pos_keys[nq, max_pos] <- (distance, gallery index) keys of each query's
- *             positives (unordered), pos_count[nq] (zeroed by the caller);
- *   sort    : ascending sort of every row of a key matrix (counts[i] valid entries);
+ *   collect : pos_keys[nq, max_pos] <- keys of each query's positives (unordered), pos_count[nq] (zeroed by the
+ *             caller); *overflow is set when a query has more than max_pos;
+ *   sort    : ctl_sort_key_rows of the positives -> the threshold list thr_keys / thr_count;
  *   count   : buckets[nq, max_pos + 1] (zeroed by the caller) += for every kept gallery row,
  *             the index of the first positive that sorts after it;
- *   finalize: ranks[nq, max_pos] (1-based rank of each positive among kept rows),
- *             ap[nq] (float64, eval_reid.py:75-79), -1 / NaN for queries without positives.
- * With a gallery sharded over ranks: collect per shard, all-gather + sort the keys, count
- * per shard, all-reduce(sum) the buckets, finalize. */
-int ctl_eval_collect(const void* q_planes, int64_t nq, const void* g_planes, int64_t ng, int32_t d, int32_t flags,
-                     const int32_t* q_pid, const int32_t* q_cam, const int32_t* g_pid, const uint64_t* g_cammask,
-                     int64_t g_index_offset, int32_t max_pos, uint64_t* pos_keys, int32_t* pos_count,
-                     int32_t* overflow, ctl_stream_t stream);
-int ctl_sort_key_rows(uint64_t* keys, const int32_t* counts, int64_t rows, int32_t row_stride, ctl_stream_t stream);
-int ctl_eval_count(const void* q_planes, int64_t nq, const void* g_planes, int64_t ng, int32_t d, int32_t flags,
-                   const int32_t* q_pid, const int32_t* q_cam, const int32_t* g_pid, const uint64_t* g_cammask,
-                   int64_t g_index_offset, int32_t max_pos, const uint64_t* pos_keys_sorted,
-                   const int32_t* pos_count, int32_t* buckets, ctl_stream_t stream);
-int ctl_eval_finalize(const int32_t* buckets, const int32_t* pos_count, int64_t nq, int32_t max_pos, int32_t* ranks,
-                      double* ap, ctl_stream_t stream);
-/* ctl_eval_finalize that also fills `packed` ([nq + 1][3] doubles: per query AP, first-hit rank (-1: none), number of
- * positives; last row: {*overflow, 0, 0}) -- everything eval_func's final reductions (utils/eval_reid.py:86-92) need, so
- * the host does ONE device->host copy per evaluation. */
-int ctl_eval_finalize_packed(const int32_t* buckets, const int32_t* pos_count, int64_t nq, int32_t max_pos, int32_t* ranks,
-                             double* ap, double* packed, const int32_t* overflow, ctl_stream_t stream);
-/* One generic pass of the distance GEMM with any combination of the streamed epilogues (the
- * entry points above are compositions of this one).  NULL pointers disable a feature.
+ *   finalize: ctl_eval_finalize_packed.
+ * Collect shares pass 1 with the top-k, count shares pass 2.
+ * With a gallery sharded over ranks, each rank's keys carrying global gallery indices: collect per shard, all-gather +
+ * sort the keys, count per shard, all-reduce(sum) the buckets, finalize; for the top-k, all-gather every rank's first k
+ * sorted candidates and sort + emit those rows again. */
+/* One pass of the distance GEMM with any combination of the streamed epilogues.  NULL pointers disable a feature.
  * With both top-k and evaluation wanted, TWO passes serve both:
  *   pass 1: gmin (+ pos_keys/pos_count)            -> ctl_select_tau, ctl_sort_key_rows
  *   pass 2: tau + cand_keys (+ thr_keys + buckets) -> ctl_sort_key_rows, ctl_topk_emit,
- *                                                     ctl_eval_finalize */
+ *                                                     ctl_eval_finalize_packed */
 typedef struct ctl_pass_desc {
   float* dist_out;            /* [nq, ld_out] full matrix */
   int64_t ld_out;
@@ -119,7 +105,7 @@ typedef struct ctl_pass_desc {
   uint64_t* cand_keys;        /* [nq, cand_cap] rows with dist <= tau */
   int32_t* cand_count;        /* [nq], zeroed by the caller */
   int32_t cand_cap;
-  const int32_t* q_pid;       /* identities: see ctl_eval_collect */
+  const int32_t* q_pid;       /* identities: see the evaluation above */
   const int32_t* q_cam;
   const int32_t* g_pid;
   const uint64_t* g_cammask;
@@ -141,6 +127,8 @@ typedef struct ctl_pass_desc {
 } ctl_pass_desc;
 int ctl_dist_pass(const void* q_planes, int64_t nq, const void* g_planes, int64_t ng, int32_t d, int32_t flags,
                   const ctl_pass_desc* desc, ctl_stream_t stream);
+/* ascending sort of every row of a key matrix (counts[i] valid entries; row_stride <= 16384) */
+int ctl_sort_key_rows(uint64_t* keys, const int32_t* counts, int64_t rows, int32_t row_stride, ctl_stream_t stream);
 /* top-k plan for (ng, k): emit_all != 0 means "skip pass 1, tau = +inf". */
 int ctl_topk_plan(int64_t ng, int32_t k, int32_t* emit_all, int32_t* n_groups, int32_t* merge, int32_t* cand_cap);
 int ctl_select_tau(const float* gmin, int64_t nq, int32_t n_groups, int32_t merge, int32_t k, float* tau,
@@ -159,6 +147,12 @@ int ctl_dist_worklist(const int32_t* q_pid, int64_t nq, const int32_t* g_pid, in
 int ctl_fill_f32(float* p, int64_t n, float value, ctl_stream_t stream);
 int ctl_topk_emit(const uint64_t* cand_keys_sorted, const int32_t* cand_count, int64_t nq, int32_t cand_cap, int32_t k,
                   int64_t* out_idx, float* out_dist, int32_t* overflow, ctl_stream_t stream);
+/* finalize: ranks[nq, max_pos] (1-based rank of each positive among kept rows), ap[nq] (float64, eval_reid.py:75-79),
+ * -1 / NaN for queries without positives; and, unless `packed` is NULL, packed[nq + 1][3] doubles: per query AP,
+ * first-hit rank (-1: none), number of positives; last row: {*overflow (0 for a NULL overflow), 0, 0} -- everything
+ * eval_func's final reductions (utils/eval_reid.py:86-92) need, so the host does ONE device->host copy per evaluation. */
+int ctl_eval_finalize_packed(const int32_t* buckets, const int32_t* pos_count, int64_t nq, int32_t max_pos, int32_t* ranks,
+                             double* ap, double* packed, const int32_t* overflow, ctl_stream_t stream);
 /* key <-> (distance, index) helpers for host-side merges of per-shard results */
 uint64_t ctl_key_encode(float dist, uint32_t index);
 void ctl_key_decode(uint64_t key, float* dist, uint32_t* index);
@@ -167,7 +161,7 @@ void ctl_key_decode(uint64_t key, float* dist, uint32_t* index);
  * CMC / mAP over a materialised distance matrix
  * replaces: utils/eval_reid.py:25-92 (eval_func) for a [nq, ld] fp32 matrix the caller computed (re-ranked distances,
  * or any other): np.argsort + the per-query loop.  The collect and count passes of ctl_dist_pass reading the matrix
- * instead of forming it: same identity arrays and junk rule (see ctl_eval_collect), same (distance, column) keys, so
+ * instead of forming it: same identity arrays and junk rule (see ctl_dist_pass), same (distance, column) keys, so
  * ctl_sort_key_rows and ctl_eval_finalize_packed complete them unchanged.  pos_count and buckets are zeroed by the caller.
  * ---------------------------------------------------------------------------------------- */
 int ctl_eval_matrix_collect(const float* dist, int64_t nq, int64_t ng, int64_t ld, const int32_t* q_pid,

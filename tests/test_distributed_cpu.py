@@ -1,5 +1,6 @@
 """CPU, world_size 2, gloo: the host-side logic of the sharded (N > 1) retrieval path --
-per-shard top-k merge under the canonical (distance, index) order, exchange 1 of the streamed
+the top-k merge of the streamed passes (every rank's k best packed keys all-gathered over ShardExchange, one sort of
+the unsigned keys per row gives the canonical (distance, index) order), exchange 1 of the streamed
 passes (retrieval._gather_keys over ShardExchange: every rank's positives' keys, unused slots
 masked), the all-reduce of the integer bucket counts (ShardExchange.sum_) -- with the device
 kernels (and the row sort) emulated in numpy from the oracle's distance matrix."""
@@ -41,17 +42,17 @@ def _worker(rank, world, port, out_q):
     shard = np.array_split(np.arange(ng), world)[rank]
     off = int(shard[0])
     Dl = D[:, shard]
-    # --- top-k: local ascending lists with GLOBAL indices, merged across ranks ---------------
+    ex = R.ShardExchange(dist.group.WORLD)
+    # --- top-k: local ascending lists with GLOBAL indices, their keys all-gathered and sorted ---------------
     order = np.argsort(Dl, axis=1, kind="stable")[:, :k]
-    idx_l = torch.from_numpy(order + off)
-    dst_l = torch.from_numpy(np.take_along_axis(Dl, order, 1))
-    idx_all = [torch.empty_like(idx_l) for _ in range(world)]
-    dst_all = [torch.empty_like(dst_l) for _ in range(world)]
-    dist.all_gather(idx_all, idx_l)
-    dist.all_gather(dst_all, dst_l)
-    midx, mdst = R.merge_topk(idx_all, dst_all, k)
+    keys_l = R.pack_keys(torch.from_numpy(np.take_along_axis(Dl, order, 1)), torch.from_numpy(order + off))
+    best = ex.rows(keys_l, [nq] * world).view(world, nq, k).permute(1, 0, 2).reshape(nq, world * k)
+    merged = np.sort(best.numpy().view(np.uint64), axis=1)[:, :k]  # ctl_sort_key_rows + ctl_topk_emit on the device
+    midx = (merged & np.uint64(0xFFFFFFFF)).astype(np.int64)
+    o = (merged >> np.uint64(32)).astype(np.uint32)
+    mdst = np.where(o & 0x80000000, o ^ 0x80000000, ~o).astype(np.uint32).view(np.float32)
     ref = np.argsort(D, axis=1, kind="stable")[:, :k]
-    ok_topk = np.array_equal(midx.numpy(), ref) and np.array_equal(mdst.numpy(), np.take_along_axis(D, ref, 1))
+    ok_topk = np.array_equal(midx, ref) and np.array_equal(mdst, np.take_along_axis(D, ref, 1))
     # --- eval: collect (emulated) -> all-gather keys -> sort -> count (emulated) -> all-reduce ----
     gp, gc = pids[nq:][shard], cams[nq:][shard]
     same = gp[None, :] == pids[:nq, None]
@@ -63,7 +64,6 @@ def _worker(rank, world, port, out_q):
     allk = _key(Dl, np.broadcast_to(shard[None, :], Dl.shape))
     for q in range(nq):
         keys[q, : cnt[q]] = allk[q][pos[q]]
-    ex = R.ShardExchange(dist.group.WORLD)
     gk, gcnt = R._gather_keys(ex, torch.from_numpy(keys.view(np.int64)), torch.from_numpy(cnt))
     ok_shape = tuple(gk.shape) == (nq, world * max_pos)
     gk = np.sort(gk.numpy().view(np.uint64), axis=1)  # ctl_sort_key_rows over the whole row: unused slots sort last
@@ -93,7 +93,7 @@ def _worker(rank, world, port, out_q):
     dist.destroy_process_group()
 
 
-def test_sharded_merge_and_key_exchange_world2_gloo():
+def test_sharded_key_merge_and_key_exchange_world2_gloo():
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
     port = _free_port()

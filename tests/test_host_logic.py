@@ -14,8 +14,8 @@ from ctl_b200.utils.eval_reid import eval_func
 from oracle import ctl_oracle as O
 
 
-def test_abi_version_and_every_declared_symbol_exported():
-    """The shared library loads, reports ABI version 4 and exports exactly what include/ctl_b200.h declares."""
+def test_abi_version_5_and_every_declared_symbol_exported():
+    """The shared library loads, reports ABI version 5 and exports exactly what include/ctl_b200.h declares."""
     header = open(os.path.join(ROOT, "include", "ctl_b200.h")).read()
     declared = set(re.findall(r"\b(ctl_[a-z0-9_]+)\s*\(", header))
     assert declared, "no declarations parsed"
@@ -23,7 +23,7 @@ def test_abi_version_and_every_declared_symbol_exported():
     missing = [n for n in sorted(declared) if not hasattr(lib, n)]
     assert not missing, f"declared in the header but not exported: {missing}"
     assert declared == set(N.SIGNATURES), declared ^ set(N.SIGNATURES)
-    assert N.lib().ctl_abi_version() == 4
+    assert N.lib().ctl_abi_version() == 5
 
 
 def test_no_cpu_fallback():

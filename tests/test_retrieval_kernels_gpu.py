@@ -430,7 +430,7 @@ def test_keys_and_topk_emit(N):
                            ovf.data_ptr(), N.stream_ptr()) == -1
 
 
-def test_eval_finalize_against_numpy(N):
+def test_eval_finalize_packed_against_numpy(N):
     """buckets[q, j] = kept gallery rows whose first LATER positive is positive j (positive j - 1 itself is one of them), so
     rank_j = buckets[q, :j + 1].sum() + 1 and AP = mean_j (j + 1) / rank_j (utils/eval_reid.py:75-79: the precision at
     every hit, averaged over the hits)."""
@@ -469,12 +469,13 @@ def test_eval_finalize_against_numpy(N):
         assert np.array_equal(p[nq], [float(flag or 0), 0.0, 0.0])
     ranks2 = torch.empty(nq, max_pos, dtype=torch.int32, device="cuda")
     ap2 = torch.empty(nq, dtype=torch.float64, device="cuda")
-    N.check(L.ctl_eval_finalize(bd.data_ptr(), cd.data_ptr(), nq, max_pos, ranks2.data_ptr(), ap2.data_ptr(), N.stream_ptr()))
+    N.check(L.ctl_eval_finalize_packed(bd.data_ptr(), cd.data_ptr(), nq, max_pos, ranks2.data_ptr(), ap2.data_ptr(), None,
+                                       None, N.stream_ptr()))
     assert torch.equal(ranks2, ranks) and np.array_equal(ap2.cpu().numpy(), ap.cpu().numpy(), equal_nan=True)
 
 
 def test_worklist_of_a_stride_without_identities(N):
-    """The form ctl_l2_topk uses for its threshold pass: no identities, every stride-th gallery tile."""
+    """The form the top-k's threshold pass uses (topk): no identities, every stride-th gallery tile."""
     L = N.lib()
     nq, ng, stride = 300, 5000, 7
     m_tiles, n_tiles = 3, 40
@@ -532,10 +533,11 @@ def _same_as_unsharded(base, idx, dst, res):
 
 
 @pytest.mark.parametrize("pid_sorted", [False, True])
-def test_sharded_protocol_on_one_device(R, N, sharded_problem, pid_sorted):
+def test_sharded_dist_pass_protocol_on_one_device(R, N, sharded_problem, pid_sorted):
     """collect per shard, gather + sort the keys, count per shard, sum the buckets, finalize (include/ctl_b200.h), and the
-    k-way merge of the shards' top-k lists: every shard writes GLOBAL gallery rows into its keys (g_index_offset, or
-    g_index_map = order + offset for a shard stored in identity order), so the result is the unsharded one bit for bit."""
+    merge of the shards' top-k lists by packed key: every shard writes GLOBAL gallery rows into its keys (g_index_offset,
+    or g_index_map = order + offset for a shard stored in identity order), so the result is the unsharded one bit for
+    bit."""
     q, gal, pids, cams, k, qp, base = sharded_problem
     L = N.lib()
     nq, ng, d = q.shape[0], gal.shape[0], q.shape[1]
@@ -559,7 +561,7 @@ def test_sharded_protocol_on_one_device(R, N, sharded_problem, pid_sorted):
             g_pid, g_mask = g_pid[o].contiguous(), g_mask[o].contiguous()
             gmap = (gp.order + start).to(torch.int32)
         shards.append((gp, g_pid, g_mask, gmap, start, n))
-        # top-k of the shard: ctl_l2_topk reports row + offset, so it takes the shard's planes in the caller's order
+        # top-k of the shard: topk() reports row + offset, so it takes the shard's planes in the caller's order
         i_s, d_s, ovf = R.topk(qp, R.build_planes(rows) if pid_sorted else gp, k, g_index_offset=start)
         assert int(ovf.item()) == 0
         idx_l.append(i_s)
@@ -567,15 +569,10 @@ def test_sharded_protocol_on_one_device(R, N, sharded_problem, pid_sorted):
         pos = torch.full((nq, mp_l), -1, dtype=torch.int64, device="cuda")
         cnt = torch.zeros(nq, dtype=torch.int32, device="cuda")
         ovf = torch.zeros(1, dtype=torch.int32, device="cuda")
-        if pid_sorted:
-            p1 = N.PassDesc(pos_keys=pos.data_ptr(), pos_count=cnt.data_ptr(), q_pid=ids.q_pid.data_ptr(),
-                            q_cam=ids.q_cam.data_ptr(), g_pid=g_pid.data_ptr(), g_cammask=g_mask.data_ptr(), max_pos=mp_l,
-                            overflow=ovf.data_ptr(), g_index_offset=start, g_index_map=gmap.data_ptr())
-            N.check(L.ctl_dist_pass(qp.ptr, nq, gp.ptr, n, d, qp.flags, C.byref(p1), s()))
-        else:
-            N.check(L.ctl_eval_collect(qp.ptr, nq, gp.ptr, n, d, qp.flags, ids.q_pid.data_ptr(), ids.q_cam.data_ptr(),
-                                       g_pid.data_ptr(), g_mask.data_ptr(), start, mp_l, pos.data_ptr(), cnt.data_ptr(),
-                                       ovf.data_ptr(), s()))
+        p1 = N.PassDesc(pos_keys=pos.data_ptr(), pos_count=cnt.data_ptr(), q_pid=ids.q_pid.data_ptr(),
+                        q_cam=ids.q_cam.data_ptr(), g_pid=g_pid.data_ptr(), g_cammask=g_mask.data_ptr(), max_pos=mp_l,
+                        overflow=ovf.data_ptr(), g_index_offset=start, g_index_map=N.ptr(gmap))
+        N.check(L.ctl_dist_pass(qp.ptr, nq, gp.ptr, n, d, qp.flags, C.byref(p1), s()))
         assert int(ovf.item()) == 0
         col = torch.arange(mp_l, device="cuda")[None, :]
         keys_l.append(torch.where(col < cnt[:, None], pos, torch.full_like(pos, -1)))  # unused slots: the largest key
@@ -587,20 +584,16 @@ def test_sharded_protocol_on_one_device(R, N, sharded_problem, pid_sorted):
     total = torch.zeros(nq, mp + 1, dtype=torch.int32, device="cuda")
     for gp, g_pid, g_mask, gmap, start, n in shards:
         buckets = torch.zeros(nq, mp + 1, dtype=torch.int32, device="cuda")
-        if pid_sorted:
-            p2 = N.PassDesc(thr_keys=thr.data_ptr(), thr_count=thr_count.data_ptr(), buckets=buckets.data_ptr(),
-                            q_pid=ids.q_pid.data_ptr(), q_cam=ids.q_cam.data_ptr(), g_pid=g_pid.data_ptr(),
-                            g_cammask=g_mask.data_ptr(), max_pos=mp, g_index_offset=start, g_index_map=gmap.data_ptr())
-            N.check(L.ctl_dist_pass(qp.ptr, nq, gp.ptr, n, d, qp.flags, C.byref(p2), s()))
-        else:
-            N.check(L.ctl_eval_count(qp.ptr, nq, gp.ptr, n, d, qp.flags, ids.q_pid.data_ptr(), ids.q_cam.data_ptr(),
-                                     g_pid.data_ptr(), g_mask.data_ptr(), start, mp, thr.data_ptr(), thr_count.data_ptr(),
-                                     buckets.data_ptr(), s()))
+        p2 = N.PassDesc(thr_keys=thr.data_ptr(), thr_count=thr_count.data_ptr(), buckets=buckets.data_ptr(),
+                        q_pid=ids.q_pid.data_ptr(), q_cam=ids.q_cam.data_ptr(), g_pid=g_pid.data_ptr(),
+                        g_cammask=g_mask.data_ptr(), max_pos=mp, g_index_offset=start, g_index_map=N.ptr(gmap))
+        N.check(L.ctl_dist_pass(qp.ptr, nq, gp.ptr, n, d, qp.flags, C.byref(p2), s()))
         total += buckets
     ranks = torch.empty(nq, mp, dtype=torch.int32, device="cuda")
     ap = torch.empty(nq, dtype=torch.float64, device="cuda")
-    N.check(L.ctl_eval_finalize(total.data_ptr(), thr_count.data_ptr(), nq, mp, ranks.data_ptr(), ap.data_ptr(), s()))
-    idx, dst = R.merge_topk(idx_l, dst_l, k)
+    N.check(L.ctl_eval_finalize_packed(total.data_ptr(), thr_count.data_ptr(), nq, mp, ranks.data_ptr(), ap.data_ptr(),
+                                       None, None, s()))
+    idx, dst = R.merge_topk_keys(R.pack_keys(torch.cat(dst_l, 1), torch.cat(idx_l, 1)), k)
     _same_as_unsharded(base, idx, dst, R._aggregate(ranks.cpu().numpy(), ap.cpu().numpy(), thr_count.cpu().numpy(),
                                                     pids[:nq], ng, 50))
 
@@ -633,8 +626,26 @@ def test_sharded_streamed_passes_under_a_stand_in_exchange(R, sharded_problem, w
             _same_as_unsharded(base, None, None, out[0])
 
 
+@pytest.mark.parametrize("world", [2, 3])
+def test_sharded_topk_only_under_a_stand_in_exchange(R, sharded_problem, world):
+    """retrieval._streamed without identities -- the code of topk_sharded -- with W ranks emulated on one device, with
+    the threshold from a subset of each shard and from every tile: every rank's k best keys, merged by key order, are
+    the unsharded top-k bit for bit."""
+    q, gal, pids, cams, k, qp, base = sharded_problem
+    ng = gal.shape[0]
+    cuts = {2: (0, 4270, ng), 3: tuple(np.concatenate([[0], np.cumsum(SHARDS)]))}[world]
+    for subset in (True, False):
+        def rank(ex):
+            lo, hi = int(cuts[ex.rank]), int(cuts[ex.rank + 1])
+            return R._streamed(ex, qp, R.build_planes(gal[lo:hi]), None, k, None, hi - lo, 0, lo, tile_lists=subset)
+
+        for idx, dst in Shards(world).run(rank):
+            assert torch.equal(idx, base[0]) and torch.equal(dst, base[1])
+
+
 def test_topk_and_eval_sharded_in_a_group_of_one(R, sharded_problem, tmp_path):
-    """retrieval.topk_and_eval_sharded itself, in a process group of one rank (a file store, no network)."""
+    """retrieval.topk_and_eval_sharded and topk_sharded (group=None: the default group) themselves, in a process group of
+    one rank (a file store, no network)."""
     import datetime
 
     import torch.distributed as dist
@@ -660,5 +671,7 @@ def test_topk_and_eval_sharded_in_a_group_of_one(R, sharded_problem, tmp_path):
             assert np.array_equal(res.cmc, base[2].cmc) and res.mAP == base[2].mAP
             assert np.array_equal(res.ranks, base[2].ranks)
             assert np.array_equal(res.single_performance, base[2].single_performance)
+        idx, dst = R.topk_sharded(q, gal, k, 0, None)
+        assert torch.equal(idx, base[0]) and torch.equal(dst, base[1])
     finally:
         dist.destroy_process_group()
