@@ -191,6 +191,9 @@ SIGNATURES = {
     "ctl_jpeg_parse": (C.c_int, [_p, _i64, C.POINTER(JpegDesc), C.POINTER(_i32), C.POINTER(_i32)]),
     "ctl_jpeg_decode_workspace_bytes": (_sz, [_p, _i64]),
     "ctl_jpeg_decode": (C.c_int, [_p, _i64, _p, _i64, _p, _p, _i64, _p, _p, _sz, _p]),
+    "ctl_resize_linear_cv_u8": (C.c_int, [_p, _i64, _p, _i64, _i32, _i32, _p, _p, _p]),
+    "ctl_visrank_compose": (C.c_int, [_p, _i64, _i32, _i32, _p, _i64, _i64, _i32, _p, _p, _p]),
+    "ctl_visrank_select": (C.c_int, [_p, _i64, _i32, _p, _p, _p, _p, _i64, _i32, _p, _p, _p, _p]),
     "ctl_adam_multi_step": (C.c_int, [_p, _i32, C.c_int64, _f, _f, _f, _f, _f, C.c_int64, _f, _p, _p]),
     "ctl_sgd_step": (C.c_int, [_p, _p, C.c_int64, _f, _f, _p, _p]),
     "ctl_loss_scale_update": (C.c_int, [_p, _p, _p, _p, _f, _f, _f, _i32, _p]),

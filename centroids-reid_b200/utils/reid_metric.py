@@ -8,6 +8,8 @@ streamed evaluation (retrieval.evaluate_streamed).
 """
 from __future__ import annotations
 
+import os
+
 import numpy as np
 import torch
 
@@ -63,6 +65,9 @@ class R1_mAP:
         self.hparms = pl_module.hparams
         self.dist_name = self.hparms.SOLVER.DISTANCE_FUNC
         self.dist_func = get_dist_func(self.dist_name)
+        self.dataset = None
+        if getattr(self.hparms.TEST, "VISUALIZE", "no") == "yes":
+            self.dataset = _eval_samples(trainer)
 
     def compute(self, feats, pids, camids, respect_camids=False):
         if self.feat_norm:
@@ -72,8 +77,6 @@ class R1_mAP:
         q_pids = np.asarray(pids[:nq])
         g_pids = np.asarray(pids[nq:])
         q_camids, g_camids = camids[:nq], camids[nq:]
-        if getattr(self.hparms.TEST, "VISUALIZE", "no") == "yes":
-            raise NotImplementedError("ranked-result visualisation (utils/visrank.py) is outside the H100 hot path")
         # reid_metric.py:113-136: F.normalize -> dist -> argsort -> eval_func(.., 50, ..), fused.
         # (the reference hard-codes max_rank=50 in the eval_func call, :134-136)
         # both operands are stored in identity order: the collect pass then skips every tile that cannot hold a positive
@@ -84,4 +87,23 @@ class R1_mAP:
         gp = _R.build_planes(feats[nq:], self.dist_name, self.feat_norm, order=go)
         res = _R.evaluate_streamed(qp, gp, q_pids, g_pids, q_camids, g_camids, 50, respect_camids)
         self.last_result = res
+        hp = self.hparms
+        if getattr(hp.TEST, "VISUALIZE", "no") == "yes":  # reid_metric.py:138-149, from the planes: no distmat
+            from .visrank import visualize_ranked_planes
+
+            print("Start visualization...")
+            visualize_ranked_planes(qp, gp, self.dataset, hp, width=hp.INPUT.SIZE_TEST[1], height=hp.INPUT.SIZE_TEST[0],
+                                    save_dir=os.path.join(hp.OUTPUT_DIR, "visrank"), topk=hp.TEST.VISUALIZE_TOPK)
         return res.cmc, res.mAP, res.all_topk
+
+
+def _eval_samples(trainer):
+    """reid_metric.py:87-90: the (path, pid, camid, index) samples of the validation (else the test) loader, which
+    TEST.VISUALIZE needs for the image files."""
+    for attr in ("val_dataloaders", "test_dataloaders"):
+        try:
+            return getattr(trainer, attr)[0].dataset.samples
+        except (AttributeError, IndexError, KeyError, TypeError):
+            continue
+    raise ValueError("TEST.VISUALIZE = 'yes' needs the image paths: pl_module.trainer.val_dataloaders[0] (or "
+                     "test_dataloaders[0]) must have a dataset with `samples`")

@@ -771,6 +771,46 @@ int ctl_jpeg_decode(const void* src, int64_t src_bytes, const void* entries_devi
                     const void* out_table_device, void* out_u8, int64_t out_bytes, int32_t* status, void* workspace,
                     size_t workspace_bytes, ctl_stream_t stream);
 
+/* ---- Ranked-result grids: visualize_ranked_results (utils/visrank.py:23-244) ----
+ * The reference reads each image with cv2.imread (the same pixels as Pillow's decode, in BGR order; the calls below
+ * work in RGB), then per grid cell runs cv2.resize(img, (w, h)), cv2.copyMakeBorder(3 px, colour), cv2.resize(.., (w, h))
+ * (visrank.py:168-174, 206-211) and pastes the cell into a white grid (visrank.py:176-184, 212-220).
+ *
+ * ctl_resize_linear_cv_u8: cv2.resize(img, (out_w, out_h)) with INTER_LINEAR on HWC uint8 3-channel images, bit for
+ * bit.  Per axis (`in` -> `out` pixels, o the output index): f = (float)((o + 0.5) * (in / out) - 0.5) in double,
+ * s = floor(f), f -= s in float, a0 = rint((float)(1 - f) * 2048) (half to even), a1 = 2048 - a0.  Along x the weights
+ * are clamped (s < 0: s = 0, f = 0; s >= in - 1: s = in - 1, f = 0); along y they are not, and the two source rows are
+ * clamped to [0, in - 1].  Per channel: hrow(y) = S[y][s] a0 + S[y][min(s + 1, in - 1)] a1,
+ * out = min((((b0 (hrow(y0) >> 4)) >> 16) + ((b1 (hrow(y1) >> 4)) >> 16) + 2) >> 2, 255).
+ * src / table_device: the ragged batch of ctl_resize_bilinear_u8 (struct ctl_resize_entry).  out_u8_nhwc: uint8
+ * [n][out_h][out_w][3].  status: int32 [n] on the device, written for every entry: 0, or 1 for an entry whose bytes
+ * do not fit in src_bytes (or with a negative or > 2^24 side); such an entry and a mock row (h or w == 0) give zeros.
+ * One launch, no workspace, no host synchronisation: capturable in a CUDA graph.  A null pointer, n < 1 or an output
+ * side outside 1..16384 is CTL_ERR_INVALID_ARGUMENT before any device work.
+ *
+ * ctl_visrank_compose: the grids uint8 [n_grids][h][Wg][3], Wg = (topk + 1) w + 2 topk + 8, from the images of
+ * ctl_resize_linear_cv_u8 (resized_u8: uint8 [n_rows][h][w][3]).  cells_device: int32 [n_cells][4] = {row of
+ * resized_u8, grid, column, border colour 0xRRGGBB}.  Every grid is first filled with 255; the cell of column c is
+ * cv2.resize(copyMakeBorder(row, 3, 3, 3, 3, colour), (w, h)), computed without an intermediate, at x = 0 for c = 0
+ * (the query) and x = c w + 2 c + 8 otherwise.  A cell with a row, grid or column (0..topk) out of range is skipped
+ * and sets *status (zeroed by the call) to 1.  No host synchronisation: capturable in a CUDA graph.
+ *
+ * ctl_visrank_select: the ranked list of visrank.py:192-232.  topk_idx: int64 [nq][k], each query's k nearest
+ * gallery rows in ascending (distance, index) order; identities as in struct ctl_pass_desc: q_pid, q_cam int32 [nq];
+ * g_pid int32 [ng]; g_cammask uint64 [ng].  A row is junk when g_pid == q_pid and bit q_cam of g_cammask is set
+ * (same pid and camera, or with camera sets the query's camera is in the centroid's set, visrank.py:196-200).
+ * Writes the first topk non-junk rows of each query to out_idx int64 [nq][topk] and out_matched int8 [nq][topk]
+ * (1 when g_pid == q_pid), padded with -1 / 0 when fewer remain.  k must cover topk plus the query's junk rows for the
+ * list to be complete.  An index outside [0, ng) stops that query and sets *status (zeroed by the call) to 1. */
+int ctl_resize_linear_cv_u8(const void* src, int64_t src_bytes, const void* table_device, int64_t n, int32_t out_h,
+                            int32_t out_w, void* out_u8_nhwc, int32_t* status, ctl_stream_t stream);
+int ctl_visrank_compose(const void* resized_u8, int64_t n_rows, int32_t h, int32_t w, const int32_t* cells_device,
+                        int64_t n_cells, int64_t n_grids, int32_t topk, void* out_u8, int32_t* status,
+                        ctl_stream_t stream);
+int ctl_visrank_select(const int64_t* topk_idx, int64_t nq, int32_t k, const int32_t* q_pid, const int32_t* q_cam,
+                       const int32_t* g_pid, const uint64_t* g_cammask, int64_t ng, int32_t topk, int64_t* out_idx,
+                       int8_t* out_matched, int32_t* status, ctl_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
